@@ -8,8 +8,13 @@ unordered pair evaluated once) -> CSR -> greedy Butina loop -> cluster ids. `val
 fingerprints resident in HBM; `e2e` = the same through the public API with HOST buffers (pinned H2D of the fingerprints
 and D2H of the ids inside the timed region).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload butina|etkdg_mmff]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload all|butina|conformers]
+                    [--dump-outputs DIR]
     torchrun --nproc-per-node N bench.py --gpus N ...     (one rank per GPU; rank 0 prints the JSON line)
+
+--dump-outputs DIR writes what the timed path returned in its last timed step as DIR/<name>.npy (float64; at most
+64 MB in all, larger arrays as a fixed seeded row sample), so that two builds can be compared output for output: the
+inputs depend only on the arguments.
 """
 
 from __future__ import annotations
@@ -33,17 +38,13 @@ METRIC_NAME = "tanimoto_pairs_per_s"
 UNIT = "pairs/s"
 
 
-def fp4_possible(words: int) -> bool:
-    return (words * 32) % 256 == 0  # the library's eligibility rule for the fp4 count tile (tanimoto_tc.cu)
-
-
 def unique_pairs(n: int) -> float:
     return n * (n - 1) / 2.0
 
 
 # ----------------------------------------------------------------------------------------------- helpers
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -97,7 +98,7 @@ def measured_peaks() -> tuple[float, str]:
             return float(json.load(open(p))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (of measured)"
         except Exception:
             pass
-    return 6650.0, "B200_PROFILING.md fallback 6.65 TB/s (of fallback)"
+    return 3350.0, "H100 SXM data sheet 3.35 TB/s (not measured)"
 
 
 # ----------------------------------------------------------------------------------------------- reference arm
@@ -153,7 +154,26 @@ def run_reference(args) -> None:
     }))
 
 
-# ----------------------------------------------------------------------------------------------- B200 arm
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(directory: str, arrays: dict) -> None:
+    """Write each array as <directory>/<name>.npy in float64. Arrays over their share of the 64 MB budget are reduced
+    to a fixed, seeded sample of rows (the sampled row indices go beside them as <name>_rows.npy)."""
+    os.makedirs(directory, exist_ok=True)
+    share = DUMP_LIMIT_BYTES // max(1, len(arrays)) - 4096  # (room for the .npy headers)
+    for name, a in arrays.items():
+        a = np.asarray(a, dtype=np.float64)
+        row_bytes = 8 * max(1, a[0].size if a.ndim > 1 and len(a) else 1)
+        if a.nbytes > share:
+            keep = max(1, share // (2 * row_bytes))  # half for the values, the other half for the row indices
+            rows = np.sort(np.random.default_rng(0).choice(len(a), size=min(keep, len(a)), replace=False))
+            np.save(os.path.join(directory, f"{name}_rows.npy"), rows.astype(np.float64))
+            a = a[rows]
+        np.save(os.path.join(directory, f"{name}.npy"), a)
+
+
+# ----------------------------------------------------------------------------------------------- GPU arm
 def run_b200(args) -> None:
     import torch
     import torch.distributed as dist
@@ -166,7 +186,7 @@ def run_b200(args) -> None:
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a B200: nvmolkit_b200 has no CPU fallback")
+        raise SystemExit("bench.py needs an H100: nvmolkit_b200 has no CPU fallback")
     # the conformer pool is generated first: its worker processes are forked before this process touches CUDA / NCCL
     pool = None
     if args.workload in ("all", "conformers") and args.etkdg_mols > 0:
@@ -192,9 +212,12 @@ def run_b200(args) -> None:
         _lib.set_option("similarity_pipeline_chunks", args.pipeline_chunks)
     if args.superpose_auto >= 0:
         _lib.set_option("similarity_superpose_auto", args.superpose_auto)
+    dumped = {}
     if args.workload == "conformers":
-        legs = run_conformer_legs(args, pool, dev, world, rank)
+        legs = run_conformer_legs(args, pool, dev, world, rank, dumped)
         if rank == 0:
+            if args.dump_outputs:
+                dump_outputs(args.dump_outputs, dumped)
             line = dict(legs["etkdg_mmff"])
             line.update({"steps": 1, "warmup": 1, "higher_is_better": True, "vs_baseline": None, "data": "synthetic",
                          "config4_mmff": legs.get("config4_mmff"), "config5_etkdg_mmff": legs.get("config5_etkdg_mmff"),
@@ -252,6 +275,7 @@ def run_b200(args) -> None:
     with ClockSampler(local) as clocks:
         ms_dev, (ids, cen) = timed(lambda: step_device(d_fp), args.steps)
         launches = _lib.launch_count() - launches0
+        dumped["butina_cluster_ids"], dumped["butina_centroids"] = ids.cpu().numpy(), cen.cpu().numpy()
         # dominant kernel alone (CUDA events on its own stream, recorded inside the library around the tile kernel)
         pass_ms = []
         tensor_path = True
@@ -270,8 +294,7 @@ def run_b200(args) -> None:
         if tensor_path:
             phases["neighbor_pass_tc"] = _lib.profile_read("neighbor_pass_tc")
     # end to end after the clock sampler has stopped (nvidia-smi queries take the driver for a while; this loop is host-driven:
-    # a pinned 256 MB copy, the call, a 4 MB copy back). Its time depends on the box's host link: 59-70 ms per step on most
-    # boxes of the pool, 115 ms on some (profiles/r02_path_a_summary.md)
+    # a pinned 256 MB copy, the call, a 4 MB copy back). Its time depends on the machine's host link
     step_e2e()
     ms_e2e, _ = timed(step_e2e, args.steps)
 
@@ -319,7 +342,9 @@ def run_b200(args) -> None:
                                         "algorithmic_GBps": (8.0e6 + 256.0 * 2000) / (ms1 * 1e-3) / 1e9}
 
     # second half of the BASELINE metric: ETKDG + MMFF mols/s on config 3 (and configs 4 / 5 on eight GPUs)
-    legs = run_conformer_legs(args, pool, dev, world, rank) if pool is not None else {}
+    legs = run_conformer_legs(args, pool, dev, world, rank, dumped) if pool is not None else {}
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, dumped)
 
     ids_h = ids.cpu().numpy()
     n_clusters = int(cen.numel())
@@ -339,48 +364,45 @@ def run_b200(args) -> None:
     n_edges = None
     algo_bytes = 256.0 * n + 4.0 * n  # fingerprints read once + counts written (SURVEY.md §8d "fused count" pass)
     achieved = algo_bytes / (kernel_ms * 1e-3) / 1e9
-    # integer-issue roof of the same kernel: 64 POPC per pair at 16 lanes/clk/SM (148 SMs, measured max clock)
+    # integer-issue roof of the same kernel: 64 POPC per pair at 16 lanes/clk/SM (SM count of the device, max SM clock
+    # sampled during the run; 1,980 MHz, the H100 SXM boost clock, when nvidia-smi gave none)
     pairs_per_rank = unique_pairs(n) / world
     popc_rate = pairs_per_rank * words / (kernel_ms * 1e-3)
+    clock_summary = clocks.summary()
+    sm_mhz = clock_summary.get("sm_max_mhz") or 1980.0
+    popc_peak = torch.cuda.get_device_properties(dev).multi_processor_count * 16 * sm_mhz * 1e6
 
     if tensor_path:
-        # dominant kernel = tcgen05 block-scaled fp4 MMA tile (kind::mxf4 over the 0/1 E2M1 expansion, unit scale
-        # factors): 2 * bits ops per pair over the tiles actually visited (upper triangle). Dense fp4 issues at 4x the
-        # bf16 rate on B200 (9 vs 2.25 PFLOP/s nominal), so the roof is 4 x the MEASURED bf16 throughput.
-        bf16 = 1700.1
-        try:
-            bf16 = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["bf16_tflops"])
-        except Exception:
-            pass
-        fp4 = (words * 32) % 256 == 0  # the library's own eligibility rule (tanimoto_tc.cu); else the int8 tile runs
-        mult = 4.0 if fp4 else 2.0
+        # dominant kernel = the wgmma u8 tile over the 0/1 byte expansion: 2 * bits ops per pair over the tiles actually
+        # visited (upper triangle). Roof: the H100 SXM data sheet's dense INT8 rate (1,979 TOPS at 700 W; not reached
+        # by a card with a lower power limit, see "clocks").
+        peak_tops = 1979.0
         tiles_pairs = unique_pairs(n) / world  # + diagonal-tile overhead (< 0.1 % at 1M)
         # superposition: one tensor-core row (column) carries the sum of S (C) fingerprints, so the pass ISSUES 1/(S C) of
         # the pair-by-pair contraction (the survivors' exact re-count is the separate verify kernel, in phases_ms);
         # superS below = S * C = pairs bounded by one accumulator
-        superS = max(1, _lib.get_option("similarity_superpose_last")) if fp4_possible(words) else 1
+        superS = max(1, _lib.get_option("similarity_superpose_last"))
         tops = tiles_pairs / superS * 2.0 * words * 32 / (kernel_ms * 1e-3) / 1e12
-        operand_bytes = ((128 + 112) * (words * 32 // 2) / (128.0 * superS * 224.0) if fp4
-                         else (128 + 256) * (words * 32) / (128.0 * 256.0))
-        roofline = {"bound": "tensor", "achieved": tops, "peak": mult * bf16, "unit": "TFLOP/s", "frac": tops / (mult * bf16),
-                    "traffic": measured_traffic().get("simTensorKernel<count>") if n == 1_000_000 and world == 1 else None,
-                    "kernel": ("simTensorKernel<count, fp4, cluster2> (tcgen05.mma kind::mxf4.block_scale, neighbor_pass_tc)" if fp4
-                               else "simTensorKernel<count> (tcgen05.mma kind::i8, neighbor_pass_tc)"),
+        # bytes from L2 into shared memory per pair: a 128-row tile and half of the 256-column tile (the other half comes
+        # by multicast to the CTA pair), one byte per bit
+        operand_bytes = (128 + 128) * (words * 32) / (128.0 * 256.0 * superS)
+        roofline = {"bound": "tensor", "achieved": tops, "peak": peak_tops, "unit": "TOP/s", "frac": tops / peak_tops,
+                    "kernel": "simTensorKernel<count, cluster> (wgmma.mma_async m64n256k32 u8, neighbor_pass_tc)",
                     "kernel_ms": kernel_ms, "ops_per_pair": 2 * words * 32 / superS, "pairs_per_accumulator": superS,
                     "candidates_verified": _lib.get_option("similarity_candidates_last") if superS > 1 else 0,
                     "unsuperposed_equivalent_TOPs": tops * superS,
-                    "peak_source": f"{mult:.0f} x MEASURED_PEAKS.json bf16_tflops (dense {'fp4' if fp4 else 'u8'} = {mult:.0f} x bf16 rate; of measured)",
-                    "hbm_algorithmic_GBps": (n * words * 32 / (2 if fp4 else 1) + 260.0 * n) / (kernel_ms * 1e-3) / 1e9,
+                    "peak_source": "H100 SXM data sheet, dense INT8 (not measured)",
+                    "hbm_algorithmic_GBps": (n * words * 32 + 260.0 * n) / (kernel_ms * 1e-3) / 1e9,
                     "l2_operand_bytes_per_pair": operand_bytes,
                     "l2_operand_TBps": tiles_pairs * operand_bytes / (kernel_ms * 1e-3) / 1e12,
-                    "note": "exact: 0/1 products, fp32 accumulation of sums <= 4096; HBM share negligible, the operand "
-                            "stream comes from L2 (TMA, column operand multicast to the CTA pair)"}
+                    "note": "exact: 0/1 products, s32 accumulation; HBM share negligible, the operand stream comes "
+                            "from L2 (TMA, column operand multicast to the CTA pair)"}
     else:
         roofline = None
     out = {
         "metric": METRIC_NAME, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps,
         "warmup": args.warmup, "ms_per_step": ms_dev, "higher_is_better": True, "scaling": "strong",
-        "vs_baseline": None, "dtype": "e2m1 0/1 x e2m1 0/1 -> f32 (exact integer counts), integer threshold test = the f64 predicate", "data": "synthetic",
+        "vs_baseline": None, "dtype": "u8 0/1 x u8 0/1 -> s32 (exact integer counts), integer threshold test = the f64 predicate", "data": "synthetic",
         "config": {"workload": "1Mx1M symmetric 2048-bit Tanimoto + Butina (sim>=0.7)" if n == 1_000_000 else
                    f"{n}x{n} symmetric 2048-bit Tanimoto + Butina (sim>=0.7) [reduced size override]",
                    "n_fingerprints": n, "fp_bits": words * 32, "cutoff": CUTOFF, "pairs_counted": "unique n(n-1)/2",
@@ -390,13 +412,13 @@ def run_b200(args) -> None:
                 "h2d": ("whole job: every rank copies 1/world of the rows from pinned host memory, the slices are all-gathered "
                         "over NVLink (distributed.sharded_upload)") if world > 1 else "pinned host -> device, whole array"},
         "gpu_launches": int(launches),
-        "clocks": clocks.summary(),
+        "clocks": clock_summary,
         "roofline": roofline if roofline is not None else {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": None, "kernel": "simTileKernel<count> (neighbor_pass)", "kernel_ms": kernel_ms,
+                     "kernel": "simTileKernel<count> (neighbor_pass)", "kernel_ms": kernel_ms,
                      "algorithmic_bytes": algo_bytes, "peak_source": peak_src,
                      "note": "pass is integer-issue bound by construction (5e-4 B/pair); see popc_roof"},
-        "popc_roof": {"achieved_popc_per_s": popc_rate, "peak_popc_per_s": 148 * 16 * 1.965e9,
-                      "frac": popc_rate / (148 * 16 * 1.965e9), "unit": "32-bit POPC/s"},
+        "popc_roof": {"achieved_popc_per_s": popc_rate, "peak_popc_per_s": popc_peak,
+                      "frac": popc_rate / popc_peak, "unit": "32-bit POPC/s"},
         "phases_ms": phases, "n_clusters": n_clusters,
     }
 
@@ -528,7 +550,7 @@ def _event_timed(fn, dev, world):
     return float(ms.item()), out
 
 
-def _conformer_roofline(stats, phases, peak, peak_src, traffic):
+def _conformer_roofline(stats, phases, peak, peak_src):
     """HBM roofline of the two kernels of the path from the device-side work counters: ALGORITHMIC bytes by SURVEY.md
     8d's (the reference's) scheme - per BFGS iteration 3 n^2 x 8 B of inverse Hessian + (1 + k_ls) x term bytes, summed
     over the iterations the kernel actually ran - divided by the kernel's CUDA-event duration."""
@@ -547,25 +569,16 @@ def _conformer_roofline(stats, phases, peak, peak_src, traffic):
                      "note": "achieved = the reference scheme's bytes (SURVEY.md 8d: 3 n^2 x 8 B + term records per iteration) / "
                              "time, so frac > 1 means: faster than that scheme could run at the HBM roof; own_scheme_* = the bytes "
                              "this kernel's one-sweep triangular update needs",
-                     "traffic": traffic.get(kernel), "kernel": kernel, "kernel_ms": ms,
+                     "kernel": kernel, "kernel_ms": ms,
                      "algorithmic_bytes": st["algorithmic_bytes"], "bfgs_iterations": st["bfgs_iterations"],
                      "energy_evals": st["energy_evals"], "gradient_evals": st["gradient_evals"],
                      "minimisations": st["minimisations"], "peak_source": peak_src}
     return out
 
 
-def measured_traffic() -> dict:
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernels, from the committed ncu --set full
-    captures of this same command (profiles/traffic.json: {kernel: {"bytes": ..., "source": ...}})."""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    try:
-        return {k: v["bytes"] for k, v in json.load(open(p)).items()}
-    except Exception:
-        return {}
-
-
-def run_conformer_legs(args, pool, dev, world, rank):
-    """Configs 3 (always), 4 and 5 (8 GPUs, or --all-configs) of BASELINE.json. Returns the dict for the JSON line."""
+def run_conformer_legs(args, pool, dev, world, rank, dumped):
+    """Configs 3 (always), 4 and 5 (8 GPUs, or --all-configs) of BASELINE.json. Returns the dict for the JSON line and
+    puts config 3's results (energies, convergence status, coordinates) into `dumped`."""
     import torch
 
     from nvmolkit_b200 import _lib
@@ -574,7 +587,6 @@ def run_conformer_legs(args, pool, dev, world, rank):
     n_pool = len(flat)
     leg = ConformerLeg(flat, mmff, dev, world, rank)
     peak, peak_src = measured_peaks()
-    traffic = measured_traffic()
     atom_offs = np.concatenate([[0], np.cumsum(flat.atom_counts)]).astype(np.int64)
     out = {}
 
@@ -587,6 +599,10 @@ def run_conformer_legs(args, pool, dev, world, rank):
     l0 = _lib.launch_count()
     ms, (raw, res) = _event_timed(lambda: leg.step(ids3, args.confs), dev, world)
     launches = _lib.launch_count() - l0
+    dumped["etkdg_embedded"] = raw.ok.cpu().numpy()
+    dumped["etkdg_mmff_energies"] = res.energies.cpu().numpy()
+    dumped["etkdg_mmff_status"] = res.status.cpu().numpy()
+    dumped["etkdg_mmff_positions"] = res.positions.reshape(-1, 3).cpu().numpy()
     stats = _lib.stats_read(reset=True)
     phases = {"etkdg": _lib.profile_read("etkdg"), "bfgs": _lib.profile_read("bfgs")}
     ok = raw.ok.cpu().numpy().astype(bool)
@@ -610,8 +626,7 @@ def run_conformer_legs(args, pool, dev, world, rank):
 
     ms_e2e, _ = _event_timed(e2e_step, dev, world)
     h2d = flat.nbytes() + mmff.nbytes()
-    # (the ncu traffic capture is of THIS workload at its default size on one GPU: not quoted for anything else)
-    roof = _conformer_roofline(stats, phases, peak, peak_src, traffic if (n3 == 10000 and args.confs == 10 and world == 1) else {})
+    roof = _conformer_roofline(stats, phases, peak, peak_src)
     out["etkdg_mmff"] = {
         "metric": "etkdg_mmff_mols_per_s", "value": n3 / (ms * 1e-3), "unit": "mols/s", "ms_per_step": ms, "n_gpus": world,
         "scaling": "strong",
@@ -659,7 +674,7 @@ def run_conformer_legs(args, pool, dev, world, rank):
         _lib.stats_read(reset=True)
         ms4, (_r4, res4) = _event_timed(lambda: leg.step(ids4, 1, embed=False, start_xyz=(atom_offs, xyz4)), dev, world)
         st4 = _lib.stats_read(reset=True)
-        roof4 = _conformer_roofline(st4, {"bfgs": _lib.profile_read("bfgs")}, peak, peak_src, {})
+        roof4 = _conformer_roofline(st4, {"bfgs": _lib.profile_read("bfgs")}, peak, peak_src)
         out["config4_mmff"] = {
             "metric": "mmff_mols_per_s", "value": n4 / (ms4 * 1e-3), "unit": "mols/s", "ms_per_step": ms4, "n_gpus": world,
             "config": {"workload": f"config 4: {n4} mols ({min(n4, n_pool)} distinct) MMFF94 200-iteration BFGS from pre-embedded "
@@ -670,7 +685,7 @@ def run_conformer_legs(args, pool, dev, world, rank):
         _lib.stats_read(reset=True)
         ms5, (raw5, res5) = _event_timed(lambda: leg.step(ids5, 1), dev, world)
         st5 = _lib.stats_read(reset=True)
-        roof5 = _conformer_roofline(st5, {"etkdg": _lib.profile_read("etkdg"), "bfgs": _lib.profile_read("bfgs")}, peak, peak_src, {})
+        roof5 = _conformer_roofline(st5, {"etkdg": _lib.profile_read("etkdg"), "bfgs": _lib.profile_read("bfgs")}, peak, peak_src)
         out["config5_etkdg_mmff"] = {
             "metric": "etkdg_mmff_mols_per_s", "value": n5 / (ms5 * 1e-3), "unit": "mols/s", "ms_per_step": ms5, "n_gpus": world,
             "config": {"workload": f"config 5: {n5} mols ({min(n5, n_pool)} distinct, config 3 generator cycled) x 1 conformer, ETKDG "
@@ -742,6 +757,8 @@ def main() -> None:
     ap.add_argument("--all-configs", action="store_true", help="run configs 4 and 5 on fewer than 8 GPUs too")
     ap.add_argument("--mmff-mols", type=int, default=100000, help="config 4 size")
     ap.add_argument("--e2e-mols", type=int, default=1000000, help="config 5 size")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the timed path's outputs of its last timed step to DIR/<name>.npy (float64, <= 64 MB)")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3

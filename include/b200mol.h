@@ -1,5 +1,5 @@
 /*
- * b200mol.h — C-ABI of libb200mol.so, the B200 (sm_100a) batched-molecule hot path.
+ * b200mol.h — C-ABI of libb200mol.so, the H100 (sm_90a) batched-molecule hot path.
  *
  * Every entry point is `extern "C"`, takes plain pointers + sizes + an opaque stream
  * (a cudaStream_t passed as void*), returns an int status (0 = OK) and never throws.
@@ -26,7 +26,7 @@ extern "C" {
 #define B200MOL_OK 0
 #define B200MOL_ERR_INVALID 1 /* bad argument (maps to ValueError / std::invalid_argument) */
 #define B200MOL_ERR_CUDA 2    /* CUDA runtime failure (maps to RuntimeError / CudaBadReturnCode) */
-#define B200MOL_ERR_NODEVICE 3 /* no sm_100 device visible: the product path has no CPU fallback */
+#define B200MOL_ERR_NODEVICE 3 /* no sm_90 device visible: the product path has no CPU fallback */
 
 #define B200MOL_METRIC_TANIMOTO 0
 #define B200MOL_METRIC_COSINE 1
@@ -36,21 +36,20 @@ const char* b200mol_last_error(void);
 int b200mol_abi_version(void);
 /* Number of kernel launches issued by this library in this process (bench.py's gpu_launches). */
 uint64_t b200mol_launch_count(void);
-/* 0 when device `dev` is compute capability 10.x; B200MOL_ERR_NODEVICE otherwise. */
+/* 0 when device `dev` is compute capability 9.0; B200MOL_ERR_NODEVICE otherwise. */
 int b200mol_check_device(int dev);
 int b200mol_free_async(void* d_ptr, void* stream);
 /* Tuning knobs (every setting computes the same results; tests/ run the variants against each other and the oracle):
- *   "similarity_tensor_min_pairs"  pair count (nX * nY) from which the similarity passes run on the tcgen05 tensor-core
- *                                  tile instead of the SIMT popcount tile (default 2^24; 0 = always, < 0 = never)
- *   "similarity_tensor_fp4"        1 (default): the thresholded count pass feeds the tensor cores block-scaled fp4
- *                                  operands (kind::mxf4, fingerprints of a multiple of 256 bits); 0: the int8 tile
- *   "similarity_tensor_cluster"    1 (default): that tile runs in clusters of two CTAs sharing the column operand
- *                                  through TMA multicast; 2: CTA pairs with tcgen05 cta_group::2 MMAs (M = 256, each
- *                                  CTA stages half of the column operand); 3: CTA pairs with the multicast column operand
- *                                  and the ROW operand stationary in shared memory for a run of 16 tile columns
- *                                  (fingerprints up to 2048 bits; half the L2 -> SM bytes per pair); 0: one CTA per tile
+ *   "similarity_tensor_min_pairs"  pair count (nX * nY) from which the similarity passes run on the wgmma tensor-core
+ *                                  tile (u8 0/1 operands) instead of the SIMT popcount tile (default 2^24; 0 = always,
+ *                                  < 0 = never)
+ *   "similarity_tensor_cluster"    1 (default): the thresholded count pass runs in clusters of two CTAs sharing the
+ *                                  column operand through TMA multicast; 3: the same pairs with the ROW operand
+ *                                  stationary in shared memory for a run of 16 tile columns (fingerprints up to 1024
+ *                                  bits, else as 1; half the L2 -> shared memory bytes per pair); 0: one CTA per tile;
+ *                                  2: runs as 1 (kept for callers written for a CTA-pair MMA, which Hopper lacks)
  *   "similarity_superpose"         4 (default), 2 or 1: fingerprints summed into one row operand of the Butina neighbour pass
- *                                  (values 0..4 are exact in fp4): one accumulator then bounds that many pair counts, the
+ *                                  (byte values 0..4): one accumulator then bounds that many pair counts, the
  *                                  few survivors are re-examined exactly by a second kernel; 1 = off
  *   "similarity_superpose_cols"    4 (default), 2 or 1: the same for the column operand (sums of products stay <= 16,
  *                                  exact): one accumulator bounds rows x cols pair counts. A pass whose candidate list
@@ -67,7 +66,7 @@ int b200mol_free_async(void* d_ptr, void* stream);
  *   "etkdg_hessian_fp64"           0 (default): the embedder keeps its BFGS inverse Hessian in fp32 (products accumulated
  *                                  in fp64; half the slab traffic); 1: in fp64, the reference's storage type. The MMFF /
  *                                  UFF minimiser always uses fp64
- *   "bfgs_l2_persist"              1: mark the inverse-Hessian slabs persisting in L2 (measured slower on B200; default 0)
+ *   "bfgs_l2_persist"              1: mark the inverse-Hessian slabs persisting in L2 (default 0)
  *   "bfgs_ctas_per_sm"             resident CTAs per SM of the minimiser / embedder kernels (default 3 = the register
  *                                  budget they are compiled for) */
 int b200mol_set_option(const char* key, long long value);

@@ -1,4 +1,4 @@
-"""nvmolkit_b200 — the batched-molecule hot path of nvMolKit, rebuilt for B200 (sm_100a).
+"""nvmolkit_b200 — the batched-molecule hot path of nvMolKit, rebuilt for H100 (sm_90a).
 
 Module names and call signatures mirror ``nvmolkit.{fingerprints, similarity, clustering, embedMolecules,
 mmffOptimization, uffOptimization, types}``; the compute is hand-written CUDA behind the C-ABI in

@@ -14,9 +14,9 @@ _checked_devices: set = set()
 
 def require_cuda() -> None:
     if not torch.cuda.is_available():
-        raise RuntimeError("nvmolkit_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+        raise RuntimeError("nvmolkit_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
     dev = torch.cuda.current_device()
-    if dev not in _checked_devices:  # once per device: sm_100 check + keep the stream-ordered pool warm
+    if dev not in _checked_devices:  # once per device: sm_90 check + keep the stream-ordered pool warm
         from nvmolkit_b200 import _lib
 
         _lib.check(_lib.load().b200mol_check_device(dev))

@@ -83,7 +83,7 @@ def load() -> C.CDLL:
         if not os.path.exists(LIB_PATH):
             raise ImportError(
                 f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a). nvmolkit_b200 has no CPU fallback.")
+                "(nvcc, sm_90a). nvmolkit_b200 has no CPU fallback.")
         lib = C.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():
             fn = getattr(lib, name)

@@ -171,8 +171,8 @@ static inline void readBfgsClocks(unsigned long long* out) {
 // A lane owns V = 16/sizeof(HT) consecutive columns of a 32*V-wide chunk: one 128-bit load and store per row, the
 // column values and column sums stay in registers for all rows of the chunk, the row sums of FOUR rows are reduced
 // together by one exchange-halving butterfly (9 shuffles for 8 values instead of 40). Columns [n, ld) hold zeros, so
-// only the chunk that contains the diagonal needs per-element masks. The sweep is issue-bound, not latency-bound
-// (profiles/r01_path_b_summary.md), hence the instruction diet.
+// only the chunk that contains the diagonal needs per-element masks. The sweep is issue-bound, not latency-bound,
+// hence the instruction diet.
 #ifndef B200_SWEEP_PREFETCH
 #define B200_SWEEP_PREFETCH 0
 #endif
@@ -275,7 +275,7 @@ __device__ __noinline__ void hessianSweepT(HT* __restrict__ H, int ld, int n, HT
     };
     // rows above the chunk's diagonal block: no masks; rows inside it (CW is a multiple of 4): masked
     // The slabs live in HBM (444 of them do not fit L2 next to the streaming term tables) and a warp has four row packs
-    // in flight. Two ways of getting further ahead were measured and rejected (profiles/r02_path_b_summary.md): the next
+    // in flight. Two ways of getting further ahead were measured and rejected: the next
     // batch in registers spills at the 80-register budget of three CTAs per SM; asking the rows of a later batch into L2
     // with prefetch.global.L2 (B200_SWEEP_PREFETCH = batches ahead) is 3-5 % SLOWER than nothing (0, the default).
     // lanes 8 q + l, l < 4: row q of the batch, 128-byte line l of its 512 bytes in this chunk

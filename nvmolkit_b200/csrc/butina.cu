@@ -1,9 +1,9 @@
-// Butina clustering on a neighbour graph held as CSR in HBM, sm_100a.
+// Butina clustering on a neighbour graph held as CSR in HBM, sm_90a.
 //
 // Definition (RDKit ML.Cluster.Butina.ClusterData(reordering=True); see include/b200mol.h): repeatedly take the free
 // point with the most free neighbours (ties -> highest index), cluster = that point + its free neighbours.
 //
-// B200 design (not the reference's): the O(N^2) work happens exactly once — the fused similarity tile
+// Design (not the reference's): the O(N^2) work happens exactly once — the fused similarity tile
 // (tanimoto.cu) emits neighbour counts AND the edge list in one pass, or the dense distance matrix is scanned once —
 // and the greedy loop then runs on the CSR graph inside ONE persistent cooperative kernel: no per-cluster host sync
 // (the reference's fused_butina does three .item() syncs per cluster, nvmolkit/clustering.py:152-169, and its dense

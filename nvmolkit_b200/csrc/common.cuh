@@ -1,4 +1,4 @@
-// Shared host/device helpers for libb200mol (sm_100a only).
+// Shared host/device helpers for libb200mol (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -101,9 +101,9 @@ inline int smCount() {  // of the current device
   int        dev        = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) dev = 0;
   if (cached[dev] == 0) {
-    int v = 148;
+    int v = 132;
     cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    cached[dev] = v > 0 ? v : 148;
+    cached[dev] = v > 0 ? v : 132;
   }
   return cached[dev];
 }

@@ -1,5 +1,5 @@
 // Distance-geometry preparation kernels: bounds-matrix triangle smoothing, power-iteration eigensolver,
-// metric-matrix embedding. One CTA per molecule, the n x n matrix resident in shared memory (sm_100a: up to 227 KB,
+// metric-matrix embedding. One CTA per molecule, the n x n matrix resident in shared memory (sm_90a: up to 227 KB,
 // n <= 164 in fp64; larger matrices are processed in place in global memory / L2 by the same code).
 //
 // Replaces src/triangle_smooth.cu:27-247 (one kernel LAUNCH per pivot k over the whole concatenated batch, all traffic

@@ -1,4 +1,4 @@
-// Flattened force fields, block-cooperative evaluation for ONE conformer held in shared memory (sm_100a).
+// Flattened force fields, block-cooperative evaluation for ONE conformer held in shared memory (sm_90a).
 //
 // Every force field exposes   View (this molecule's term ranges),
 //                             eval<false>(view, pos, nullptr, tid, nT) -> this thread's partial energy,
@@ -14,7 +14,7 @@
 // within a wave, waves of a warp are ordered by __syncwarp, and the accumulators are summed in a fixed order afterwards
 // (bfgs_device.cuh gradOf). So the gradient - hence a whole minimisation - is bit-reproducible run to run, and the
 // gradient pass no longer waits on shared-memory fp64 CAS loops (1.4 per clock and SM measured, 6-8 per pair term:
-// that alone was ~4 SM-clocks per term against ~2.5 for the term's arithmetic, profiles/r01_path_b_summary.md).
+// that alone was ~4 SM-clocks per term against ~2.5 for the term's arithmetic).
 // The reference scatters with global atomicAdd(double) (mmff_kernels_device.cuh, dist_geom_kernels_device.cuh:66-94).
 //
 // Term math follows RDKit as restated by the reference: MMFF src/forcefields/mmff_kernels_device.cuh:28-661,
@@ -91,9 +91,9 @@ __device__ __forceinline__ void loadTerm(const b200mol_term_table& T, int t, Ter
 // Energy mode: thread-strided over the terms. Gradient mode: warp-strided over the waves, lane = term of the wave.
 // Both loops keep the NEXT term's record in flight while the current one is evaluated: the records stream from L2 / HBM
 // (a molecule's tables are 70-120 KB and ten thousand molecules do not fit L2), and a load-then-use loop paid that
-// latency once per term and thread - it, not the arithmetic, set the evaluation time (profiles/r02_path_b_summary.md).
+// latency once per term and thread - it, not the arithmetic, set the evaluation time.
 #ifndef B200_TERM_PREFETCH
-#define B200_TERM_PREFETCH 0  // 0 = load-then-use (default: neither prefetch form paid on B200, profiles/r02_path_b_summary.md); 1 = prefetch.global.L1 of the next record; 2 = next record in registers
+#define B200_TERM_PREFETCH 0  // 0 = load-then-use (default); 1 = prefetch.global.L1 of the next record; 2 = next record in registers
 #endif
 template <int K, int P>
 __device__ __forceinline__ void prefetchTerm(const b200mol_term_table& T, int t) {

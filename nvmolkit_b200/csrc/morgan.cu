@@ -1,4 +1,4 @@
-// Morgan (ECFP-style) fingerprints from flattened molecular graphs, one warp per molecule, sm_100a.
+// Morgan (ECFP-style) fingerprints from flattened molecular graphs, one warp per molecule, sm_90a.
 //
 // Algorithm = RDKit's MorganEnvGenerator as restated by the reference (src/morgan_fingerprint_cpu.cpp:61-255,
 // GPU twin src/morgan_fingerprint_kernels.cu:152-432), bit-exact:
@@ -8,7 +8,7 @@
 //   emitted before (this round by an atom with a smaller (invariant, index), or in any earlier round); otherwise the
 //   atom is dead from then on (dead atoms' invariants become 0, their neighbourhoods freeze).
 //
-// B200 design: the reference sorts all (bitset, invariant, atom) tuples of a round with a tile-wide CUB merge sort and
+// Design: the reference sorts all (bitset, invariant, atom) tuples of a round with a tile-wide CUB merge sort and
 // scans earlier rounds linearly in global memory. Only the equivalence classes matter, so this kernel replaces the sort
 // with a rank test — "is there an equal bitset with a smaller (invariant, atom) key, or an equal accepted bitset from
 // an earlier round" — all in shared memory, and handles molecules of any size that fits shared memory (no CPU twin).

@@ -1,4 +1,4 @@
-// N x M popcount similarity over packed u32 fingerprints (Tanimoto / cosine), sm_100a.
+// N x M popcount similarity over packed u32 fingerprints (Tanimoto / cosine), sm_90a.
 //
 // One CTA = one 128 x 128 tile of pairs. The two fingerprint blocks ([128 rows][<=128 B] per K chunk) are staged into
 // shared memory by TMA (cp.async.bulk.tensor.2d, hardware swizzle so that 16-byte LDS is bank-conflict free) and
@@ -307,7 +307,6 @@ extern int g_bfgsCtasPerSm;
 extern int g_bfgsL2Persist;
 extern int g_etkdgHessianFp64;
 extern int g_butinaMinCommits;
-extern int g_tensorFp4;
 extern int g_tensorCluster;
 extern int g_superpose;
 extern int g_superposeLast;
@@ -315,7 +314,7 @@ extern int g_superposeCols;
 extern int g_superposeAuto;
 extern int g_pipelineChunks;
 extern unsigned long long g_candidatesLast;
-long long g_tensorMinPairs = 1ll << 24;  // pair count from which the count mode runs on tcgen05 (< 0: never)
+long long g_tensorMinPairs = 1ll << 24;  // pair count from which the passes run on the tensor-core tile (< 0: never)
 
 void launchThreshTable(int maxS, double cutoff, uint16_t* thresh, cudaStream_t s) {
   threshTableKernel<<<(maxS + 1 + 127) / 128, 128, 0, s>>>(maxS, cutoff, thresh);
@@ -443,7 +442,6 @@ extern "C" int b200mol_set_option(const char* key, long long value) {
       B200_REQUIRE(value >= 1 && value <= 8, "similarity_pipeline_chunks must be in [1, 8]");
       g_pipelineChunks = static_cast<int>(value);
     }
-    else if (k == "similarity_tensor_fp4") g_tensorFp4 = value != 0;
     else if (k == "similarity_tensor_cluster") {
       B200_REQUIRE(value >= 0 && value <= 3, "similarity_tensor_cluster must be 0, 1, 2 or 3");
       g_tensorCluster = static_cast<int>(value);
@@ -464,7 +462,6 @@ extern "C" int b200mol_get_option(const char* key, long long* value) {
     else if (k == "bfgs_ctas_per_sm") *value = g_bfgsCtasPerSm;
     else if (k == "bfgs_l2_persist") *value = g_bfgsL2Persist;
     else if (k == "etkdg_hessian_fp64") *value = g_etkdgHessianFp64;
-    else if (k == "similarity_tensor_fp4") *value = g_tensorFp4;
     else if (k == "similarity_tensor_cluster") *value = g_tensorCluster;
     else if (k == "similarity_superpose") *value = g_superpose;
     else if (k == "similarity_superpose_cols") *value = g_superposeCols;
@@ -492,9 +489,12 @@ extern "C" int b200mol_check_device(int dev) {
     int n = 0;
     if (cudaGetDeviceCount(&n) != cudaSuccess || dev < 0 || dev >= n)
       fail(B200MOL_ERR_NODEVICE, "no CUDA device %d visible: libb200mol has no CPU fallback", dev);
-    int major = 0;
+    int major = 0, minor = 0;
     B200_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-    if (major != 10) fail(B200MOL_ERR_NODEVICE, "device %d is compute capability %d.x; libb200mol is sm_100a only", dev, major);
+    B200_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
+    if (major != 9 || minor != 0)
+      fail(B200MOL_ERR_NODEVICE, "device %d is compute capability %d.%d; libb200mol is built for sm_90a (H100) only", dev, major,
+           minor);
     retainPoolMemory(dev);
   });
 }

@@ -1,4 +1,4 @@
-// TMA (cp.async.bulk.tensor) + mbarrier helpers, sm_100a. Hand-written PTX wrappers; no CUTLASS.
+// TMA (cp.async.bulk.tensor) + mbarrier helpers, sm_90a. Hand-written PTX wrappers; no CUTLASS.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -101,16 +101,6 @@ __device__ __forceinline__ void tmaLoad2DMulticast(void* smemDst, const CUtensor
     "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], "
     "[%2], %5;" ::"r"(smemAddr(smemDst)),
     "l"(reinterpret_cast<uint64_t>(tm)), "r"(smemAddr(bar)), "r"(c0), "r"(c1), "h"(ctaMask)
-    : "memory");
-}
-// CTA-pair (cta_group::2) load: data lands in THIS CTA's shared memory, the bytes are counted on the barrier at the same
-// offset in the pair's LEADER (rank 0): clearing the peer bit of the shared::cluster address names the leader's copy
-// (cute/arch/copy_sm100_tma.hpp, Sm100MmaPeerBitMask).
-__device__ __forceinline__ void tmaLoad2DPair(void* smemDst, const CUtensorMap* tm, int c0, int c1, uint64_t* leaderBar) {
-  asm volatile(
-    "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
-      smemAddr(smemDst)),
-    "l"(reinterpret_cast<uint64_t>(tm)), "r"(smemAddr(leaderBar) & 0xFEFFFFFFu), "r"(c0), "r"(c1)
     : "memory");
 }
 // arrive on the barrier at the same offset in CTA `rank` of the cluster

@@ -11,7 +11,7 @@ import torch
 class HardwareOptions:
     """Batching knobs (reference: nvmolkit/types.py:26-122, src/hardware_options.h:26-35).
 
-    The B200 path runs one process per GPU and one persistent kernel per call, so ``batchSize`` /
+    This package runs one process per GPU and one persistent kernel per call, so ``batchSize`` /
     ``batchesPerGpu`` only bound how many conformers are resident at once; ``gpuIds`` selects the device
     (the first id) inside a single process. The fields, validation and (de)serialisation match the reference.
     """

@@ -36,7 +36,7 @@ def test_no_cpu_fallback_without_device(built_lib):
     if torch.cuda.is_available():
         return
     assert built_lib.b200mol_check_device(0) == _lib.ERR_NODEVICE
-    assert b"no CPU fallback" in built_lib.b200mol_last_error() or b"sm_100a" in built_lib.b200mol_last_error()
+    assert b"no CPU fallback" in built_lib.b200mol_last_error() or b"sm_90a" in built_lib.b200mol_last_error()
 
 
 def test_product_package_never_imports_oracle():

@@ -280,17 +280,17 @@ def test_butina_parallel_rounds_keep_the_greedy_order(cuda, min_commits, n, degr
     assert (ids.numpy() == ids_cpu).all() and (cen.numpy() == cen_cpu).all()
 
 
-# ------------------------------------------------------------------ tensor-core (tcgen05 int8) path of the count pass
+# ------------------------------------------------------------------ tensor-core (wgmma u8) path of the count pass
 @pytest.fixture(params=[(1, 4, 4), (0, 4, 4), (2, 4, 4), (3, 4, 4), (1, 1, 1), (3, 1, 1), (0, 2, 1), (1, 4, 1), (1, 1, 4),
                         (0, 2, 4)],
                 ids=["multicast_pair-super4x4", "single_cta-super4x4", "pair_mma-super4x4", "row_stationary-super4x4",
                      "multicast_pair-plain", "row_stationary-plain", "single_cta-super2x1", "multicast_pair-super4x1",
                      "multicast_pair-super1x4", "single_cta-super2x4"])
 def force_tensor_path(cuda, request):
-    """Every test that takes this fixture runs on all four tile variants of the fp4 count pass:
-    similarity_tensor_cluster = 1 (CTA pair, multicast column operand), 0 (one CTA per tile),
-    2 (CTA pair with tcgen05 cta_group::2 MMAs), 3 (CTA pair, multicast column operand, row operand stationary) - crossed
-    with the row x column superposition of the Butina neighbour pass (4 x 4 = default ... 1 x 1 = off)."""
+    """Every test that takes this fixture runs on all values of similarity_tensor_cluster: 1 (CTA pair, multicast column
+    operand), 0 (one CTA per tile), 2 (accepted for callers of the CTA-pair MMA that Hopper lacks: runs as 1),
+    3 (CTA pair, multicast column operand, row operand stationary for fingerprints up to 1024 bits) - crossed with the
+    row x column superposition of the Butina neighbour pass (4 x 4 = default ... 1 x 1 = off)."""
     from nvmolkit_b200 import _lib
 
     _lib.set_option("similarity_tensor_min_pairs", 0)
@@ -332,7 +332,7 @@ def test_tensor_fused_butina_equals_rdkit_definition(cuda, force_tensor_path, ce
 
 @pytest.mark.parametrize("n", [2, 3, 5, 127, 129, 897, 1023])
 def test_tensor_fused_butina_on_ragged_sizes(cuda, force_tensor_path, n):
-    """Sizes that are no multiple of the superposition factors, the tile rows (128) or the tile columns (224 / 448): the
+    """Sizes that are no multiple of the superposition factors, the tile rows (128) or the tile columns (256): the
     last super row / super column sums fewer fingerprints, the last tile is clipped."""
     from nvmolkit_b200.clustering import fused_butina_device
 
@@ -344,12 +344,41 @@ def test_tensor_fused_butina_on_ragged_sizes(cuda, force_tensor_path, n):
 
 
 def test_tensor_neighbor_counts_on_a_many_tile_problem(cuda, force_tensor_path):
-    """9,000 points = 71 tile rows x 41 tile columns: several row groups and, for the row-stationary tile, several runs of
-    16 tile columns per row with a row-operand reload between them."""
+    """9,000 points = 71 tile rows x 36 tile columns: several row groups, and for the CTA pairs an odd number of tile
+    rows (the last pair's lower tile lies past the end)."""
     from nvmolkit_b200.clustering import fused_butina_device
 
     fp = S.clustered_fingerprints(180, 50, seed=99)
     ids, cen = fused_butina_device(_dev(fp, cuda), 0.3)
+    ids_cpu, cen_cpu = oracle.butina_fp(fp, 0.3)
+    assert (ids.cpu().numpy() == ids_cpu).all() and (cen.cpu().numpy() == cen_cpu).all()
+
+
+@pytest.mark.parametrize("superpose", [1, 4])
+def test_row_stationary_tile_reloads_its_row_operand(cuda, superpose):
+    """1024-bit fingerprints keep the row tile of the row-stationary variant in shared memory: 9,000 points are several
+    runs of 16 tile columns per tile row with a row-operand reload between them (and, superposed, several row groups)."""
+    from nvmolkit_b200 import _lib
+
+    fp = S.clustered_fingerprints(180, 50, bits=1024, seed=98)
+    counts = torch.zeros(len(fp), dtype=torch.int32, device=cuda)
+    dfp = _dev(fp, cuda)
+    _lib.set_option("similarity_tensor_min_pairs", 0)
+    _lib.set_option("similarity_tensor_cluster", 3)
+    _lib.set_option("similarity_superpose", superpose)
+    _lib.set_option("similarity_superpose_cols", superpose)
+    try:
+        _lib.call("b200mol_tanimoto_count_ge", dfp.data_ptr(), len(fp), dfp.data_ptr(), len(fp), 32, 0, 0.3, 1,
+                  counts.data_ptr(), torch.cuda.current_stream().cuda_stream)
+        from nvmolkit_b200.clustering import fused_butina_device
+
+        ids, cen = fused_butina_device(dfp, 0.3)
+    finally:
+        _lib.set_option("similarity_tensor_cluster", 1)
+        _lib.set_option("similarity_superpose", 4)
+        _lib.set_option("similarity_superpose_cols", 4)
+        _lib.set_option("similarity_tensor_min_pairs", 1 << 24)
+    assert (counts.cpu().numpy() == oracle.count_ge(fp, fp, 0.3)).all()
     ids_cpu, cen_cpu = oracle.butina_fp(fp, 0.3)
     assert (ids.cpu().numpy() == ids_cpu).all() and (cen.cpu().numpy() == cen_cpu).all()
 

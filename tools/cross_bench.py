@@ -33,7 +33,7 @@ for n in sizes:
     torch.cuda.synchronize()
     ms_call = e0.elapsed_time(e1) / reps
     try:
-        ms_k, phase = _lib.profile_read("cross_tc"), "cross_tc (tcgen05 tile: fp4 operands when the fingerprint is a multiple of 256 bits, else int8)"
+        ms_k, phase = _lib.profile_read("cross_tc"), "cross_tc (wgmma u8 tensor-core tile)"
     except ValueError:
         ms_k, phase = ms_call, "whole call (SIMT popcount tile; below similarity_tensor_min_pairs)"
     bytes_ = 8.0 * n * n + 512.0 * n
