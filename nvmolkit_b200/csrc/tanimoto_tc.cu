@@ -10,14 +10,18 @@
 //              s32 accumulation exact), so one accumulator bounds S * C pair counts.
 //   tile       128 x 256 accumulators per step of a persistent CTA (optionally a cluster of two CTAs that share the
 //              column operand through TMA multicast)
-//   warp 0     TMA producer: [128 | 256 rows][128 B] K-chunks, SWIZZLE_128B, mbarrier ring of 4 stages
+//   warp 0     TMA producer: [128 | 256 rows][128 B] K-chunks, SWIZZLE_128B, mbarrier ring of 4 stages; per tile also
+//              the rows' and columns' {popcount, pre-filter term} (computed once per pass by tileMetaKernel) with one
+//              bulk copy into a 2-deep metadata ring, so the consumers issue no global load and meet at no barrier
+//              between tiles
 //   warpgroups 1-2  each issues wgmma.mma_async m64n256k32 .s32.u8.u8 for 64 of the tile's rows (accumulators in
 //              registers) and runs the epilogue on them: a fixed-point pre-filter (256 acc - floor(256 alpha |B_j|) >=
 //              floor(256 alpha |A_i|)) decides "no pair of this group can reach its threshold"; survivors go to a candidate list that
 //              verifyCandidatesKernel re-counts exactly with the integer threshold table (bit-exact with the fp64
 //              predicate, see tanimoto.cu). Unsuperposed (S = C = 1) the same warps apply the exact test themselves:
-//              neighbour counts for both endpoints + warp-aggregated edges. Materialise modes write fp64 Tanimoto /
-//              cosine values straight from the accumulator registers.
+//              neighbour counts for both endpoints + edges. Candidates and edges are staged per warp in shared memory
+//              and leave with one global atomic per 128-entry flush. Materialise modes write fp64 Tanimoto / cosine
+//              values straight from the accumulator registers.
 // A pilot over a prefix sample picks C for the data at hand; a candidate-list overflow reruns with fewer pairs per
 // accumulator before anything has been counted.
 //
@@ -51,8 +55,8 @@ struct TcParams {
   uint32_t        tilesM, tilesN;
   int             symmetric;
   uint32_t        groupOffset, groupStride;  // multi-GPU: this rank owns tile-row groups with group % stride == offset
-  const int32_t*  popX;
-  const int32_t*  popY;
+  const int2*     rowMeta;  // per row of the X operand, whole tiles: {popcount, floor(256 alpha popcount)} (tileMetaKernel)
+  const int2*     colMeta;  // per row of the Y operand (tile column), whole tiles: {popcount, -floor(256 alpha popcount)}
   const uint16_t* thresh;
   int             threshLen;
   int             sign;
@@ -65,7 +69,7 @@ struct TcParams {
   int             outVec;    // materialise modes: out 16-byte aligned and nY even (two values per store)
   const double*   recipG;    // RN(1/u), u = 0 .. 2 * bits (global memory, 64 KB at most: L1-resident)
   // Row superposition (count mode): a row of the X operand is the SUM of superS consecutive fingerprints (values 0..4),
-  // so one accumulator bounds superS pair counts at once; n / tilesM then count SUPER rows, popX holds the smallest
+  // so one accumulator bounds superS pair counts at once; n / tilesM then count SUPER rows, rowMeta holds the smallest
   // popcount of each super row, and the epilogue only lists candidates (super row, column) for the exact verification
   // kernel. rowSpan = fingerprints per tile row = kTM * superS.
   int                 superS;
@@ -120,15 +124,23 @@ __global__ void expandBitsSuperKernel(const uint32_t* __restrict__ fp, size_t n,
   out[2 * t + 1] = make_uint4(b[4], b[5], b[6], b[7]);
 }
 
-// smallest popcount among the fingerprints of each super row (the epilogue's conservative pre-filter needs the lowest
-// threshold any pair of the group can have)
-__global__ void superMinPopKernel(const int32_t* __restrict__ pop, size_t n, int S, size_t nSuper, int32_t* __restrict__ out) {
+// What the tile epilogue needs of each operand row, computed once per pass and fetched by the producer per tile with
+// one bulk copy: .x = the smallest popcount among the S fingerprints summed into the row (the conservative pre-filter
+// needs the lowest threshold any pair of the group can have; with S = 1 the popcount itself), .y = dir * floor(256
+// alpha .x), the pre-filter's fixed-point term (dir = +1 for rows, -1 for columns). Rows past the end, up to whole
+// tiles (nPad), get popcount 0 and dir * 0x3fffffff, which no accumulator passes.
+__global__ void tileMetaKernel(const int32_t* __restrict__ pop, size_t n, int S, size_t nSuper, size_t nPad, float alpha, int dir,
+                               int2* __restrict__ out) {
   const size_t R = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (R >= nSuper) return;
+  if (R >= nPad) return;
+  if (R >= nSuper) {
+    out[R] = make_int2(0, dir * 0x3fffffff);
+    return;
+  }
   int m = 0x3fffffff;
   for (int s = 0; s < S; ++s)
     if (R * S + s < n) m = min(m, pop[R * S + s]);
-  out[R] = m;
+  out[R] = make_int2(m, dir * static_cast<int>(floorf(__fmul_rd(256.0f * alpha, static_cast<float>(m)))));
 }
 
 // Exact verification of the candidates of a superposed pass: one warp per (super row R, super column J), for each of
@@ -278,29 +290,66 @@ __device__ __forceinline__ void wgmmaWait() {
   asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
 
-// Appends the (row, column) pairs of `bits` (bit e: row e < 2 ? r0 : r1, column c0 + (e & 1)) of every lane of the warp
-// to `list` with one atomic per warp. Entries past `cap` are dropped; the cursor still counts them.
-__device__ __forceinline__ void appendPairs(uint32_t bits, uint32_t r0, uint32_t r1, uint32_t c0, int2* list,
-                                            unsigned long long* cursor, unsigned long long cap, int lane) {
-  const int mine = __popc(bits);
-  int       incl = mine;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int v = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += v;
-  }
-  const int          total = __shfl_sync(0xffffffffu, incl, 31);
-  unsigned long long base  = 0;
-  if (lane == 31) base = atomicAdd(cursor, static_cast<unsigned long long>(total));
-  base                  = __shfl_sync(0xffffffffu, base, 31);
-  unsigned long long at = base + incl - mine;
-#pragma unroll
-  for (int e = 0; e < 4; ++e)
-    if ((bits >> e) & 1u) {
-      if (at < cap) list[at] = make_int2(static_cast<int>(e < 2 ? r0 : r1), static_cast<int>(c0 + (e & 1)));
-      ++at;
-    }
+// 16-byte shared-memory load that the compiler may not merge with another one of the same address: the count epilogue
+// reads its column metadata in the pre-filter and again for the survivors, and keeping the pre-filter's 32 int4 alive
+// until then would spill
+__device__ __forceinline__ int4 ldsFresh(const int4* p) {
+  int4 v;
+  asm volatile("ld.volatile.shared.v4.s32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(smemAddr(p)));
+  return v;
 }
+
+// The list of one epilogue warp of the count tile - candidates when superposed, else edges (if asked for): (row, column)
+// pairs are parked in kStagePairs shared-memory slots and leave with ONE global atomic per flush, when the slots are
+// full and at the end of the warp's work. The atomic's result (the store address) is waited on once per flush instead
+// of once per column block with a hit. Entries past the list's capacity are dropped; the cursor still counts them.
+constexpr int kStagePairs = 128;  // >= the 4 x 32 pairs one add() can bring
+struct PairStage {
+  int n;  // pairs parked in `slot` (the warp's kStagePairs shared-memory slots, passed in: no register holds the address)
+  __device__ __forceinline__ void flush(const TcParams& p, int2* slot, int lane) {
+    if (n == 0) return;
+    const bool               super  = p.superS * p.superC > 1;
+    int2* const              list   = super ? p.cand : p.edges;
+    const unsigned long long cap    = super ? p.candCap : p.edgeCap;
+    __syncwarp();
+    unsigned long long base = 0;
+    if (lane == 0) base = atomicAdd(super ? p.candCursor : p.edgeCursor, static_cast<unsigned long long>(n));
+    base = __shfl_sync(0xffffffffu, base, 0);
+    for (int k = lane; k < n; k += 32)
+      if (base + k < cap) list[base + k] = slot[k];
+    __syncwarp();
+    n = 0;
+  }
+  // the pairs of `bits` (bit e: row e < 2 ? r0 : r1, column c0 + (e & 1)) of every lane of the warp
+  __device__ __forceinline__ void add(const TcParams& p, int2* slot, uint32_t bits, uint32_t r0, uint32_t r1, uint32_t c0, int lane) {
+    const int mine = __popc(bits);
+    int       incl = mine;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int v = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += v;
+    }
+    const int total = __shfl_sync(0xffffffffu, incl, 31);
+    if (n + total > kStagePairs) flush(p, slot, lane);
+    int at = n + incl - mine;
+#pragma unroll
+    for (int e = 0; e < 4; ++e)
+      if ((bits >> e) & 1u) slot[at++] = make_int2(static_cast<int>(e < 2 ? r0 : r1), static_cast<int>(c0 + (e & 1)));
+    n += total;
+  }
+};
+
+#ifdef B200_TC_TIMING
+// clock64() attribution of the tile loop (make tctiming, tools/pair_pass_timing.py). Consumer warps (lane 0, summed over
+// warps): 0 the wait for the tile's metadata, 1 fullBar waits, 2 wgmma waits, 3 pre-filter, 4 candidate / edge path
+// (with the last flush), 5 warp-tiles, 6 the whole tile loop; 7 the producer thread's emptyBar waits.
+__device__ unsigned long long g_tcClk[8];
+#define B200_TC_T0(t) const long long t = clock64()
+#define B200_TC_T1(t, slot) tcClk[slot] += clock64() - (t)
+#else
+#define B200_TC_T0(t)
+#define B200_TC_T1(t, slot)
+#endif
 
 // Work units. A unit = one tile (CL = 0) or two vertically adjacent tiles of one tile column (CTA pairs: unit row r
 // holds tile rows 2 r and 2 r + 1, the two CTAs share the column operand). Unit rows come in groups of G (p.groupTiles
@@ -413,8 +462,12 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
   constexpr int  kAResident = ST ? kMaxChunksStat * kABytes : 0;  // the stationary row tile, ahead of the ring
   __shared__ uint64_t fullBar[kStages], emptyBar[kStages];
   __shared__ uint64_t aFull[ST ? kMaxChunksStat : 1], aEmpty[ST ? kMaxChunksStat : 1];
-  __shared__ __align__(8) int popB[2][kTN];
-  __shared__ __align__(8) int colI[2][COUNT ? kTN : 2];  // count mode: -floor(256 alpha |B_j|), hugely negative past the end
+  // the tile's row and column metadata (tileMetaKernel), two tiles deep: the producer fetches tile t + 1's while the
+  // consumers still read tile t's
+  __shared__ uint64_t metaFull[2], metaEmpty[2];
+  __shared__ __align__(16) int2 colMeta[2][kTN];
+  __shared__ __align__(16) int2 rowMeta[2][kTM];
+  __shared__ int2 pairSlots[COUNT ? 8 : 1][COUNT ? kStagePairs : 1];  // count mode: each epilogue warp's PairStage
 
   const uint32_t rank      = CL ? clusterCtaRank() : 0u;
   const uint32_t firstUnit = CL ? blockIdx.x / 2 : blockIdx.x, unitStep = CL ? gridDim.x / 2 : gridDim.x;
@@ -422,6 +475,9 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
   const uint32_t smemBase  = smemA + kAResident;                    // the ring
   uint8_t*       smemGen   = smemRaw + (smemBase - smemAddr(smemRaw));
   const int      warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#ifdef B200_TC_TIMING
+  unsigned long long tcClk[8] = {};
+#endif
 
   if (threadIdx.x == 0) {
     tmaPrefetchDesc(&tmA);
@@ -435,6 +491,10 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
         mbarInit(&aFull[s], 1);
         mbarInit(&aEmpty[s], 8);  // the row tile is this CTA's own: its eight consumer warps
       }
+    for (int s = 0; s < 2; ++s) {
+      mbarInit(&metaFull[s], 1);
+      mbarInit(&metaEmpty[s], 8);
+    }
     fenceBarrierInit();
   }
   __syncthreads();
@@ -444,12 +504,20 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
     // ===================== TMA producer (one thread) =====================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if (threadIdx.x == 0) {
-      int      stage = 0;
-      uint32_t phase = 0, aPhase = 0;
+      int      stage = 0, meta = 0;
+      uint32_t phase = 0, aPhase = 0, metaPhase = 0;
       for (Walk w(p, firstUnit, unitStep); !w.done; w.next(p)) {
         uint32_t tm, tnBeg, tnEnd;
         if (!w.coords(p, rank, tm, tnBeg, tnEnd)) continue;
         for (uint32_t tn = tnBeg; tn < tnEnd; ++tn) {
+          mbarWait(&metaEmpty[meta], metaPhase ^ 1);
+          mbarExpectTx(&metaFull[meta], (kTN + kTM) * sizeof(int2));
+          bulkLoad1D(colMeta[meta], p.colMeta + static_cast<size_t>(tn) * kTN, kTN * sizeof(int2), &metaFull[meta]);
+          bulkLoad1D(rowMeta[meta], p.rowMeta + static_cast<size_t>(tm) * kTM, kTM * sizeof(int2), &metaFull[meta]);
+          if (++meta == 2) {
+            meta = 0;
+            metaPhase ^= 1;
+          }
           for (int kc = 0; kc < p.kChunks; ++kc) {
             if constexpr (ST) {
               if (tn == tnBeg) {  // this unit's row tile, chunk kc: once the previous unit's last tile is done with it
@@ -458,7 +526,9 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
                 tmaLoad2D(smemRaw + (smemA - smemAddr(smemRaw)) + kc * kABytes, &tmA, kc * kTK, tm * kTM, &aFull[kc]);
               }
             }
+            B200_TC_T0(tw);
             mbarWait(&emptyBar[stage], phase ^ 1);
+            B200_TC_T1(tw, 7);
             uint8_t* dst = smemGen + stage * kStgBytes;
             mbarExpectTx(&fullBar[stage], kStgBytes);
             if constexpr (!ST) tmaLoad2D(dst, &tmA, kc * kTK, tm * kTM, &fullBar[stage]);
@@ -479,6 +549,9 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
         }
         aPhase ^= 1;
       }
+#ifdef B200_TC_TIMING
+      atomicAdd(&g_tcClk[7], tcClk[7]);
+#endif
     }
   } else {
     // ===================== MMA + epilogue (warpgroups 1 and 2: rows 0..63 and 64..127 of the tile) =====================
@@ -488,33 +561,26 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
     uint32_t       acc[128];
     int            stage = 0;
     uint32_t       phase = 0, local = 0, aPhase = 0;
+    PairStage      pairs{0};
     auto release = [&](int s) {  // this warp's MMAs on stage s have retired
       if (lane == 0) {
         mbarArrive(&emptyBar[s]);
         if constexpr (CL) mbarArriveRemote(&emptyBar[s], rank ^ 1u);
       }
     };
+    B200_TC_T0(tLoop);
     for (Walk w(p, firstUnit, unitStep); !w.done; w.next(p)) {
       uint32_t tm, tnBeg, tnEnd;
       if (!w.coords(p, rank, tm, tnBeg, tnEnd)) continue;
       for (uint32_t tn = tnBeg; tn < tnEnd; ++tn) {
-        const int      buf = local & 1;
-        const uint32_t r0  = tm * kTM + wg * 64 + (warp & 3) * 16 + (lane >> 2), r1 = r0 + 8;
-        const int      pa0 = r0 < p.n ? __ldg(p.popX + r0) : 0, pa1 = r1 < p.n ? __ldg(p.popX + r1) : 0;
-        {  // this tile's column popcounts (double-buffered: the other warpgroup may still read the previous tile's)
-          const uint32_t gc = tn * kTN + ct;
-          const int      pb = gc < p.nY ? __ldg(p.popY + gc) : 0;
-          popB[buf][ct]     = pb;
-          if constexpr (COUNT) colI[buf][ct] = gc < p.nY ? -static_cast<int>(floorf(__fmul_rd(256.0f * p.alpha, static_cast<float>(pb)))) : -0x3fffffff;
-        }
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-
         int prev = -1;
         for (int kc = 0; kc < p.kChunks; ++kc) {
+          B200_TC_T0(tFull);
           if constexpr (ST) {
             if (tn == tnBeg) mbarWait(&aFull[kc], aPhase);
           }
           mbarWait(&fullBar[stage], phase);
+          B200_TC_T1(tFull, 1);
           fenceAccumulators(acc);
           wgmmaFence();
           const uint32_t sAddr = smemBase + stage * kStgBytes;
@@ -524,7 +590,9 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
           for (int k = 0; k < kTK / 32; ++k) wgmmaU8(acc, aDesc + 2 * k, bDesc + 2 * k, (kc | k) != 0 ? 1u : 0u);
           wgmmaCommit();
           if (prev >= 0) {
+            B200_TC_T0(tMma);
             wgmmaWait<1>();  // the previous chunk's MMAs have read their stage
+            B200_TC_T1(tMma, 2);
             release(prev);
           }
           prev = stage;
@@ -533,7 +601,11 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
             phase ^= 1;
           }
         }
-        wgmmaWait<0>();
+        {
+          B200_TC_T0(tMma);
+          wgmmaWait<0>();
+          B200_TC_T1(tMma, 2);
+        }
         fenceAccumulators(acc);
         release(prev);
         if constexpr (ST) {
@@ -541,6 +613,18 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
             for (int kc = 0; kc < p.kChunks; ++kc) mbarArrive(&aEmpty[kc]);
         }
 
+        const int meta = local & 1;
+        {
+          B200_TC_T0(tMeta);
+          mbarWait(&metaFull[meta], (local >> 1) & 1);  // (long since landed: requested before the tile's first K chunk)
+          B200_TC_T1(tMeta, 0);
+        }
+        const int      rl = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // this thread's rows rl, rl + 8 of the tile
+        const uint32_t r0 = tm * kTM + rl, r1 = r0 + 8;
+        const int2     ra0 = rowMeta[meta][rl], ra1 = rowMeta[meta][rl + 8];
+        const int      pa0 = ra0.x, pa1 = ra1.x;
+        // colMeta[meta][8 j + 2 q + h] = {popcount, pre-filter term} of column c0 + 8 j + h, as one 16-byte load
+        const int4*    cm = reinterpret_cast<const int4*>(&colMeta[meta][2 * q]);
         const uint32_t c0 = tn * kTN + 2 * q;  // column of acc[0]; acc[4 j ..] sit 8 j further
         if constexpr (COUNT) {
           // Pre-filter: a pair (or a superposed group of pairs) can only pass with c >= alpha (|A| + |B|) (the exact
@@ -548,52 +632,76 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
           // products in 1/256 units and rounded down (acc <= 65,536: no overflow)
           //   256 acc - floor(256 alpha |B_j|)  >=  floor(256 alpha |A_i|)
           // is necessary. The common case is "no survivor in this thread's 128 accumulators": a max per row decides it.
-          const int rowI0 = r0 < p.n ? static_cast<int>(floorf(__fmul_rd(256.0f * p.alpha, static_cast<float>(pa0)))) : 0x3fffffff;
-          const int rowI1 = r1 < p.n ? static_cast<int>(floorf(__fmul_rd(256.0f * p.alpha, static_cast<float>(pa1)))) : 0x3fffffff;
+          B200_TC_T0(tPre);
+          const int rowI0 = ra0.y, rowI1 = ra1.y;
           int       m0 = -0x3fffffff, m1 = -0x3fffffff;
 #pragma unroll
           for (int j = 0; j < 32; ++j) {
-            const int2 ci = *reinterpret_cast<const int2*>(&colI[buf][8 * j + 2 * q]);
-            m0            = max(m0, max(256 * static_cast<int>(acc[4 * j]) + ci.x, 256 * static_cast<int>(acc[4 * j + 1]) + ci.y));
-            m1            = max(m1, max(256 * static_cast<int>(acc[4 * j + 2]) + ci.x, 256 * static_cast<int>(acc[4 * j + 3]) + ci.y));
+            const int4 ci = cm[4 * j];
+            m0            = max(m0, max(256 * static_cast<int>(acc[4 * j]) + ci.y, 256 * static_cast<int>(acc[4 * j + 1]) + ci.w));
+            m1            = max(m1, max(256 * static_cast<int>(acc[4 * j + 2]) + ci.y, 256 * static_cast<int>(acc[4 * j + 3]) + ci.w));
           }
           const bool super = p.superS * p.superC > 1;
-          // every (row, column) of the tile is a pair with row fingerprints < column fingerprints: the tile's last row
-          // group ends before its first column group starts
-          const bool interior = !p.symmetric || (static_cast<uint64_t>(tm) * kTM + kTM) * p.superS <= static_cast<uint64_t>(tn) * kTN * p.superC;
           int        hits0 = 0, hits1 = 0;
-          if (__any_sync(0xffffffffu, m0 >= rowI0 || m1 >= rowI1)) {
+          const bool anySurvivor = __any_sync(0xffffffffu, m0 >= rowI0 || m1 >= rowI1);
+          B200_TC_T1(tPre, 3);
+          B200_TC_T0(tCand);
+          if (anySurvivor && super) {
+            // The survivors of the pre-filter as bits 4 (j % 8) + e of sv[j / 8], in one unrolled pass over the
+            // accumulators; the candidate list then takes them in a ROLLED loop over the column blocks that hold any.
+            // (Unrolled 32 times, the list code made the tile loop hundreds of KB of straight-line code that ran from
+            // cold instruction caches on every tile with a survivor.)
+            uint32_t sv[4] = {0, 0, 0, 0}, blocks = 0;  // blocks: bit j = a survivor in column block j
 #pragma unroll
             for (int j = 0; j < 32; ++j) {
-              uint32_t bits = 0;
+              const int4 ci  = ldsFresh(cm + 4 * j);
+              uint32_t   nib = 0;
+#pragma unroll
+              for (int e = 0; e < 4; ++e)
+                if (256 * static_cast<int>(acc[4 * j + e]) + ((e & 1) ? ci.w : ci.y) >= (e < 2 ? rowI0 : rowI1)) nib |= 1u << e;
+              sv[j >> 3] |= nib << (4 * (j & 7));
+              if (nib) blocks |= 1u << j;
+            }
+            // the column blocks where any lane of the warp has a survivor, one at a time
+            for (uint32_t todo = __reduce_or_sync(0xffffffffu, blocks); todo; todo &= todo - 1) {
+              const int      j   = __ffs(todo) - 1;
+              const uint32_t nib = ((j < 8 ? sv[0] : j < 16 ? sv[1] : j < 24 ? sv[2] : sv[3]) >> (4 * (j & 7))) & 0xFu;
+              uint32_t       bits = 0;
+#pragma unroll
+              for (int e = 0; e < 4; ++e) {
+                const uint32_t r = e < 2 ? r0 : r1, c = c0 + 8 * j + (e & 1);
+                // the exact verification kernel re-examines the group: a pair i < j must exist
+                if ((nib >> e) & 1u && r < p.n && c < p.nY &&
+                    (!p.symmetric || r * static_cast<uint32_t>(p.superS) + 1u < (c + 1u) * static_cast<uint32_t>(p.superC)))
+                  bits |= 1u << e;
+              }
+              if (__any_sync(0xffffffffu, bits != 0)) pairs.add(p, pairSlots[warp - 4], bits, r0, r1, c0 + 8 * j, lane);
+            }
+          } else if (anySurvivor) {  // unsuperposed: the exact test, neighbour counts for both endpoints and the edges
+#pragma unroll
+            for (int j = 0; j < 32; ++j) {
+              uint32_t   bits = 0;
+              const int4 ci   = ldsFresh(cm + 4 * j);
 #pragma unroll
               for (int e = 0; e < 4; ++e) {
                 const uint32_t r = e < 2 ? r0 : r1, c = c0 + 8 * j + (e & 1);
                 const int      a = static_cast<int>(acc[4 * j + e]);
-                if (256 * a + colI[buf][8 * j + 2 * q + (e & 1)] < (e < 2 ? rowI0 : rowI1) || r >= p.n || c >= p.nY) continue;
-                bool ok;
-                if (super)  // superposed: the exact verification kernel re-examines the group (a pair i < j must exist)
-                  ok = interior || !p.symmetric || r * static_cast<uint32_t>(p.superS) + 1u < (c + 1u) * static_cast<uint32_t>(p.superC);
-                else
-                  ok = (!p.symmetric || r < c) && a >= p.thresh[(e < 2 ? pa0 : pa1) + popB[buf][8 * j + 2 * q + (e & 1)]];
-                if (ok) bits |= 1u << e;
+                if (256 * a + ((e & 1) ? ci.w : ci.y) < (e < 2 ? rowI0 : rowI1) || r >= p.n || c >= p.nY) continue;
+                if ((!p.symmetric || r < c) && a >= p.thresh[(e < 2 ? pa0 : pa1) + ((e & 1) ? ci.z : ci.x)]) bits |= 1u << e;
               }
               if (!__any_sync(0xffffffffu, bits != 0)) continue;
-              if (super) {
-                appendPairs(bits, r0, r1, c0 + 8 * j, p.cand, p.candCursor, p.candCap, lane);
-                continue;
-              }
               hits0 += __popc(bits & 3u);
               hits1 += __popc(bits >> 2);
               if (p.countsY)
 #pragma unroll
                 for (int e = 0; e < 4; ++e)
                   if ((bits >> e) & 1u) atomicAdd(p.countsY + c0 + 8 * j + (e & 1), p.sign);
-              if (p.edges) appendPairs(bits, r0, r1, c0 + 8 * j, p.edges, p.edgeCursor, p.edgeCap, lane);
+              if (p.edges) pairs.add(p, pairSlots[warp - 4], bits, r0, r1, c0 + 8 * j, lane);
             }
           }
           if (hits0) atomicAdd(p.counts + r0, p.sign * hits0);
           if (hits1) atomicAdd(p.counts + r1, p.sign * hits1);
+          B200_TC_T1(tCand, 4);
         } else {
           // fp64 Tanimoto / cosine straight from the accumulators: a quad of lanes writes 64 contiguous bytes of a row
 #pragma unroll
@@ -603,7 +711,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
               const int cnt = static_cast<int>(acc[4 * j + e]);
-              const int pak = e < 2 ? pa0 : pa1, pb = popB[buf][8 * j + 2 * q + (e & 1)];
+              const int pak = e < 2 ? pa0 : pa1, pb = (e & 1) ? cm[4 * j].z : cm[4 * j].x;
               v[e]          = 0.0;
               if (cnt != 0) {
                 if constexpr (MODE == kTcTanimoto) {
@@ -633,10 +741,25 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
             }
           }
         }
+        __syncwarp();
+        if (lane == 0) mbarArrive(&metaEmpty[meta]);
         ++local;
+#ifdef B200_TC_TIMING
+        tcClk[5] += 1;
+#endif
       }
       aPhase ^= 1;
     }
+    if constexpr (COUNT) {
+      B200_TC_T0(tFlush);
+      pairs.flush(p, pairSlots[warp - 4], lane);  // (n stays 0 when the pass lists nothing)
+      B200_TC_T1(tFlush, 4);
+    }
+#ifdef B200_TC_TIMING
+    B200_TC_T1(tLoop, 6);
+    if (lane == 0)
+      for (int k = 0; k < 7; ++k) atomicAdd(&g_tcClk[k], tcClk[k]);
+#endif
   }
   __syncthreads();
   if constexpr (CL) clusterSync();  // no CTA leaves while its peer may still signal its barriers
@@ -687,8 +810,10 @@ bool launchSimilarityTensor(SimMode mode, const SimLaunch& q, cudaStream_t s) {
     const double sX = static_cast<double>(pilot.nX), sY = static_cast<double>(pilot.nY);
     const double pilotPairs = q.symmetric ? sX * (sX - 1) / 2.0 : sX * sY;
     const double totalPairs = (q.symmetric ? nX * (nX - 1) / 2.0 : nX * nY) / (q.groupStride < 1 ? 1 : q.groupStride);
-    // seconds per unsuperposed pair / per verified pair; only their ratio (about 1 : 120) steers the choice
-    constexpr double tPair = 0.85e-12, tVerify = 0.1e-9;
+    // seconds per unsuperposed pair / per verified pair; only their ratio (about 1 : 30) steers the choice. tPair is the
+    // measured pass: 214 ms for the 5.0e11 pairs of the 1M bench at S C = 8 (H100 SXM, 400 W limit). On the bench data
+    // the pilot then costs 4 x 4 at 0.39 s and 4 x 2 at 0.24 s, and runs 4 x 2.
+    constexpr double tPair = 3.4e-12, tVerify = 0.1e-9;
     double bestT = totalPairs * tPair;  // unsuperposed
     int    bestS = 1, bestC = 1;
     for (int c = C; c >= 1; c >>= 1) {
@@ -784,24 +909,21 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
   const uint8_t* expY = ownY ? expYown.get() : expX.get();
 
   Scratch<int32_t> popX(q.nX, s), popYown(same ? 0 : q.nY, s);
-  Scratch<int32_t> popSuper(superS > 1 ? nSuper : 0, s), popSuperY(superC > 1 && ownY ? nSuperY : 0, s);
   launchRowPopcount(q.x, q.nX, q.words, popX.get(), s);
   if (!same) launchRowPopcount(q.y, q.nY, q.words, popYown.get(), s);
   const int32_t* popYExact = same ? popX.get() : popYown.get();
-  p.popX = popX.get();
-  p.popY = popYExact;
-  if (superS > 1) {
-    superMinPopKernel<<<static_cast<unsigned>((nSuper + 255) / 256), 256, 0, s>>>(popX.get(), q.nX, superS, nSuper, popSuper.get());
-    B200_LAUNCHED();
-    p.popX = popSuper.get();
-  }
-  if (superC > 1) {
-    if (ownY) {
-      superMinPopKernel<<<static_cast<unsigned>((nSuperY + 255) / 256), 256, 0, s>>>(popYExact, q.nY, superC, nSuperY, popSuperY.get());
-      B200_LAUNCHED();
-      p.popY = popSuperY.get();
-    } else p.popY = popSuper.get();
-  }
+  // the epilogue's per-row metadata of both operands, padded to whole tiles for the producer's bulk copies (the lower
+  // tile of a CTA pair may lie one tile row past the end)
+  const size_t  rowsPad = (static_cast<size_t>(p.tilesM) + 1) * kTM, colsPad = static_cast<size_t>(p.tilesN) * kTN;
+  Scratch<int2> rowMeta(rowsPad, s), colMeta(colsPad, s);
+  tileMetaKernel<<<static_cast<unsigned>((rowsPad + 255) / 256), 256, 0, s>>>(popX.get(), q.nX, superS, nSuper, rowsPad, p.alpha, 1,
+                                                                             rowMeta.get());
+  B200_LAUNCHED();
+  tileMetaKernel<<<static_cast<unsigned>((colsPad + 255) / 256), 256, 0, s>>>(popYExact, q.nY, superC, nSuperY, colsPad, p.alpha, -1,
+                                                                             colMeta.get());
+  B200_LAUNCHED();
+  p.rowMeta = rowMeta.get();
+  p.colMeta = colMeta.get();
   // candidates of a superposed pass: (super row, super column) pairs the exact kernel re-examines. Sized for the
   // neighbour graphs this pass is used on (tens of edges per point); a denser graph overflows it and the caller falls back.
   unsigned long long          candCap = 0;
@@ -981,3 +1103,12 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
 }
 
 }  // namespace b200
+
+#ifdef B200_TC_TIMING
+extern "C" void b200mol_debug_clocks_tc(unsigned long long* out8) {  // reads and resets the tile loop's clock counters
+  cudaDeviceSynchronize();
+  cudaMemcpyFromSymbol(out8, b200::g_tcClk, sizeof(b200::g_tcClk));
+  unsigned long long z[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  cudaMemcpyToSymbol(b200::g_tcClk, z, sizeof(z));
+}
+#endif

@@ -103,6 +103,12 @@ __device__ __forceinline__ void tmaLoad2DMulticast(void* smemDst, const CUtensor
     "l"(reinterpret_cast<uint64_t>(tm)), "r"(smemAddr(bar)), "r"(c0), "r"(c1), "h"(ctaMask)
     : "memory");
 }
+// 1-D bulk copy global -> shared memory (16-byte aligned addresses, size a multiple of 16), completing on `bar`.
+__device__ __forceinline__ void bulkLoad1D(void* smemDst, const void* src, uint32_t bytes, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smemAddr(smemDst)),
+               "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(smemAddr(bar))
+               : "memory");
+}
 // arrive on the barrier at the same offset in CTA `rank` of the cluster
 __device__ __forceinline__ void mbarArriveRemote(uint64_t* bar, uint32_t rank) {
   asm volatile(
