@@ -345,7 +345,12 @@ void launchSimilarity(SimMode mode, const SimLaunch& q, cudaStream_t s) {
   tp.nX         = q.nX;
   tp.nY         = q.nY;
   tp.words      = q.words;
-  tp.innerWords = q.words < kChunkW ? q.words : kChunkW;
+  // The box is 4, 8, 16 or 32 words wide (16, 32, 64 or 128 B): exactly the span of the swizzle makeTensorMap2D picks
+  // for it, so box rows lie back to back in shared memory as the tile's address arithmetic assumes. A narrower
+  // fingerprint (384, 640, 768 or 896 bits) gets the next such box; TMA zero-fills the words past the row end, and
+  // they add nothing to the counts, as in the last chunk of a fingerprint wider than 1024 bits.
+  tp.innerWords = 4;
+  while (tp.innerWords < q.words && tp.innerWords < kChunkW) tp.innerWords <<= 1;
   tp.nChunks    = (q.words + kChunkW - 1) / kChunkW;
   tp.tilesM     = static_cast<uint32_t>((q.nX + kBM - 1) / kBM);
   tp.tilesN     = static_cast<uint32_t>((q.nY + kBN - 1) / kBN);

@@ -715,9 +715,10 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
               v[e]          = 0.0;
               if (cnt != 0) {
                 if constexpr (MODE == kTcTanimoto) {
-                  // c / u through one reciprocal + one Newton step: exhaustively verified on the CPU to equal the
-                  // correctly rounded quotient for every 1 <= c <= u <= 8192 (tests/test_oracle_golden.py); int ->
-                  // double through the 2^52 trick, RN(1/u) from the table
+                  // c / u through one reciprocal + one Newton step: equal to the correctly rounded quotient for every
+                  // 1 <= c <= u <= 8192, which oracle_recip_quotient_mismatches (oracle/oracle_fp.c) checks pair by
+                  // pair in test_reciprocal_newton_quotient_is_correctly_rounded; int -> double through the 2^52
+                  // trick, RN(1/u) from the table
                   const int    u  = pak + pb - cnt;
                   const double dc = __hiloint2double(0x43300000, cnt) - 4503599627370496.0;
                   const double du = __hiloint2double(0x43300000, u) - 4503599627370496.0;

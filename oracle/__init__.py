@@ -66,6 +66,8 @@ def _declare(L: C.CDLL) -> None:
     L.oracle_morgan_one.restype = C.c_int
     L.oracle_morgan.argtypes = [i32p, i32p, u32p, u32p, u16p, u16p, C.c_long, C.c_int, C.c_int, u32p]
     L.oracle_morgan.restype = None
+    L.oracle_recip_quotient_mismatches.argtypes = [C.c_int, C.c_int]
+    L.oracle_recip_quotient_mismatches.restype = C.c_long
     for name, fn in _LATE_DECL.items():
         if hasattr(L, name):
             fn(getattr(L, name))
@@ -99,6 +101,12 @@ def count_ge(x, y, cutoff: float, metric: str = "tanimoto", sign: int = 1, count
     lib().oracle_count_ge(_p(x, C.c_uint32), x.shape[0], _p(y, C.c_uint32), y.shape[0], x.shape[1], METRIC[metric],
                           float(cutoff), int(sign), _p(counts, C.c_int32))
     return counts
+
+
+def recip_quotient_mismatches(umax: int, newton: bool = True) -> int:
+    """Pairs 1 <= c <= u <= umax where the tensor tile's c / u = fma(fma(-q0, u, c), r, q0) (r = RN(1/u), q0 = RN(c r))
+    is not the correctly rounded quotient; newton=False counts those of q0 alone."""
+    return int(lib().oracle_recip_quotient_mismatches(int(umax), int(bool(newton))))
 
 
 def butina_dense(dist, cutoff: float):

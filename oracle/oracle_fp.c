@@ -84,6 +84,24 @@ void oracle_count_ge(const uint32_t* X, long nX, const uint32_t* Y, long nY, int
   free(py);
 }
 
+/* The materialised tensor-core Tanimoto epilogue (nvmolkit_b200/csrc/tanimoto_tc.cu) computes c / u without a division:
+ * r = RN(1/u), q0 = RN(c r), q = fma(fma(-q0, u, c), r, q0). Returns the number of pairs 1 <= c <= u <= umax for which
+ * q differs from the correctly rounded c / u (every pair is checked; umax = 8192 covers 4096-bit fingerprints).
+ * newton = 0 drops the correction step (q = q0), so that a caller can see the check find mismatches where they exist. */
+long oracle_recip_quotient_mismatches(int umax, int newton) {
+  long bad = 0;
+#pragma omp parallel for schedule(dynamic, 64) reduction(+ : bad)
+  for (int u = 1; u <= umax; ++u) {
+    const double du = (double)u, r = 1.0 / du;
+    for (int c = 1; c <= u; ++c) {
+      const double dc = (double)c, q0 = dc * r;
+      const double q  = newton ? fma(fma(-q0, du, dc), r, q0) : q0;
+      bad += q != dc / du;
+    }
+  }
+  return bad;
+}
+
 /* ---- Butina (ClusterData, reordering=True) on neighbour lists ---- */
 typedef struct {
   long* start; /* [n+1] */

@@ -14,18 +14,48 @@ def _dev(fp, cuda):
     return torch.from_numpy(np.ascontiguousarray(fp).view(np.int32)).to(cuda)
 
 
+def _with_every_density(fp, seed):
+    """fp with rows 1, 2, ... (as many as there are) replaced by an empty row, an all-ones row and rows of bit density
+    0.02, 0.5 and 0.97, each followed by a near duplicate (1 to 8 flipped bits). Intersections and unions then reach the
+    full width, and similarities span [0, 1]."""
+    n, words = fp.shape
+    bits = 32 * words
+    rng = np.random.default_rng(seed)
+    rows = []
+    for p in (0.0, 1.0, 0.02, 0.5, 0.97):
+        r = rng.random(bits) < p
+        d = r.copy()
+        d[rng.choice(bits, size=rng.integers(1, 9), replace=False)] ^= True
+        rows += [r, d]
+    out = fp.copy()
+    k = min(len(rows), n - 1)
+    if k > 0:
+        out[1:1 + k] = S.pack_bits(np.array(rows[:k]))
+    return out
+
+
+# Fingerprint widths the C-ABI accepts (multiples of 128 bits up to 4096) beyond the powers of two. On the SIMT tile:
+# a row narrower than 128 bytes that is no power of two of words (384 - 896 bits), a partial last K chunk (1152, 3072
+# bits), more K chunks than stages (3072, 4096 bits). On the tensor tile: odd K-chunk counts (384, 640, 896 bits: 3, 5,
+# 7) for the row-stationary variant, 9 chunks (1152) just past its limit, 24 and 32 chunks.
+SIMT_WIDTHS = [384, 640, 768, 896, 1152, 3072, 4096]
+TENSOR_WIDTHS = [384, 640, 896, 1152, 3072, 4096]
+
+
 # ------------------------------------------------------------------ similarity
-@pytest.mark.parametrize("bits", [128, 256, 512, 1024, 2048])
+@pytest.mark.parametrize("bits", [128, 256, 512, 1024, 2048] + SIMT_WIDTHS)
 @pytest.mark.parametrize("n,m", [(1, 1), (1, 300), (127, 129), (128, 128), (257, 513)])
 def test_cross_tanimoto_bit_exact(cuda, bits, n, m):
-    from nvmolkit_b200.similarity import crossTanimotoSimilarity
+    from nvmolkit_b200.similarity import crossCosineSimilarity, crossTanimotoSimilarity
 
-    a = S.random_fingerprints(n, bits=bits, p=0.05, seed=n * 7 + bits, near_dups=n // 4)
-    b = S.random_fingerprints(m, bits=bits, p=0.05, seed=m * 11 + bits + 1, near_dups=m // 4)
+    a = _with_every_density(S.random_fingerprints(n, bits=bits, p=0.05, seed=n * 7 + bits, near_dups=n // 4), bits)
+    b = _with_every_density(S.random_fingerprints(m, bits=bits, p=0.05, seed=m * 11 + bits + 1, near_dups=m // 4), bits + 1)
     b[: min(n, m) // 2] = a[: min(n, m) // 2]
-    got = crossTanimotoSimilarity(_dev(a, cuda), _dev(b, cuda)).numpy()
+    da, db = _dev(a, cuda), _dev(b, cuda)
+    got = crossTanimotoSimilarity(da, db).numpy()
     assert got.dtype == np.float64 and got.shape == (n, m)
     assert (got == oracle.similarity_cross(a, b)).all()
+    assert (crossCosineSimilarity(da, db).numpy() == oracle.similarity_cross(a, b, metric="cosine")).all()
 
 
 def test_cross_tanimoto_config1_1k_x_1k(cuda):
@@ -93,21 +123,35 @@ def test_memory_constrained_host_variant(cuda):
     _lib.call("b200mol_similarity_cross_host", a.ctypes.data, 700, b.ctypes.data, 333, 64, 0, out.ctypes.data,
               2 * 128 * 333 * 8)
     assert (out == oracle.similarity_cross(a, b)).all()
+    # 4096 bits, every density class, both metrics, several row blocks
+    a = _with_every_density(S.random_fingerprints(700, bits=4096, seed=23, near_dups=100), 23)
+    b = _with_every_density(S.random_fingerprints(333, bits=4096, seed=24, near_dups=50), 24)
+    b[:20] = a[:20]
+    for metric in ("tanimoto", "cosine"):
+        out = np.empty((700, 333))
+        _lib.call("b200mol_similarity_cross_host", a.ctypes.data, 700, b.ctypes.data, 333, 128, _lib.METRIC[metric],
+                  out.ctypes.data, 2 * 128 * 333 * 8)
+        assert (out == oracle.similarity_cross(a, b, metric=metric)).all(), metric
 
 
 @pytest.mark.parametrize("metric", ["tanimoto", "cosine"])
 @pytest.mark.parametrize("cutoff", [0.0, 0.3, 0.35, 0.65, 1.0])
 def test_count_ge_exact(cuda, metric, cutoff):
+    """SIMT tile, at every width class and with rows of every density, both signs."""
     from nvmolkit_b200 import _lib
 
-    x = S.clustered_fingerprints(12, 25, seed=31)
-    y = S.clustered_fingerprints(12, 11, seed=31)  # same centres, other members
-    dx, dy = _dev(x, cuda), _dev(y, cuda)
-    counts = torch.full((x.shape[0],), 1000, dtype=torch.int32, device=cuda)
-    _lib.call("b200mol_tanimoto_count_ge", dx.data_ptr(), x.shape[0], dy.data_ptr(), y.shape[0], 64,
-              _lib.METRIC[metric], cutoff, -1, counts.data_ptr(), torch.cuda.current_stream().cuda_stream)
-    want = oracle.count_ge(x, y, cutoff, metric=metric, sign=-1, counts=np.full(x.shape[0], 1000, dtype=np.int32))
-    assert (counts.cpu().numpy() == want).all()
+    for bits, dense in [(2048, False), (2048, True)] + [(bits, True) for bits in SIMT_WIDTHS]:
+        x = S.clustered_fingerprints(12, 25, bits=bits, seed=31)
+        y = S.clustered_fingerprints(12, 11, bits=bits, seed=31)  # same centres, other members
+        if dense:
+            x, y = _with_every_density(x, bits), _with_every_density(y, bits + 1)
+        dx, dy = _dev(x, cuda), _dev(y, cuda)
+        for sign in (-1, 1):
+            counts = torch.full((x.shape[0],), 1000, dtype=torch.int32, device=cuda)
+            _lib.call("b200mol_tanimoto_count_ge", dx.data_ptr(), x.shape[0], dy.data_ptr(), y.shape[0], bits // 32,
+                      _lib.METRIC[metric], cutoff, sign, counts.data_ptr(), torch.cuda.current_stream().cuda_stream)
+            want = oracle.count_ge(x, y, cutoff, metric=metric, sign=sign, counts=np.full(x.shape[0], 1000, dtype=np.int32))
+            assert (counts.cpu().numpy() == want).all(), (bits, sign)
 
 
 def test_threshold_boundary_is_fp64_exact(cuda):
@@ -304,20 +348,21 @@ def force_tensor_path(cuda, request):
     _lib.set_option("similarity_tensor_min_pairs", 1 << 24)
 
 
-@pytest.mark.parametrize("bits", [128, 512, 2048])
+@pytest.mark.parametrize("bits", [128, 512, 2048] + TENSOR_WIDTHS)
 @pytest.mark.parametrize("nx,ny", [(1, 1), (127, 255), (128, 256), (129, 257), (700, 333)])
 def test_tensor_count_ge_exact(cuda, force_tensor_path, bits, nx, ny):
     from nvmolkit_b200 import _lib
 
-    x = S.clustered_fingerprints(max(1, nx // 25 + 1), 25, bits=bits, seed=41)[:nx]
-    y = S.clustered_fingerprints(max(1, ny // 11 + 1), 11, bits=bits, seed=41)[:ny]
+    x = _with_every_density(S.clustered_fingerprints(max(1, nx // 25 + 1), 25, bits=bits, seed=41)[:nx], bits)
+    y = _with_every_density(S.clustered_fingerprints(max(1, ny // 11 + 1), 11, bits=bits, seed=41)[:ny], bits + 1)
     dx, dy = _dev(x, cuda), _dev(y, cuda)
     for cutoff in (0.3, 0.65):
-        counts = torch.full((nx,), 7, dtype=torch.int32, device=cuda)
-        _lib.call("b200mol_tanimoto_count_ge", dx.data_ptr(), nx, dy.data_ptr(), ny, bits // 32, 0, cutoff, 1,
-                  counts.data_ptr(), torch.cuda.current_stream().cuda_stream)
-        want = oracle.count_ge(x, y, cutoff, counts=np.full(nx, 7, dtype=np.int32))
-        assert (counts.cpu().numpy() == want).all(), (bits, nx, ny, cutoff)
+        for sign in (1, -1):
+            counts = torch.full((nx,), 7, dtype=torch.int32, device=cuda)
+            _lib.call("b200mol_tanimoto_count_ge", dx.data_ptr(), nx, dy.data_ptr(), ny, bits // 32, 0, cutoff, sign,
+                      counts.data_ptr(), torch.cuda.current_stream().cuda_stream)
+            want = oracle.count_ge(x, y, cutoff, sign=sign, counts=np.full(nx, 7, dtype=np.int32))
+            assert (counts.cpu().numpy() == want).all(), (bits, nx, ny, cutoff, sign)
 
 
 @pytest.mark.parametrize("centres,members,cutoff", [(1, 1, 0.3), (7, 40, 0.3), (40, 25, 0.3), (60, 17, 0.5), (100, 50, 0.3)])
@@ -341,6 +386,32 @@ def test_tensor_fused_butina_on_ragged_sizes(cuda, force_tensor_path, n):
         ids, cen = fused_butina_device(_dev(fp, cuda), cutoff)
         ids_cpu, cen_cpu = oracle.butina_fp(fp, cutoff)
         assert (ids.cpu().numpy() == ids_cpu).all() and (cen.cpu().numpy() == cen_cpu).all(), (n, cutoff)
+
+
+@pytest.mark.parametrize("bits", [640, 4096])
+def test_tensor_fused_butina_at_wide_and_odd_widths(cuda, force_tensor_path, bits):
+    """Fused Butina on 4096-bit fingerprints (32 K chunks) and on 640-bit ones (no power of two: 5 K chunks), with rows
+    of every density among the clustered ones."""
+    from nvmolkit_b200.clustering import fused_butina_device
+
+    fp = _with_every_density(S.clustered_fingerprints(40, 25, bits=bits, seed=bits), bits)
+    for cutoff in (0.3, 0.62):
+        ids, cen = fused_butina_device(_dev(fp, cuda), cutoff)
+        ids_cpu, cen_cpu = oracle.butina_fp(fp, cutoff)
+        assert (ids.cpu().numpy() == ids_cpu).all() and (cen.cpu().numpy() == cen_cpu).all(), (bits, cutoff)
+
+
+@pytest.mark.parametrize("metric", ["tanimoto", "cosine"])
+@pytest.mark.parametrize("bits", [640, 4096])
+def test_fused_butina_at_wide_and_odd_widths(cuda, metric, bits):
+    """The same on the SIMT tile, for both metrics."""
+    from nvmolkit_b200.clustering import fused_butina_device
+
+    fp = _with_every_density(S.clustered_fingerprints(40, 25, bits=bits, seed=bits), bits)
+    for cutoff in (0.3, 0.62):
+        ids, cen = fused_butina_device(_dev(fp, cuda), cutoff, metric=metric)
+        ids_cpu, cen_cpu = oracle.butina_fp(fp, cutoff, metric=metric)
+        assert (ids.cpu().numpy() == ids_cpu).all() and (cen.cpu().numpy() == cen_cpu).all(), (bits, cutoff)
 
 
 def test_tensor_neighbor_counts_on_a_many_tile_problem(cuda, force_tensor_path):
@@ -462,13 +533,13 @@ def test_tensor_and_simt_paths_agree_on_identical_rows(cuda, force_tensor_path):
     assert (ids.cpu().numpy() == 0).all() and cen.cpu().numpy().tolist() == [599]
 
 
-@pytest.mark.parametrize("bits", [128, 1024, 2048])
+@pytest.mark.parametrize("bits", [128, 1024, 2048] + TENSOR_WIDTHS)
 @pytest.mark.parametrize("n,m", [(1, 1), (127, 300), (129, 256), (640, 513)])
 def test_tensor_cross_similarity_bit_exact(cuda, force_tensor_path, bits, n, m):
     from nvmolkit_b200.similarity import crossCosineSimilarity, crossTanimotoSimilarity
 
-    a = S.random_fingerprints(n, bits=bits, p=0.05, seed=n * 7 + bits, near_dups=n // 4)
-    b = S.random_fingerprints(m, bits=bits, p=0.05, seed=m * 11 + bits + 1, near_dups=m // 4)
+    a = _with_every_density(S.random_fingerprints(n, bits=bits, p=0.05, seed=n * 7 + bits, near_dups=n // 4), bits)
+    b = _with_every_density(S.random_fingerprints(m, bits=bits, p=0.05, seed=m * 11 + bits + 1, near_dups=m // 4), bits + 1)
     b[: min(n, m) // 2] = a[: min(n, m) // 2]
     a[0] = 0  # empty fingerprint row
     da, db = _dev(a, cuda), _dev(b, cuda)
