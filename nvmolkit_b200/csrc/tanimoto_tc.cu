@@ -7,7 +7,9 @@
 //
 //   pre-pass   bits -> one u8 per bit (0 / 1) once per fingerprint set, 2 KB per 2048-bit row; for the neighbour pass a
 //              row operand is the SUM of S = 4 fingerprints and a column operand the sum of C = 1, 2 or 4 (bytes <= 4,
-//              s32 accumulation exact), so one accumulator bounds S * C pair counts.
+//              s32 accumulation exact), so one accumulator bounds S * C pair counts. The superposed pass first gathers
+//              the fingerprints in popcount order (stable), so that a group sums fingerprints of nearly equal popcount
+//              and the pre-filter's bound, set by the group's smallest popcount, is about as tight as a single pair's.
 //   tile       128 x 256 accumulators per step of a persistent CTA (optionally a cluster of two CTAs that share the
 //              column operand through TMA multicast)
 //   warp 0     TMA producer: [128 | 256 rows][128 B] K-chunks, SWIZZLE_128B, mbarrier ring of 4 stages; per tile also
@@ -18,15 +20,17 @@
 //              registers) and runs the epilogue on them: a fixed-point pre-filter (256 acc - floor(256 alpha |B_j|) >=
 //              floor(256 alpha |A_i|)) decides "no pair of this group can reach its threshold"; survivors go to a candidate list that
 //              verifyCandidatesKernel re-counts exactly with the integer threshold table (bit-exact with the fp64
-//              predicate, see tanimoto.cu). Unsuperposed (S = C = 1) the same warps apply the exact test themselves:
+//              predicate, see tanimoto.cu) and maps back to the caller's indices. Unsuperposed (S = C = 1) the same warps apply the exact test themselves:
 //              neighbour counts for both endpoints + edges. Candidates and edges are staged per warp in shared memory
 //              and leave with one global atomic per 128-entry flush. Materialise modes write fp64 Tanimoto / cosine
 //              values straight from the accumulator registers.
-// A pilot over a prefix sample picks C for the data at hand; a candidate-list overflow reruns with fewer pairs per
-// accumulator before anything has been counted.
+// A pilot over a prefix sample (itself ordered by popcount) picks C for the data at hand; a candidate-list overflow
+// reruns with fewer pairs per accumulator before anything has been counted.
 //
 // Replaces crossSimilarityKernelTensorOp (src/similarity_kernels.cu:104-240) + the Triton count kernel
 // (nvmolkit/_fusedButina.py:99-179) for the fused Butina pass.
+#include <cub/device/device_radix_sort.cuh>
+
 #include "profile.cuh"
 #include "similarity.cuh"
 #include "tma.cuh"
@@ -124,6 +128,20 @@ __global__ void expandBitsSuperKernel(const uint32_t* __restrict__ fp, size_t n,
   out[2 * t + 1] = make_uint4(b[4], b[5], b[6], b[7]);
 }
 
+__global__ void iotaKernel(int32_t* __restrict__ v, size_t n) {
+  const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i < n) v[i] = static_cast<int32_t>(i);
+}
+
+// out row i = fp row perm[i]; one thread per 16 bytes
+__global__ void gatherRowsKernel(const uint4* __restrict__ fp, const int32_t* __restrict__ perm, size_t n, int chunks,
+                                 uint4* __restrict__ out) {
+  const size_t t = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (t >= n * static_cast<size_t>(chunks)) return;
+  const size_t i = t / chunks;
+  out[t]         = fp[static_cast<size_t>(perm[i]) * chunks + t % chunks];
+}
+
 // What the tile epilogue needs of each operand row, computed once per pass and fetched by the producer per tile with
 // one bulk copy: .x = the smallest popcount among the S fingerprints summed into the row (the conservative pre-filter
 // needs the lowest threshold any pair of the group can have; with S = 1 the popcount itself), .y = dir * floor(256
@@ -146,6 +164,8 @@ __global__ void tileMetaKernel(const int32_t* __restrict__ pop, size_t n, int S,
 // Exact verification of the candidates of a superposed pass: one warp per (super row R, super column J), for each of
 // the S * C pairs (i = S R + s, j = C J + c) of the group the exact count |X_i & Y_j| and the exact integer threshold
 // test; counts for both endpoints and the (i < j) edge list exactly as the unsuperposed epilogue produces them.
+// x, y, popX and popY are in the pass's popcount order; permX / permY map a row back to the caller's index, where the
+// counts land and the edges are written (symmetric: as (min, max) of the two, so that still i < j).
 // A block takes 64 consecutive candidates at a time (one coalesced load; the warp that listed them worked on one quarter
 // of a tile row, so their row operands are L1 / L2 hits), a warp one candidate: all of its 128-bit row loads and the two
 // popcount loads are in flight together; edges are parked in 64 shared-memory slots per warp that leave with ONE global
@@ -154,6 +174,7 @@ __global__ void __launch_bounds__(256) verifyCandidatesKernel(const uint32_t* __
                                                              const int2* __restrict__ cand, unsigned long long nCand, int S, int C,
                                                              uint32_t nRows, uint32_t nCols, int symmetric,
                                                              const int32_t* __restrict__ popX, const int32_t* __restrict__ popY,
+                                                             const int32_t* __restrict__ permX, const int32_t* __restrict__ permY,
                                                              const uint16_t* __restrict__ thresh, int sign, int32_t* counts,
                                                              int32_t* countsY, int2* edges, unsigned long long* edgeCursor,
                                                              unsigned long long edgeCap) {
@@ -220,16 +241,22 @@ __global__ void __launch_bounds__(256) verifyCandidatesKernel(const uint32_t* __
       int v = cnt[f];
       for (int o = G >> 1; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
       const bool hit = gl == 0 && live[f] && v >= thresh[popSum[f]];
+      int        i = 0, j = 0;  // the pair in the caller's order
       if (hit) {
-        atomicAdd(counts + iOf[f], sign);
-        if (countsY) atomicAdd(countsY + jOf[f], sign);
+        i = permX[iOf[f]], j = permY[jOf[f]];
+        if (symmetric && i > j) {
+          const int t = i;
+          i = j, j = t;
+        }
+        atomicAdd(counts + i, sign);
+        if (countsY) atomicAdd(countsY + j, sign);
       }
       if (edges) {
         const unsigned hits = __ballot_sync(0xffffffffu, hit);
         if (hits) {
           const int total = __popc(hits);  // <= 16
           if (nStaged + total > kStage) flush();
-          if (hit) stage[warp][nStaged + __popc(hits & ((1u << lane) - 1u))] = make_int2(static_cast<int>(iOf[f]), static_cast<int>(jOf[f]));
+          if (hit) stage[warp][nStaged + __popc(hits & ((1u << lane) - 1u))] = make_int2(i, j);
           nStaged += total;
         }
       }
@@ -237,6 +264,28 @@ __global__ void __launch_bounds__(256) verifyCandidatesKernel(const uint32_t* __
   }
   }
   if (edges) flush();
+}
+
+// The results of an unsuperposed pass over the fingerprints in popcount order, moved to the caller's indices:
+// counts[permX[i]] += countsOrd[i] (a permutation: no two threads meet), and the edges the pass appended to the list
+// ([*start, *end) within its capacity) renamed in place, as (min, max) when symmetric so that still i < j.
+__global__ void mapBackKernel(const int32_t* __restrict__ countsOrd, const int32_t* __restrict__ permX, size_t nX, int32_t* counts,
+                              const int32_t* __restrict__ permY, int symmetric, int2* edges, const unsigned long long* start,
+                              const unsigned long long* end, unsigned long long cap) {
+  const size_t t0 = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x, step = static_cast<size_t>(gridDim.x) * blockDim.x;
+  for (size_t i = t0; i < nX; i += step)
+    if (countsOrd[i]) counts[permX[i]] += countsOrd[i];
+  if (!edges) return;
+  const unsigned long long e1 = min(*end, cap);
+  for (unsigned long long e = *start + t0; e < e1; e += step) {
+    const int2 v = edges[e];
+    int        i = permX[v.x], j = permY[v.y];
+    if (symmetric && i > j) {
+      const int t = i;
+      i = j, j = t;
+    }
+    edges[e] = make_int2(i, j);
+  }
 }
 
 __global__ void recipTableKernel(double* __restrict__ r, int len) {  // r[u] = RN(1 / u), r[0] = 0
@@ -771,6 +820,37 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
 void launchRowPopcount(const uint32_t* fp, size_t n, int words, int32_t* pop, cudaStream_t s);
 void launchThreshTable(int maxS, double cutoff, uint16_t* thresh, cudaStream_t s);
 
+// A fingerprint set in popcount order: row i of fp is the caller's row perm[i], pop its popcount; ascending, ties in the
+// caller's order (CUB's radix sort is stable), so the same input always gives the same order.
+struct PopOrder {
+  Scratch<uint32_t> fp;
+  Scratch<int32_t>  pop, perm;
+};
+static PopOrder popcountOrder(const uint32_t* fp, const int32_t* pop, size_t n, int words, cudaStream_t s) {
+  PopOrder o;
+  o.fp   = Scratch<uint32_t>(n * static_cast<size_t>(words), s);
+  o.pop  = Scratch<int32_t>(n, s);
+  o.perm = Scratch<int32_t>(n, s);
+  Scratch<int32_t> index(n, s);
+  iotaKernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(index.get(), n);
+  B200_LAUNCHED();
+  int endBit = 1;  // popcounts are <= 32 words, non-negative: the low bits of the key are enough
+  while ((1 << endBit) <= 32 * words) ++endBit;
+  size_t tmpBytes = 0;
+  B200_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmpBytes, pop, o.pop.get(), index.get(), o.perm.get(), static_cast<int>(n), 0,
+                                            endBit, s));
+  Scratch<uint8_t> tmp(tmpBytes, s);
+  B200_CUDA(cub::DeviceRadixSort::SortPairs(tmp.get(), tmpBytes, pop, o.pop.get(), index.get(), o.perm.get(), static_cast<int>(n), 0,
+                                            endBit, s));
+  g_launchCount.fetch_add(1);
+  const int    chunks = words / 4;
+  const size_t t      = n * static_cast<size_t>(chunks);
+  gatherRowsKernel<<<static_cast<unsigned>((t + 255) / 256), 256, 0, s>>>(reinterpret_cast<const uint4*>(fp), o.perm.get(), n, chunks,
+                                                                          reinterpret_cast<uint4*>(o.fp.get()));
+  B200_LAUNCHED();
+  return o;
+}
+
 int g_superpose = 4;      // fingerprints summed into one row of the count pass (option "similarity_superpose": 1, 2 or 4)
 int g_superposeCols = 4;  // ... and into one column ("similarity_superpose_cols": 1, 2 or 4); 4 x 4 sums stay <= 16, exact
 int g_superposeLast = 0;  // pairs per accumulator the last graph pass really ran with (1 after an overflow fallback)
@@ -781,8 +861,8 @@ int g_pipelineChunks = 4;  // chunks of a superposed pass whose verification ove
 int g_superposeAuto = 1;  // 1: a large graph pass picks rows x cols from a pilot over one row group ("similarity_superpose_auto")
 unsigned long long g_candidatesLast = 0;  // candidates the last superposed pass listed ("similarity_candidates_last")
 
-static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, int superS, int superC, bool* overflow,
-                             unsigned long long* pilotCand = nullptr);
+static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, int superS, int superC, bool ordered,
+                             bool* overflow, unsigned long long* pilotCand = nullptr);
 
 // Count / materialise modes on tensor cores. Returns false when the problem shape is not eligible (caller uses the SIMT tile).
 bool launchSimilarityTensor(SimMode mode, const SimLaunch& q, cudaStream_t s) {
@@ -792,12 +872,13 @@ bool launchSimilarityTensor(SimMode mode, const SimLaunch& q, cudaStream_t s) {
   const bool graphPass = mode == kCountTanimoto && (q.symmetric || q.edges != nullptr);
   if (!graphPass || g_superpose * g_superposeCols == 1) {
     if (graphPass) g_superposeLast = 1;
-    return launchTensorImpl(mode, q, s, 1, 1, nullptr);
+    return launchTensorImpl(mode, q, s, 1, 1, false, nullptr);
   }
   int S = g_superpose, C = g_superposeCols;
   // How far superposition pays depends on the data: the sum of S C random intersections must stay below the threshold
   // ONE true neighbour pair reaches, or every accumulator is a candidate. A pilot over a prefix sample of the
-  // fingerprints (at most 1/64 of the pairs; candidates listed but nothing counted) measures the candidate rate of each
+  // fingerprints (at most 1/64 of the pairs; candidates listed but nothing counted; launchTensorImpl orders the sample by
+  // popcount as it does the whole set, while a prefix of the whole set's order would hold only its lowest popcounts) measures the candidate rate of each
   // column factor, widest first; the model
   //   time(S, C) = pairs / (S C) * tPair + candidates * S C * tVerify
   // picks the cheapest. A narrower factor can only win while the wider one spends more time verifying than multiplying, so the search stops as soon as it does not.
@@ -812,14 +893,15 @@ bool launchSimilarityTensor(SimMode mode, const SimLaunch& q, cudaStream_t s) {
     const double pilotPairs = q.symmetric ? sX * (sX - 1) / 2.0 : sX * sY;
     const double totalPairs = (q.symmetric ? nX * (nX - 1) / 2.0 : nX * nY) / (q.groupStride < 1 ? 1 : q.groupStride);
     // seconds per unsuperposed pair / per verified pair; only their ratio (about 1 : 30) steers the choice. tPair is the
-    // measured pass: 214 ms for the 5.0e11 pairs of the 1M bench at S C = 8 (H100 SXM, 400 W limit). On the bench data
-    // the pilot then costs 4 x 4 at 0.39 s and 4 x 2 at 0.24 s, and runs 4 x 2.
-    constexpr double tPair = 3.4e-12, tVerify = 0.1e-9;
+    // measured pass: 108-110 ms for the 5.0e11 pairs of the 1M bench at S C = 16 (H100 SXM, 400 W limit). On the bench
+    // data (sample in popcount order) the pilot then costs 4 x 4 at 0.17 s and runs it; tools/pilot_model.py prints
+    // these figures for any fingerprint set without a GPU.
+    constexpr double tPair = 3.5e-12, tVerify = 0.1e-9;
     double bestT = totalPairs * tPair;  // unsuperposed
     int    bestS = 1, bestC = 1;
     for (int c = C; c >= 1; c >>= 1) {
       unsigned long long got = 0;
-      if (!launchTensorImpl(mode, pilot, s, S, c, nullptr, &got)) return false;
+      if (!launchTensorImpl(mode, pilot, s, S, c, true, nullptr, &got)) return false;
       const double tPass = totalPairs / (S * c) * tPair;
       const double tVer  = static_cast<double>(got) * totalPairs / pilotPairs * S * c * tVerify;
       if (tPass + tVer < bestT) bestT = tPass + tVer, bestS = S, bestC = c;
@@ -829,18 +911,23 @@ bool launchSimilarityTensor(SimMode mode, const SimLaunch& q, cudaStream_t s) {
   }
   while (S * C > 1) {
     bool overflow = false;
-    if (!launchTensorImpl(mode, q, s, S, C, &overflow)) return false;
+    if (!launchTensorImpl(mode, q, s, S, C, true, &overflow)) return false;
     g_superposeLast = S * C;
     if (!overflow) return true;  // else: the candidate list overflowed (dense graph / loose cutoff), nothing was counted yet
     if (C > 1) C = 1;            // second chance: rows only
     else S = 1;
   }
+  // The unsuperposed pass that completes a superposed one stays in popcount order: a sharded call's ranks decide their
+  // fallbacks independently, and their row groups must still be groups of ONE order for the union to be every pair once.
   g_superposeLast = 1;
-  return launchTensorImpl(mode, q, s, 1, 1, nullptr);
+  return launchTensorImpl(mode, q, s, 1, 1, true, nullptr);
 }
 
-static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, int superS, int superC, bool* overflow,
-                             unsigned long long* pilotCand) {
+// ordered (graph passes of the count mode): run on the fingerprints in popcount order and map the results back. Every
+// pass of a graph pass with superposition on is ordered, also an unsuperposed fallback (of the whole call, of a rank or
+// of a pipeline chunk): it must cover the same row groups as the superposed pass it replaces or completes.
+static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, int superS, int superC, bool ordered,
+                             bool* overflow, unsigned long long* pilotCand) {
   if (mode == kCountCosine) return false;
   const int bits = q.words * 32;
   if (bits % kTK != 0 || bits > 4096) return false;
@@ -851,6 +938,7 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
   const int  rowBytes = bits;  // one byte per bit of the fingerprint
   if (!count) superS = superC = 1;  // only the count mode verifies
   const bool   super  = superS * superC > 1;
+  ordered             = count && (ordered || super);  // (a superposed pass is always ordered)
   const size_t nSuper = (q.nX + superS - 1) / superS;   // rows of the X operand
   const size_t nSuperY = (q.nY + superC - 1) / superC;  // rows of the Y operand (tile columns)
 
@@ -893,6 +981,36 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
     if (p.alpha < 0.0f) p.alpha = 0.0f;
   }
 
+  Scratch<int32_t> popX(q.nX, s), popYown(same ? 0 : q.nY, s);
+  launchRowPopcount(q.x, q.nX, q.words, popX.get(), s);
+  if (!same) launchRowPopcount(q.y, q.nY, q.words, popYown.get(), s);
+  // A superposed pass runs on the fingerprints ordered by popcount (a stable sort: ties keep the caller's order, so every
+  // rank of a sharded pass builds the same order). The S (C) fingerprints summed into one operand row then have nearly
+  // the same popcount, and the pre-filter, which must assume the group's smallest, sits at the members' own threshold
+  // instead of about a standard deviation below it. Row groups, pipeline chunks and rank ownership all live in this
+  // order; the verification maps each pair back (permX / permY). An unsuperposed pass in this order counts and lists
+  // edges in it, and mapBackKernel moves its results to the caller's indices.
+  PopOrder       ordX, ordYown;
+  const uint32_t *fx = q.x, *fy = q.y;
+  const int32_t * popXs = popX.get(), *popYs = same ? popX.get() : popYown.get(), *permX = nullptr, *permY = nullptr;
+  if (ordered) {
+    ordX = popcountOrder(q.x, popX.get(), q.nX, q.words, s);
+    if (!same) ordYown = popcountOrder(q.y, popYown.get(), q.nY, q.words, s);
+    const PopOrder& ordY = same ? ordX : ordYown;
+    fx = ordX.fp.get(), fy = ordY.fp.get();
+    popXs = ordX.pop.get(), popYs = ordY.pop.get();
+    permX = ordX.perm.get(), permY = ordY.perm.get();
+  }
+  const bool                  mapBack = ordered && !super;
+  Scratch<int32_t>            countsOrd(mapBack ? q.nX : 0, s);
+  Scratch<unsigned long long> edgeStart(mapBack && q.edges ? 1 : 0, s);
+  if (mapBack) {
+    B200_CUDA(cudaMemsetAsync(countsOrd.get(), 0, q.nX * sizeof(int32_t), s));
+    p.counts  = countsOrd.get();
+    p.countsY = q.symmetric ? countsOrd.get() : nullptr;
+    if (q.edges) B200_CUDA(cudaMemcpyAsync(edgeStart.get(), q.edgeCursor, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, s));
+  }
+
   // 0/1 expansion of the fingerprints (2 KB per 2048-bit row); a superposed operand is the sum of superS (superC)
   // consecutive expansions. X and Y share one buffer when they are the same set, summed alike.
   const bool       ownY = !same || superS != superC;
@@ -905,22 +1023,18 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
     else expandBitsKernel<<<grid, 256, 0, s>>>(src, nw, reinterpret_cast<uint4*>(dst));
     B200_LAUNCHED();
   };
-  expand(q.x, q.nX, superS, nSuper, expX.get());
-  if (ownY) expand(q.y, q.nY, superC, nSuperY, expYown.get());
+  expand(fx, q.nX, superS, nSuper, expX.get());
+  if (ownY) expand(fy, q.nY, superC, nSuperY, expYown.get());
   const uint8_t* expY = ownY ? expYown.get() : expX.get();
 
-  Scratch<int32_t> popX(q.nX, s), popYown(same ? 0 : q.nY, s);
-  launchRowPopcount(q.x, q.nX, q.words, popX.get(), s);
-  if (!same) launchRowPopcount(q.y, q.nY, q.words, popYown.get(), s);
-  const int32_t* popYExact = same ? popX.get() : popYown.get();
   // the epilogue's per-row metadata of both operands, padded to whole tiles for the producer's bulk copies (the lower
   // tile of a CTA pair may lie one tile row past the end)
   const size_t  rowsPad = (static_cast<size_t>(p.tilesM) + 1) * kTM, colsPad = static_cast<size_t>(p.tilesN) * kTN;
   Scratch<int2> rowMeta(rowsPad, s), colMeta(colsPad, s);
-  tileMetaKernel<<<static_cast<unsigned>((rowsPad + 255) / 256), 256, 0, s>>>(popX.get(), q.nX, superS, nSuper, rowsPad, p.alpha, 1,
+  tileMetaKernel<<<static_cast<unsigned>((rowsPad + 255) / 256), 256, 0, s>>>(popXs, q.nX, superS, nSuper, rowsPad, p.alpha, 1,
                                                                              rowMeta.get());
   B200_LAUNCHED();
-  tileMetaKernel<<<static_cast<unsigned>((colsPad + 255) / 256), 256, 0, s>>>(popYExact, q.nY, superC, nSuperY, colsPad, p.alpha, -1,
+  tileMetaKernel<<<static_cast<unsigned>((colsPad + 255) / 256), 256, 0, s>>>(popYs, q.nY, superC, nSuperY, colsPad, p.alpha, -1,
                                                                              colMeta.get());
   B200_LAUNCHED();
   p.rowMeta = rowMeta.get();
@@ -1008,8 +1122,8 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
   auto launchVerify = [&](const int2* list, unsigned long long nCand, cudaStream_t on) {
     PhaseTimer         t("verify_candidates", on);
     const unsigned int blocks2 = static_cast<unsigned int>(std::min<unsigned long long>((nCand + 63) / 64, static_cast<unsigned long long>(smCount()) * 16));
-    verifyCandidatesKernel<<<blocks2, 256, 0, on>>>(q.x, q.y, q.words, list, nCand, superS, superC, static_cast<uint32_t>(q.nX),
-                                                    static_cast<uint32_t>(q.nY), q.symmetric ? 1 : 0, popX.get(), popYExact,
+    verifyCandidatesKernel<<<blocks2, 256, 0, on>>>(fx, fy, q.words, list, nCand, superS, superC, static_cast<uint32_t>(q.nX),
+                                                    static_cast<uint32_t>(q.nY), q.symmetric ? 1 : 0, popXs, popYs, permX, permY,
                                                     thresh.get(), q.sign, q.rowCounts, q.symmetric ? q.rowCounts : nullptr, q.edges,
                                                     q.edgeCursor, q.edgeCap);
     B200_LAUNCHED();
@@ -1064,8 +1178,8 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
       qk.groupOffset = p.groupOffset + static_cast<uint32_t>(redo[r]) * p.groupStride;
       qk.groupStride = static_cast<uint32_t>(K) * p.groupStride;
       bool again     = false;
-      if (!launchTensorImpl(mode, qk, s, superS, 1, &again)) return false;
-      if (again && !launchTensorImpl(mode, qk, s, 1, 1, nullptr)) return false;
+      if (!launchTensorImpl(mode, qk, s, superS, 1, true, &again)) return false;
+      if (again && !launchTensorImpl(mode, qk, s, 1, 1, true, nullptr)) return false;
     }
     return true;
   }
@@ -1074,8 +1188,16 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
   int blocks = smCount();
   if (static_cast<uint64_t>(blocks) > unitsOf(p)) blocks = static_cast<int>(unitsOf(p));
   if (mode == kCountTanimoto) {
-    PhaseTimer t("neighbor_pass_tc", s);
-    launchCount(p);
+    {
+      PhaseTimer t("neighbor_pass_tc", s);
+      launchCount(p);
+    }
+    if (mapBack) {
+      const unsigned grid = static_cast<unsigned>(std::min<size_t>((q.nX + 255) / 256, static_cast<size_t>(smCount()) * 8));
+      mapBackKernel<<<grid, 256, 0, s>>>(countsOrd.get(), permX, q.nX, q.rowCounts, permY, p.symmetric, q.edges, edgeStart.get(),
+                                         q.edgeCursor, q.edgeCap);
+      B200_LAUNCHED();
+    }
   } else if (mode == kMaterialiseTanimoto) {
     PhaseTimer t("cross_tc", s);
     simTensorKernel<kTcTanimoto, 0><<<blocks, kThreadsTC, smemBytes, s>>>(tmA, tmB, p);
