@@ -52,7 +52,7 @@ SIGNATURES = {
     "b200mol_etk_minimize": (C.c_int, [_vp, C.c_int, C.c_int, C.c_int32, _vp, _vp, C.c_int, _vp, C.c_int, C.c_double, _vp, _vp,
                                        _vp, _vp, _vp]),
     "b200mol_poly_minimize": (C.c_int, [C.c_int32, _vp, C.c_int, C.c_int, _vp, _vp, _vp, C.c_int, C.c_double, C.c_int,
-                                        _vp, _vp, _vp, _vp]),
+                                        C.c_int, _vp, _vp, _vp, _vp]),
     "b200mol_etkdg_embed": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int32, _vp, _vp, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp]),
     "b200mol_etkdg_initial_coords": (C.c_int, [_vp, _vp, C.c_int32, _vp, _vp, C.c_int, C.c_int32, _vp, _vp, _vp]),
     "b200mol_etkdg_check": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int32, _vp, _vp, C.c_int, _vp, _vp, _vp]),

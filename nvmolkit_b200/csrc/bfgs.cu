@@ -46,21 +46,24 @@ struct Batch {
   double*        energy;
   int8_t*        status;
   int32_t*       iters;
-  double*        hessWs;
+  void*          hessWs;  // inverse-Hessian slabs of the kernel's storage type HT
   size_t         hessStride;
   int*           queue;
   int            maxN;
   unsigned long long* stats;
 };
 
-template <class FF>
+// HT = storage type of the inverse-Hessian slab: double for the force fields, float as well for the analytic test
+// systems (the embedder's default type, bfgs_device.cuh)
+template <class FF, class HT>
 __global__ void __launch_bounds__(kT, kMinCtas) bfgsKernel(const typename FF::System sys, const typename FF::Params par, const Batch b) {
   extern __shared__ __align__(16) double sm[];
   __shared__ double                     red[kRed];
   __shared__ double                     colBuf[kColBuf];
   __shared__ int                        nextConf;
   constexpr int                         DIM = FF::kDim;
-  const BfgsWork w = carveWork(sm, b.maxN, b.hessWs + static_cast<size_t>(blockIdx.x) * b.hessStride, red, colBuf, b.stats);
+  const BfgsWorkT<HT> w =
+      carveWork<HT>(sm, b.maxN, static_cast<HT*>(b.hessWs) + static_cast<size_t>(blockIdx.x) * b.hessStride, red, colBuf, b.stats);
   const int      tid = threadIdx.x;
   for (;;) {
     __syncthreads();
@@ -83,7 +86,7 @@ __global__ void __launch_bounds__(kT, kMinCtas) bfgsKernel(const typename FF::Sy
       }
     }
     __syncthreads();
-    const BfgsOutcome o = bfgsMinimize<FF>(view, w, n, b.maxIters, b.gradTol, b.scaleGrads != 0, b.maxRestarts);
+    const BfgsOutcome o = bfgsMinimize<FF, HT>(view, w, n, b.maxIters, b.gradTol, b.scaleGrads != 0, b.maxRestarts);
     for (int i = tid; i < n; i += kT) gpos[i] = w.pos[i];
     if (tid == 0) {
       b.energy[conf] = o.energy;
@@ -123,7 +126,7 @@ __global__ void __launch_bounds__(kT) energyGradKernel(const typename FF::System
   }
 }
 
-template <class FF>
+template <class FF, class HT = double>
 void runMinimize(const typename FF::System& sys, const typename FF::Params& par, int nConf, const int32_t* confMol,
                  const int32_t* confAtomStart, int maxAtoms, double* pos, int maxIters, double gradTol, int scaleGrads,
                  const uint8_t* active, double* energy, int8_t* status, int32_t* iters, cudaStream_t s) {
@@ -136,24 +139,24 @@ void runMinimize(const typename FF::System& sys, const typename FF::Params& par,
   B200_REQUIRE(smem <= 200 * 1024, "molecule too large for the shared-memory BFGS (%d atoms)", maxAtoms);
   static bool configured[kMaxDevices] = {};  // per instantiation and device; static + dynamic may pass 48 KB together
   if (!configured[currentDeviceSlot()]) {
-    B200_CUDA(cudaFuncSetAttribute(bfgsKernel<FF>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    B200_CUDA(cudaFuncSetAttribute(bfgsKernel<FF, HT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     configured[currentDeviceSlot()] = true;
   }
   int perSm = 0;
-  B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, bfgsKernel<FF>, kT, smem));
+  B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, bfgsKernel<FF, HT>, kT, smem));
   B200_REQUIRE(perSm >= 1, "BFGS kernel does not fit");
   perSm            = perSm > g_bfgsCtasPerSm ? g_bfgsCtasPerSm : perSm;
   int blocks       = smCount() * perSm;
   if (blocks > nConf) blocks = nConf;
-  const size_t       stride = static_cast<size_t>(maxN) * bfgsLd<double>(maxN);
-  Scratch<double>    hess(stride * blocks, s);
+  const size_t       stride = static_cast<size_t>(maxN) * bfgsLd<HT>(maxN);
+  Scratch<HT>        hess(stride * blocks, s);
   Scratch<int>       queue(1, s);
   B200_CUDA(cudaMemsetAsync(queue.get(), 0, sizeof(int), s));
   Batch b{nConf, confMol, confAtomStart, pos, maxIters, gradTol, scaleGrads, 0, active, energy, status, iters,
           hess.get(), stride, queue.get(), maxN, pathBStats() + kStatCount};
-  L2Persist  keep(s, hess.get(), stride * blocks * sizeof(double), g_bfgsL2Persist != 0);
+  L2Persist  keep(s, hess.get(), stride * blocks * sizeof(HT), g_bfgsL2Persist != 0);
   PhaseTimer t("bfgs", s);
-  bfgsKernel<FF><<<blocks, kT, smem, s>>>(sys, par, b);
+  bfgsKernel<FF, HT><<<blocks, kT, smem, s>>>(sys, par, b);
   B200_LAUNCHED();
 }
 
@@ -295,12 +298,16 @@ extern "C" int b200mol_etk_minimize(const b200mol_etk_system* sys, int plain, in
 }
 extern "C" int b200mol_poly_minimize(int32_t nSys, const int32_t* d_starts, int max_dim, int power, const double* d_w,
                                      const double* d_c, double* d_x, int max_iters, double grad_tol, int scale_grads,
-                                     double* d_energy, int8_t* d_status, int32_t* d_iters, void* stream) {
+                                     int hessian_fp32, double* d_energy, int8_t* d_status, int32_t* d_iters, void* stream) {
   return guarded([&] {
     B200_REQUIRE(power == 2 || power == 4, "power must be 2 or 4");
     ff::Poly::System sys{power, d_w, d_c, d_starts};
-    runMinimize<ff::Poly>(sys, {}, nSys, nullptr, d_starts, max_dim, d_x, max_iters, grad_tol, scale_grads, nullptr, d_energy,
-                          d_status, d_iters, asStream(stream));
+    if (hessian_fp32)
+      runMinimize<ff::Poly, float>(sys, {}, nSys, nullptr, d_starts, max_dim, d_x, max_iters, grad_tol, scale_grads, nullptr,
+                                   d_energy, d_status, d_iters, asStream(stream));
+    else
+      runMinimize<ff::Poly, double>(sys, {}, nSys, nullptr, d_starts, max_dim, d_x, max_iters, grad_tol, scale_grads, nullptr,
+                                    d_energy, d_status, d_iters, asStream(stream));
   });
 }
 

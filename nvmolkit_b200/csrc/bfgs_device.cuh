@@ -114,7 +114,9 @@ __device__ void gradOf(const typename FF::View& v, const double* x, double* acc,
 //                   gradient), acc[1] = hdg (H * dGrad), acc[2] = newPos (trial point / H * grad): each of the three is
 //                   dead while the gradient is being accumulated, so only kWarps - 3 vectors are extra
 // HT = storage type of the inverse Hessian: double (default; bit-for-bit the RDKit recurrence) or float (half the slab
-// traffic, products and sums still accumulate in fp64) for the embedding stages whose trajectories are chaotic anyway.
+// traffic) for the embedding stages whose trajectories are chaotic anyway. The sweep computes in HT: with float the
+// rank-2 update, the products, the per-lane column partials, the row sums and their butterfly are fp32; only the
+// cross-warp column reduction and the accumulated H*dGrad / H*grad are fp64.
 template <class HT = double>
 struct BfgsWorkT {
   double *pos, *grad, *dir, *newPos, *dGrad, *hdg;  // shared memory, maxN each

@@ -45,8 +45,8 @@ struct EmbedArgs {
   int32_t*                attempts;       // [nSlots]
   double*                 energy;         // [nSlots] DG energy (first-stage weights) of the accepted attempt
   unsigned long long*     stageFailures;  // [kNumStages] (may be NULL)
-  void*                   hessWs;  // inverse-Hessian slabs: fp32 by default (fp64 accumulation; half the traffic), fp64 with
-                                   // option "etkdg_hessian_fp64" (the reference's storage type)
+  void*                   hessWs;  // inverse-Hessian slabs: fp32 by default (swept in fp32, bfgs_device.cuh; half the
+                                   // traffic), fp64 with option "etkdg_hessian_fp64" (the reference's storage type)
   size_t                  hessStride;
   int*                    queue;
   int                     maxN;

@@ -405,7 +405,7 @@ void launchSimilarity(SimMode mode, const SimLaunch& q, cudaStream_t s) {
 using namespace b200;
 
 extern "C" const char* b200mol_last_error(void) { return g_lastError.c_str(); }
-extern "C" int         b200mol_abi_version(void) { return 1; }
+extern "C" int         b200mol_abi_version(void) { return 2; }
 extern "C" uint64_t    b200mol_launch_count(void) { return g_launchCount.load(); }
 
 extern "C" int b200mol_profile_enable(int on) {

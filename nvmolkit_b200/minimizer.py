@@ -97,8 +97,10 @@ def energy_and_grad(system: FlatSystem, batch: ConformerBatch, want_grad: bool =
 
 
 def poly_minimize(starts: np.ndarray, power: int, w: np.ndarray, c: np.ndarray, x0: np.ndarray, max_iters: int,
-                  grad_tol: float, scale_grads: bool, stream=None):
-    """Analytic test systems E = sum w (x - c)^power driven through the same BFGS kernel (tests)."""
+                  grad_tol: float, scale_grads: bool, stream=None, *, hessian_fp32: bool = False):
+    """Analytic test systems E = sum w (x - c)^power driven through the same BFGS kernel (tests).
+
+    `hessian_fp32`: keep the inverse Hessian in fp32, the embedder's default slab type (fp64 otherwise, like MMFF / UFF)."""
     sptr = stream_ptr(stream)
     require_cuda()
     dev = torch.device("cuda", torch.cuda.current_device())
@@ -112,6 +114,6 @@ def poly_minimize(starts: np.ndarray, power: int, w: np.ndarray, c: np.ndarray, 
         status = torch.ones(n, dtype=torch.int8, device=dev)
         iters = torch.zeros(n, dtype=torch.int32, device=dev)
         _lib.call("b200mol_poly_minimize", n, d_starts.data_ptr(), int(np.diff(starts).max()), int(power), d_w.data_ptr(),
-                  d_c.data_ptr(), d_x.data_ptr(), int(max_iters), float(grad_tol), 1 if scale_grads else 0, e.data_ptr(),
-                  status.data_ptr(), iters.data_ptr(), sptr)
+                  d_c.data_ptr(), d_x.data_ptr(), int(max_iters), float(grad_tol), 1 if scale_grads else 0,
+                  1 if hessian_fp32 else 0, e.data_ptr(), status.data_ptr(), iters.data_ptr(), sptr)
     return d_x, e, status, iters

@@ -47,17 +47,24 @@ def test_bfgs_quartic_and_harmonic(cuda):
 def test_mmff_energy_and_gradient_parity(cuda):
     from nvmolkit_b200.minimizer import energy_and_grad
 
-    system, xyz, _ = S.random_mmff_system(12, 4, 40, seed=21)
+    system, xyz, mols = S.random_mmff_system(12, 4, 40, seed=21)
     rng = np.random.default_rng(0)
     coords = [[x + rng.normal(0, 0.05, x.shape), x + rng.normal(0, 0.2, x.shape)] for x in xyz]
-    batch = ConformerBatch.from_coords(system, coords)
-    e, g = energy_and_grad(system, batch)
-    e, g = e.cpu().numpy(), g.cpu().numpy()
-    for c in range(batch.n_conf):
-        a0, a1 = batch.atom_starts[c], batch.atom_starts[c + 1]
-        eo, go, _ = oracle.ff_energy_grad("mmff", system.atom_counts, system.tables, batch.conf_mol[c], batch.positions[a0:a1])
-        assert _rel(e[c], eo) < 1e-11
-        assert np.abs(g[a0:a1] - go).max() < 1e-9 * max(1.0, np.abs(go).max())
+    # the same batch again with one molecule near the energy kernel's 948-atom limit among the small ones
+    _, xyz_l, mols_l = S.random_mmff_system(1, 440, 450, seed=42)
+    assert len(mols_l[0]["z"]) == 895
+    mols_b = mols[:6] + mols_l + mols[6:]
+    system_b = FlatSystem.from_molecules("mmff", [len(m["z"]) for m in mols_b], [m["terms"] for m in mols_b])
+    coords_b = coords[:6] + [[x + rng.normal(0, 0.05, x.shape), x + rng.normal(0, 0.2, x.shape)] for x in xyz_l] + coords[6:]
+    for system, coords in ((system, coords), (system_b, coords_b)):
+        batch = ConformerBatch.from_coords(system, coords)
+        e, g = energy_and_grad(system, batch)
+        e, g = e.cpu().numpy(), g.cpu().numpy()
+        for c in range(batch.n_conf):
+            a0, a1 = batch.atom_starts[c], batch.atom_starts[c + 1]
+            eo, go, _ = oracle.ff_energy_grad("mmff", system.atom_counts, system.tables, batch.conf_mol[c], batch.positions[a0:a1])
+            assert _rel(e[c], eo) < 1e-11, (len(system.atom_counts), c)
+            assert np.abs(g[a0:a1] - go).max() < 1e-9 * max(1.0, np.abs(go).max())
 
 
 def test_dg_and_etk_energy_and_gradient_parity(cuda):
