@@ -61,6 +61,9 @@ int b200mol_free_async(void* d_ptr, void* stream);
  *                                  sample per column factor and keeps the factor a cost model finds cheapest (the
  *                                  sum of rows x cols random intersections must stay below one true pair's threshold);
  *                                  0: always start from the configured factors
+ *   "similarity_popcount_band"     1 (default): a neighbour pass in popcount order (superposed, its fallbacks, the
+ *                                  pilot) skips, per row group of 8,192 fingerprints, the tile columns whose popcounts
+ *                                  no row of the group can reach a neighbour with; 0: visits them. Results identical
  *   "butina_min_round_commits"     a parallel Butina round that commits fewer clusters than this hands over to the
  *                                  one-cluster-per-step loop (default 32; 0 = rounds only, >= 1e9 = stepwise only)
  *   "etkdg_hessian_fp64"           0 (default): the embedder keeps its BFGS inverse Hessian in fp32 and sweeps it in fp32
@@ -72,7 +75,10 @@ int b200mol_free_async(void* d_ptr, void* stream);
  *                                  budget they are compiled for) */
 int b200mol_set_option(const char* key, long long value);
 /* Current value of an option; also "similarity_superpose_last": pairs per accumulator the last neighbour pass really ran with
- * (1 after a candidate-list overflow made it fall back), and "similarity_candidates_last": how many candidates it listed. */
+ * (1 after a candidate-list overflow made it fall back), "similarity_candidates_last": how many candidates it listed, and
+ * what the tensor-core count passes of the last neighbour pass walked after its pilot: "similarity_units_planned_last"
+ * (work units the host sized the grids for), "similarity_units_last" and "similarity_tiles_last" (units and tiles the
+ * kernels counted; these two synchronise the device). */
 int b200mol_get_option(const char* key, long long* value);
 /* Per-phase CUDA-event timing inside the library (off by default). Phases: "neighbor_pass" (the N^2 tile kernel
  * alone), "csr_build", "cluster_loop", "bfgs". b200mol_profile_read waits for the phase's stop event. */

@@ -314,6 +314,9 @@ extern int g_superposeCols;
 extern int g_superposeAuto;
 extern int g_pipelineChunks;
 extern unsigned long long g_candidatesLast;
+extern int g_popcountBand;
+extern unsigned long long g_unitsPlanned;
+void readWalkCounters(unsigned long long* units, unsigned long long* tiles);
 long long g_tensorMinPairs = 1ll << 24;  // pair count from which the passes run on the tensor-core tile (< 0: never)
 
 void launchThreshTable(int maxS, double cutoff, uint16_t* thresh, cudaStream_t s) {
@@ -447,6 +450,7 @@ extern "C" int b200mol_set_option(const char* key, long long value) {
       B200_REQUIRE(value >= 1 && value <= 8, "similarity_pipeline_chunks must be in [1, 8]");
       g_pipelineChunks = static_cast<int>(value);
     }
+    else if (k == "similarity_popcount_band") g_popcountBand = value != 0;
     else if (k == "similarity_tensor_cluster") {
       B200_REQUIRE(value >= 0 && value <= 3, "similarity_tensor_cluster must be 0, 1, 2 or 3");
       g_tensorCluster = static_cast<int>(value);
@@ -474,6 +478,13 @@ extern "C" int b200mol_get_option(const char* key, long long* value) {
     else if (k == "similarity_pipeline_chunks") *value = g_pipelineChunks;
     else if (k == "similarity_candidates_last") *value = static_cast<long long>(g_candidatesLast);
     else if (k == "similarity_superpose_last") *value = g_superposeLast;  // read-only: pairs per accumulator of the last pass
+    else if (k == "similarity_popcount_band") *value = g_popcountBand;
+    else if (k == "similarity_units_planned_last") *value = static_cast<long long>(g_unitsPlanned);  // read-only
+    else if (k == "similarity_units_last" || k == "similarity_tiles_last") {  // read-only; synchronises the device
+      unsigned long long units = 0, tiles = 0;
+      readWalkCounters(&units, &tiles);
+      *value = static_cast<long long>(k == "similarity_units_last" ? units : tiles);
+    }
     else if (k == "butina_min_round_commits") *value = g_butinaMinCommits;
     else fail(B200MOL_ERR_INVALID, "unknown option '%s'", key);
   });

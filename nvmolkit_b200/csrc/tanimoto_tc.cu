@@ -30,6 +30,7 @@
 // Replaces crossSimilarityKernelTensorOp (src/similarity_kernels.cu:104-240) + the Triton count kernel
 // (nvmolkit/_fusedButina.py:99-179) for the fused Butina pass.
 #include <cub/device/device_radix_sort.cuh>
+#include <vector>
 
 #include "profile.cuh"
 #include "similarity.cuh"
@@ -85,7 +86,19 @@ struct TcParams {
   int2*               cand;
   unsigned long long* candCursor;
   unsigned long long  candCap;
+  // Popcount band (ordered count passes; nullptr elsewhere): per row group, the end of the tile columns that can hold a
+  // neighbour of any of its rows (popcountBandKernel). The walk skips the tile columns at and past it.
+  const uint32_t*     bandEnd;
+  unsigned long long* walked;  // [0] += units walked (once per CTA pair), [1] += tiles a CTA ran; nullptr: not counted
 };
+
+// The popcount band. A pair with popcounts a, b and intersection c <= min(a, b) can only be a neighbour if
+// c >= thresh[a + b]. thresh is not monotone where no pair reaches a sum (0xFFFF at s < 2, and at small odd s for small
+// cutoffs), so the band tests its suffix minimum tmin[s] = min over s' >= s of thresh[s']: tmin[A + b] > A says that no
+// column of popcount b' >= b can be a neighbour of a row of popcount A, and then none of a row of popcount a <= A either
+// (tests/test_pair_pass_popcount_band_gpu.py checks both against the fp64 predicate for every pair up to 4096 bits). For a
+// row group whose largest popcount is A, no column past the first one this cuts can be a neighbour of any of its rows.
+__host__ __device__ __forceinline__ bool bandCuts(const uint16_t* tmin, int A, int b) { return tmin[A + b] > A; }
 
 enum TcMode : int { kTcCount = 0, kTcTanimoto = 1, kTcCosine = 2 };
 }  // namespace
@@ -288,6 +301,40 @@ __global__ void mapBackKernel(const int32_t* __restrict__ countsOrd, const int32
   }
 }
 
+// The popcount band of an ordered count pass, in one block: the suffix minimum of thresh (len entries) into shared
+// memory, then one thread per row group of kGroupRows fingerprints. popX and popY are in the pass's (ascending) order, so
+// the group's largest popcount is its last row's, and bandCuts is monotone along popY: a bisection finds the first column
+// jCut it cuts. Tile columns at or past ceil(jCut / colSpan) hold no neighbour of the group, whatever the superposition.
+constexpr int kBandThreads = 128;
+__global__ void __launch_bounds__(kBandThreads) popcountBandKernel(const int32_t* __restrict__ popX, size_t nX,
+                                                                   const int32_t* __restrict__ popY, size_t nY,
+                                                                   const uint16_t* __restrict__ thresh, int len, uint32_t colSpan,
+                                                                   uint32_t tilesN, uint32_t groups, uint32_t* __restrict__ bandEnd) {
+  extern __shared__ uint16_t tmin[];
+  __shared__ uint16_t carry[kBandThreads + 1];
+  const int t = threadIdx.x, per = (len + kBandThreads - 1) / kBandThreads, i0 = t * per, i1 = min(len, i0 + per);
+  uint16_t  m = 0xFFFF;
+  for (int i = i1 - 1; i >= i0; --i) tmin[i] = m = min(m, thresh[i]);  // the suffix minimum within this thread's slice
+  carry[t] = m;
+  if (t == 0) carry[kBandThreads] = 0xFFFF;
+  __syncthreads();
+  if (t == 0)
+    for (int k = kBandThreads - 1; k >= 0; --k) carry[k] = min(carry[k], carry[k + 1]);
+  __syncthreads();
+  for (int i = i0; i < i1; ++i) tmin[i] = min(tmin[i], carry[t + 1]);  // ... and past it
+  __syncthreads();
+  for (uint32_t g = t; g < groups; g += kBandThreads) {
+    const int A  = popX[min(nX, (static_cast<size_t>(g) + 1) * kGroupRows) - 1];
+    size_t    lo = 0, hi = nY;
+    while (lo < hi) {
+      const size_t mid = (lo + hi) / 2;
+      if (bandCuts(tmin, A, popY[mid])) hi = mid;
+      else lo = mid + 1;
+    }
+    bandEnd[g] = static_cast<uint32_t>(min(static_cast<size_t>(tilesN), (lo + colSpan - 1) / colSpan));
+  }
+}
+
 __global__ void recipTableKernel(double* __restrict__ r, int len) {  // r[u] = RN(1 / u), r[0] = 0
   const int u = blockIdx.x * blockDim.x + threadIdx.x;
   if (u <= len) r[u] = u ? __drcp_rn(static_cast<double>(u)) : 0.0;
@@ -409,8 +456,11 @@ __device__ unsigned long long g_tcClk[8];
 // RUN > 1 (the row-stationary tile, CL = 3): a unit is a RUN of consecutive tile columns of one unit row - the row
 // operand is loaded once per unit and stays in shared memory - and the units of a group go chunk-major (all rows of the
 // group take column chunk q, then q + 1): the CTA pairs of a group stream the same column tiles at about the same time.
+// In an ordered pass a group also ends at its popcount band (p.bandEnd): the tile columns past it hold no neighbour of
+// any of its rows. The band is per group, so the rule that the upper tile of a pair decides for both still holds.
 // Ownership is serpentine over cycles of `groupStride` groups (even cycles: group = cycle * stride + offset, odd
-// cycles mirrored), which balances the triangle's shrinking rows across ranks to < 0.1 %.
+// cycles mirrored), which balances the triangle's shrinking rows across ranks to < 0.1 % (with the band on the bench
+// data: tools/pilot_model.py prints the ranks' shares).
 // A CTA walks units first, first + step, ... of the concatenated owned groups; (cycle, index in group) are kept
 // incrementally, the only divisions are by compile-time constants and happen once per group.
 template <bool PAIR, int RUN = 1>
@@ -437,13 +487,17 @@ struct UnitWalk {
         // first tile column holding a pair with row < col for the group's top tile row tm0 = group * groupTiles:
         // (tn + 1) * colSpan - 1 > tm0 * rowSpan   (rowSpan / colSpan = fingerprints per tile row / tile column)
         tn0   = p.symmetric ? (group * p.groupTiles * p.rowSpan + 1u) / p.colSpan : 0u;
-        if (tn0 < p.tilesN) units = gRows * ((p.tilesN - tn0 + RUN - 1) / RUN);
+        const uint32_t tnLim = limit(p);
+        if (tn0 < tnLim) units = gRows * ((tnLim - tn0 + RUN - 1) / RUN);
       }
       if (inGroup < units) return;
       inGroup -= units;
       ++cycle;
     }
   }
+  // the end of the group's tile columns: its popcount band, if the pass has one (read again per unit rather than kept in
+  // a register: the consumers' 128 accumulators leave none to spare)
+  __device__ uint32_t limit(const TcParams& p) const { return p.bandEnd ? min(p.tilesN, __ldg(p.bandEnd + group)) : p.tilesN; }
   __device__ void next(const TcParams& p) {
     inGroup += step;
     if (inGroup >= units) {
@@ -463,7 +517,7 @@ struct UnitWalk {
       col = inGroup / gRows;
     }
     tnBeg              = tn0 + col * RUN;
-    tnEnd              = min(p.tilesN, tnBeg + RUN);
+    tnEnd              = RUN == 1 ? tnBeg + 1 : min(limit(p), tnBeg + RUN);  // (a unit of one column lies inside the limit)
     const uint32_t tr  = group * G + row;  // unit row
     const uint32_t top = PAIR ? 2 * tr : tr;
     // the upper tile decides for both CTAs of a pair (if it has no pair with row < col, neither has the lower one); a
@@ -476,9 +530,9 @@ struct UnitWalk {
   }
 };
 
-// host twin of the walk's unit count (sizes the grid)
+// host twin of the walk's unit count (sizes the grid); band = the host copy of p.bandEnd (nullptr when p has none)
 template <bool PAIR, int RUN = 1>
-uint64_t countUnits(const TcParams& p) {
+uint64_t countUnits(const TcParams& p, const uint32_t* band) {
   const uint32_t G        = PAIR ? p.groupTiles / 2 : p.groupTiles;
   const uint32_t unitRows = PAIR ? (p.tilesM + 1) / 2 : p.tilesM;
   uint64_t       total    = 0;
@@ -487,7 +541,8 @@ uint64_t countUnits(const TcParams& p) {
     if (static_cast<uint64_t>(group) * G >= unitRows) continue;
     const uint32_t gRows = std::min(G, unitRows - group * G);
     const uint32_t tn0   = p.symmetric ? (group * p.groupTiles * p.rowSpan + 1u) / p.colSpan : 0u;
-    if (tn0 < p.tilesN) total += static_cast<uint64_t>(gRows) * ((p.tilesN - tn0 + RUN - 1) / RUN);
+    const uint32_t tnLim = band ? std::min(p.tilesN, band[group]) : p.tilesN;
+    if (tn0 < tnLim) total += static_cast<uint64_t>(gRows) * ((tnLim - tn0 + RUN - 1) / RUN);
   }
   return total;
 }
@@ -517,6 +572,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
   __shared__ __align__(16) int2 colMeta[2][kTN];
   __shared__ __align__(16) int2 rowMeta[2][kTM];
   __shared__ int2 pairSlots[COUNT ? 8 : 1][COUNT ? kStagePairs : 1];  // count mode: each epilogue warp's PairStage
+  __shared__ uint32_t walkCount[2];  // units the producer walked, tiles it ran (in shared memory: no register to spare)
 
   const uint32_t rank      = CL ? clusterCtaRank() : 0u;
   const uint32_t firstUnit = CL ? blockIdx.x / 2 : blockIdx.x, unitStep = CL ? gridDim.x / 2 : gridDim.x;
@@ -529,6 +585,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
 #endif
 
   if (threadIdx.x == 0) {
+    walkCount[0] = walkCount[1] = 0;
     tmaPrefetchDesc(&tmA);
     tmaPrefetchDesc(&tmB);
     for (int s = 0; s < kStg; ++s) {
@@ -557,7 +614,9 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
       uint32_t phase = 0, aPhase = 0, metaPhase = 0;
       for (Walk w(p, firstUnit, unitStep); !w.done; w.next(p)) {
         uint32_t tm, tnBeg, tnEnd;
+        atomicAdd(&walkCount[0], 1u);
         if (!w.coords(p, rank, tm, tnBeg, tnEnd)) continue;
+        atomicAdd(&walkCount[1], tnEnd - tnBeg);
         for (uint32_t tn = tnBeg; tn < tnEnd; ++tn) {
           mbarWait(&metaEmpty[meta], metaPhase ^ 1);
           mbarExpectTx(&metaFull[meta], (kTN + kTM) * sizeof(int2));
@@ -597,6 +656,10 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
           }
         }
         aPhase ^= 1;
+      }
+      if (p.walked) {  // (both CTAs of a pair walk the same units: rank 0 counts them)
+        if (rank == 0) atomicAdd(p.walked, static_cast<unsigned long long>(walkCount[0]));
+        atomicAdd(p.walked + 1, static_cast<unsigned long long>(walkCount[1]));
       }
 #ifdef B200_TC_TIMING
       atomicAdd(&g_tcClk[7], tcClk[7]);
@@ -860,9 +923,31 @@ int g_pipelineChunks = 4;  // chunks of a superposed pass whose verification ove
                            // (option "similarity_pipeline_chunks"; 1 = off)
 int g_superposeAuto = 1;  // 1: a large graph pass picks rows x cols from a pilot over one row group ("similarity_superpose_auto")
 unsigned long long g_candidatesLast = 0;  // candidates the last superposed pass listed ("similarity_candidates_last")
+int g_popcountBand = 1;  // ordered passes skip the tile columns past each row group's popcount band ("similarity_popcount_band")
+// What the count passes of the last graph call (after its pilot) walked: units the host sized the grids for, and what
+// the kernels counted ("similarity_units_planned_last", "similarity_units_last", "similarity_tiles_last").
+unsigned long long g_unitsPlanned = 0;
+namespace {
+__device__ unsigned long long g_walkedDev[2];  // [0] units, [1] tiles (TcParams::walked)
+}
+static unsigned long long* walkCounters() {
+  void* ptr = nullptr;
+  B200_CUDA(cudaGetSymbolAddress(&ptr, g_walkedDev));
+  return static_cast<unsigned long long*>(ptr);
+}
+static void resetWalkCounters(cudaStream_t s) {
+  g_unitsPlanned = 0;
+  B200_CUDA(cudaMemsetAsync(walkCounters(), 0, 2 * sizeof(unsigned long long), s));
+}
+void readWalkCounters(unsigned long long* units, unsigned long long* tiles) {
+  unsigned long long v[2] = {0, 0};
+  B200_CUDA(cudaDeviceSynchronize());
+  B200_CUDA(cudaMemcpyFromSymbol(v, g_walkedDev, sizeof(v)));
+  *units = v[0], *tiles = v[1];
+}
 
 static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, int superS, int superC, bool ordered,
-                             bool* overflow, unsigned long long* pilotCand = nullptr);
+                             bool* overflow, unsigned long long* pilotCand = nullptr, double* pilotPairs = nullptr);
 
 // Count / materialise modes on tensor cores. Returns false when the problem shape is not eligible (caller uses the SIMT tile).
 bool launchSimilarityTensor(SimMode mode, const SimLaunch& q, cudaStream_t s) {
@@ -871,7 +956,10 @@ bool launchSimilarityTensor(SimMode mode, const SimLaunch& q, cudaStream_t s) {
   // (b200mol_tanimoto_count_ge) stays asynchronous on the unsuperposed tile.
   const bool graphPass = mode == kCountTanimoto && (q.symmetric || q.edges != nullptr);
   if (!graphPass || g_superpose * g_superposeCols == 1) {
-    if (graphPass) g_superposeLast = 1;
+    if (graphPass) {
+      g_superposeLast = 1;
+      resetWalkCounters(s);
+    }
     return launchTensorImpl(mode, q, s, 1, 1, false, nullptr);
   }
   int S = g_superpose, C = g_superposeCols;
@@ -882,6 +970,10 @@ bool launchSimilarityTensor(SimMode mode, const SimLaunch& q, cudaStream_t s) {
   // column factor, widest first; the model
   //   time(S, C) = pairs / (S C) * tPair + candidates * S C * tVerify
   // picks the cheapest. A narrower factor can only win while the wider one spends more time verifying than multiplying, so the search stops as soon as it does not.
+  // With the popcount band, `pairs` are the pairs the band leaves: the pilot counts them in its sample, at each column
+  // factor, and the candidate rate is per such pair. The whole set's band is only known after its own sort, so the pass
+  // is costed at the sample's share of banded pairs; every term of the model scales with that share alike, so the
+  // choice does not depend on it.
   if (g_superposeAuto && q.nX >= 8 * static_cast<size_t>(kGroupRows) && C > 1) {
     const double nX = static_cast<double>(q.nX), nY = static_cast<double>(q.nY);
     SimLaunch pilot   = q;
@@ -893,22 +985,27 @@ bool launchSimilarityTensor(SimMode mode, const SimLaunch& q, cudaStream_t s) {
     const double pilotPairs = q.symmetric ? sX * (sX - 1) / 2.0 : sX * sY;
     const double totalPairs = (q.symmetric ? nX * (nX - 1) / 2.0 : nX * nY) / (q.groupStride < 1 ? 1 : q.groupStride);
     // seconds per unsuperposed pair / per verified pair; only their ratio (about 1 : 30) steers the choice. tPair is the
-    // measured pass: 108-110 ms for the 5.0e11 pairs of the 1M bench at S C = 16 (H100 SXM, 400 W limit). On the bench
-    // data (sample in popcount order) the pilot then costs 4 x 4 at 0.17 s and runs it; tools/pilot_model.py prints
-    // these figures for any fingerprint set without a GPU.
+    // measured pass: 101.8 ms for the 4.67e11 pairs the popcount band leaves of the 1M bench at S C = 16 (H100 SXM, 400 W
+    // limit; 108-110 ms for all 5.0e11 pairs without the band). On the bench data (sample in popcount order) the pilot
+    // then costs 4 x 4 at 0.17 s and runs it; tools/pilot_model.py prints these figures for any fingerprint set without
+    // a GPU.
     constexpr double tPair = 3.5e-12, tVerify = 0.1e-9;
-    double bestT = totalPairs * tPair;  // unsuperposed
+    double bestT = -1.0;  // unsuperposed, costed at the widest factor's banded share
     int    bestS = 1, bestC = 1;
     for (int c = C; c >= 1; c >>= 1) {
       unsigned long long got = 0;
-      if (!launchTensorImpl(mode, pilot, s, S, c, true, nullptr, &got)) return false;
-      const double tPass = totalPairs / (S * c) * tPair;
-      const double tVer  = static_cast<double>(got) * totalPairs / pilotPairs * S * c * tVerify;
+      double             left = pilotPairs;
+      if (!launchTensorImpl(mode, pilot, s, S, c, true, nullptr, &got, &left)) return false;
+      const double passPairs = totalPairs * (left / pilotPairs);
+      if (bestT < 0.0) bestT = passPairs * tPair;
+      const double tPass = passPairs / (S * c) * tPair;
+      const double tVer  = left > 0.0 ? static_cast<double>(got) * passPairs / left * S * c * tVerify : 0.0;
       if (tPass + tVer < bestT) bestT = tPass + tVer, bestS = S, bestC = c;
       if (tVer <= tPass) break;
     }
     S = bestS, C = bestC;
   }
+  resetWalkCounters(s);
   while (S * C > 1) {
     bool overflow = false;
     if (!launchTensorImpl(mode, q, s, S, C, true, &overflow)) return false;
@@ -926,8 +1023,26 @@ bool launchSimilarityTensor(SimMode mode, const SimLaunch& q, cudaStream_t s) {
 // ordered (graph passes of the count mode): run on the fingerprints in popcount order and map the results back. Every
 // pass of a graph pass with superposition on is ordered, also an unsuperposed fallback (of the whole call, of a rank or
 // of a pipeline chunk): it must cover the same row groups as the superposed pass it replaces or completes.
+// Pairs i < j (symmetric) or (i, j) of a pass over all row groups that the popcount band leaves (band = nullptr: all).
+static double bandPairs(const TcParams& p, const uint32_t* band, size_t nX, size_t nY) {
+  double total = 0.0;
+  for (size_t r0 = 0, g = 0; r0 < nX; r0 += kGroupRows, ++g) {
+    const size_t r1 = std::min(nX, r0 + kGroupRows);
+    const size_t e  = band ? std::min(nY, static_cast<size_t>(band[g]) * p.colSpan) : nY;  // columns [0, e) are visited
+    if (!p.symmetric) {
+      total += static_cast<double>(r1 - r0) * static_cast<double>(e);
+      continue;
+    }
+    const size_t iEnd = std::min(r1, e > 0 ? e - 1 : 0);  // rows i with a column i < j < e
+    if (iEnd <= r0) continue;
+    const double m = static_cast<double>(iEnd - r0);
+    total += m * static_cast<double>(e - 1) - (static_cast<double>(r0) + static_cast<double>(iEnd) - 1.0) * m / 2.0;
+  }
+  return total;
+}
+
 static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, int superS, int superC, bool ordered,
-                             bool* overflow, unsigned long long* pilotCand) {
+                             bool* overflow, unsigned long long* pilotCand, double* pilotPairs) {
   if (mode == kCountCosine) return false;
   const int bits = q.words * 32;
   if (bits % kTK != 0 || bits > 4096) return false;
@@ -1059,6 +1174,22 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
     p.threshLen = maxS + 1;
   }
   p.thresh = thresh.get();
+  // The popcount band of an ordered pass (superposed passes, their unsuperposed fallbacks, the pilot), with a host copy
+  // for the unit count that sizes the grid: one read of a few hundred bytes per pass.
+  const uint32_t        groups = static_cast<uint32_t>((q.nX + kGroupRows - 1) / kGroupRows);
+  const bool            banded = ordered && g_popcountBand;
+  Scratch<uint32_t>     band(banded ? groups : 0, s);
+  std::vector<uint32_t> bandHost(banded ? groups : 0);
+  if (banded) {
+    popcountBandKernel<<<1, kBandThreads, (maxS + 1) * sizeof(uint16_t), s>>>(popXs, q.nX, popYs, q.nY, thresh.get(), maxS + 1,
+                                                                              p.colSpan, p.tilesN, groups, band.get());
+    B200_LAUNCHED();
+    B200_CUDA(cudaMemcpyAsync(bandHost.data(), band.get(), groups * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    B200_CUDA(cudaStreamSynchronize(s));
+    p.bandEnd = band.get();
+  }
+  const uint32_t* bandH = banded ? bandHost.data() : nullptr;
+  if (count) p.walked = walkCounters();
 
   CUtensorMap tmA, tmB;
   makeTensorMap2D(&tmA, expX.get(), nSuper, rowBytes, kTM, kTK, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1);
@@ -1084,11 +1215,12 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
   }
   // units a call owns: tiles, or vertical tile pairs (same enumeration as the kernel's UnitWalk)
   auto unitsOf = [&](const TcParams& pk) -> uint64_t {
-    return stationary ? countUnits<true, kRunStat>(pk) : cluster ? countUnits<true>(pk) : countUnits<false>(pk);
+    return stationary ? countUnits<true, kRunStat>(pk, bandH) : cluster ? countUnits<true>(pk, bandH) : countUnits<false>(pk, bandH);
   };
   // the count kernel over the row groups `pk` selects (false: none of them is owned by this call)
   auto launchCount = [&](const TcParams& pk) -> bool {
     const uint64_t units = unitsOf(pk);
+    if (!pilotCand) g_unitsPlanned += units;
     if (units == 0) return false;
     if (cluster) {
       cudaLaunchConfig_t cfg{};
@@ -1211,8 +1343,9 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
     unsigned long long nCand = 0;
     B200_CUDA(cudaMemcpyAsync(&nCand, candCursor.get(), sizeof(nCand), cudaMemcpyDeviceToHost, s));
     B200_CUDA(cudaStreamSynchronize(s));
-    if (pilotCand) {  // dry run over one row group: the candidate count is the result
+    if (pilotCand) {  // dry run over one row group: the candidate count is the result, over the pairs the band leaves
       *pilotCand = nCand;
+      if (pilotPairs) *pilotPairs = bandPairs(p, bandH, q.nX, q.nY);
       return true;
     }
     g_candidatesLast = nCand;
