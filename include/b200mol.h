@@ -407,6 +407,29 @@ int b200mol_rms_prune(int32_t nMols, const int32_t* d_mol_conf_start, const int3
                       const int32_t* d_match_offset, const int32_t* d_match_len, const int16_t* d_match_atoms, double rms_thresh,
                       const uint8_t* d_conf_valid, uint8_t* d_keep, void* stream);
 
+/* Torsion fingerprint deviation (TFD) matrices between the conformers of each molecule (RDKit
+ * TorsionFingerprints.GetTFDMatrix). Conformer k of molecule m is conformer d_conf_order[h_mol_conf_start[m] + k]
+ * (d_conf_order NULL = identity), which owns atoms [d_conf_atom_start[c], ...) of d_xyz[.][3] (f64).
+ * Torsions of molecule m are [h_tors_start[m], h_tors_start[m+1]); torsion t has the quartets
+ * [h_quartet_start[t], h_quartet_start[t+1]) of h_quartets[.][4] (molecule-local atom indices), type h_type[t]
+ * (B200MOL_TFD_SINGLE: one quartet; _SYMMETRIC: the minimum over quartet pairs; _RING: the ring's consecutive
+ * quartets, compared through the mean |phi|), weight h_weight[t] >= 0 and h_maxdev[t] > 0 (degrees).
+ * For conformers I > J: TFD = sum_t w_t d_t / maxDev_t / sum_t w_t, 0 when sum w <= 1e-10; d as in RDKit's
+ * CalculateTFD, with phi = 0 for a quartet whose cross product i-j x j-k or j-k x k-l is exactly zero.
+ * d_out (f32): the lower triangles of all molecules, concatenated: molecule m starts at sum_{m'<m} C(C-1)/2, and
+ * holds (I, J) at I(I-1)/2 + J. A molecule with fewer than two conformers contributes nothing; one without torsions
+ * gives zeros. The torsion and conformer-count tables are HOST arrays: the call plans its tiles from them and uploads
+ * the plan in one cudaMemcpyAsync from pageable memory (which CUDA may stage synchronously, as for any pageable copy);
+ * coordinates and output stay on the device and both kernels run on `stream`.
+ * Replaces GetTFDMatricesGpuBuffer / tfdMatrixKernel (src/tfd/tfd_gpu.cpp, src/tfd/tfd_kernels.cu:84-166). */
+#define B200MOL_TFD_SINGLE 0
+#define B200MOL_TFD_SYMMETRIC 1
+#define B200MOL_TFD_RING 2
+int b200mol_tfd_matrices(int32_t nMols, const int32_t* h_mol_conf_start, const int32_t* d_conf_order,
+                         const int32_t* d_conf_atom_start, const double* d_xyz, const int32_t* h_tors_start,
+                         const int32_t* h_quartet_start, const int16_t* h_quartets, const uint8_t* h_type,
+                         const double* h_weight, const double* h_maxdev, float* d_out, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Distance-geometry preparation (per-molecule, matrix resident in shared memory).
  * Matrices are concatenated: matrix m occupies d_x[starts[m] .. starts[m+1]) = n_m * n_m doubles, row-major.

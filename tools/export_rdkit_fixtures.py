@@ -13,6 +13,10 @@ and commit the resulting .npz. `tests/test_rdkit_fixtures.py` then replays it (s
     minimised energies on the same conformers (tests/test_mmff.cu:1521-1608 style)              -> <= 1e-4 relative
   * ETKDG: raw + smoothed bounds matrices, flattened DG / ETK / check tables, RDKit's EmbedMultipleConfs coordinates
     (per-molecule RMSD / bounds-violation statistics are compared, not coordinates)
+  * TFD (to tests/golden/rdkit_tfd.npz, replayed by tests/test_tfd.py): RDKit's torsion lists and weights
+    (TorsionFingerprints.CalculateTorsionLists / CalculateTorsionWeights) in the flat layout of b200mol_tfd_matrices,
+    the tables nvmolkit_b200.tfd.tfd_torsions builds for the same molecules, ETKDG conformers and
+    TorsionFingerprints.GetTFDMatrix on them
 
 The default molecule set is a small drug-like SMILES list embedded below (aspirin, ibuprofen, caffeine, ...); pass
 --smiles benchmarks/data/chembl_10k.smi of the reference checkout for the BASELINE configs' real input.
@@ -149,6 +153,47 @@ def main() -> None:
     out["rdkit_embedded_positions"] = np.concatenate([c.GetPositions() for m in hmols for c in m.GetConformers()])
     np.savez_compressed(args.out, **out)
     print(f"wrote {args.out}: {len(mols)} molecules, {len(hmols)} with conformers, RDKit {rdkit.__version__}")
+    export_tfd(hmols, os.path.join(os.path.dirname(os.path.abspath(args.out)), "rdkit_tfd.npz"))
+
+
+def export_tfd(hmols, path: str, n_confs: int = 6) -> None:
+    """RDKit's TFD inputs and matrices (weights on, maxDev 'equal', symmRadius 2, colinear bonds ignored)."""
+    import rdkit
+    from rdkit import Chem
+    from rdkit.Chem import TorsionFingerprints as TF
+    from rdkit.Chem import rdDistGeom
+
+    from nvmolkit_b200 import tfd
+
+    mols, per_mol, coords, matrices = [], [], [], []
+    for m in hmols:
+        mh = Chem.Mol(m)
+        mh.RemoveAllConformers()
+        p = rdDistGeom.ETKDGv3()
+        p.randomSeed = 7
+        if len(rdDistGeom.EmbedMultipleConfs(mh, n_confs, p)) < 2:
+            continue
+        tl, tlr = TF.CalculateTorsionLists(mh, maxDev="equal", symmRadius=2, ignoreColinearBonds=True)
+        weights = TF.CalculateTorsionWeights(mh, ignoreColinearBonds=True) if (tl or tlr) else []
+        tors = [([tuple(q) for q in quartets], tfd.SYMMETRIC if len(quartets) > 1 else tfd.SINGLE, 1.0, float(md))
+                for quartets, md in tl]
+        tors += [([tuple(q) for q in quartets], tfd.RING, 1.0, float(md)) for quartets, md in tlr]
+        tors = [(q, t, float(w), md) for (q, t, _w, md), w in zip(tors, weights)] if len(weights) == len(tors) else tors
+        mols.append(mh)
+        per_mol.append(tors)
+        coords.append([c.GetPositions() for c in mh.GetConformers()])
+        matrices.append(np.asarray(TF.GetTFDMatrix(mh, useWeights=True, maxDev="equal"), np.float64))
+    ref = tfd.TFDTorsions.from_lists(per_mol)
+    flat = tfd.FlatTFDMolecules.from_coordinates(ref, coords)
+    ours = tfd.tfd_torsions(mols)
+    out = {"rdkit_version": np.array(rdkit.__version__), "smiles": np.array([Chem.MolToSmiles(m) for m in mols]),
+           "mol_conf_start": flat.mol_conf_start, "conf_atom_start": flat.conf_atom_start, "xyz": flat.xyz,
+           "tfd": np.concatenate(matrices) if matrices else np.zeros(0), "tfd_sizes": np.array([len(x) for x in matrices])}
+    for k in ("tors_start", "quartet_start", "quartets", "type", "weight", "maxdev"):
+        out[k] = getattr(ref, k)
+        out[f"adapter_{k}"] = getattr(ours, k)
+    np.savez_compressed(path, **out)
+    print(f"wrote {path}: {len(mols)} molecules")
 
 
 if __name__ == "__main__":
