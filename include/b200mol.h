@@ -430,6 +430,24 @@ int b200mol_tfd_matrices(int32_t nMols, const int32_t* h_mol_conf_start, const i
                          const int32_t* h_quartet_start, const int16_t* h_quartets, const uint8_t* h_type,
                          const double* h_weight, const double* h_maxdev, float* d_out, void* stream);
 
+/* Conformer RMSD matrices (RDKit AllChem.GetConformerRMSMatrix, over all atoms). Conformer k of molecule m is conformer
+ * d_conf_order[h_mol_conf_start[m] + k] (d_conf_order NULL = identity), which owns exactly h_mol_atoms[m] atoms from
+ * d_conf_atom_start[c] of d_xyz[.][3] (f64). For conformers I > J:
+ *   prealigned == 0: sqrt(max(0, Ga + Gb - 2 (s1 + s2 + sign(det H) s3)) / n), the RMSD after the best proper rigid
+ *                    superposition (Ga, Gb: sums of squared centred coordinates; s_i: singular values of the covariance
+ *                    H of the centred coordinates). The coordinates are not modified.
+ *   prealigned != 0: sqrt(sum_k |a_k - b_k|^2 / n) on the coordinates as given.
+ * d_out (f64): the lower triangles of all molecules, concatenated: molecule m starts at sum_{m'<m} C(C-1)/2 (int64), and
+ * holds (I, J) at I(I-1)/2 + J. A molecule with fewer than two conformers contributes nothing; one with two or more and
+ * no atoms is an error. The conformer and atom-count tables are HOST arrays: the call plans its tiles from them and
+ * uploads the plan in one cudaMemcpyAsync from pageable memory; coordinates and output stay on the device and both
+ * kernels run on `stream`. Sums run in a fixed order: results are bitwise repeatable and independent of the other
+ * molecules of the call.
+ * Replaces conformerRmsdBatchMatrixGpu (src/conformer_rmsd.cu, nvmolkit/conformerRmsd.cpp). */
+int b200mol_conformer_rmsd(int32_t nMols, const int32_t* h_mol_conf_start, const int32_t* h_mol_atoms,
+                           const int32_t* d_conf_order, const int32_t* d_conf_atom_start, const double* d_xyz,
+                           int32_t prealigned, double* d_out, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Distance-geometry preparation (per-molecule, matrix resident in shared memory).
  * Matrices are concatenated: matrix m occupies d_x[starts[m] .. starts[m+1]) = n_m * n_m doubles, row-major.

@@ -24,6 +24,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "tiles.cuh"
 #include "tma.cuh"
 
 namespace b200 {
@@ -54,16 +55,6 @@ struct TorDesc {  // 16 B: bulk-copied as a block
   int32_t type;   // B200MOL_TFD_*
   float   wm;     // w / maxDev
 };
-
-__device__ __forceinline__ int upperIndex(const int64_t* starts, int n, int64_t v) {  // largest m with starts[m] <= v
-  int lo = 0, hi = n;
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (starts[mid] <= v) lo = mid;
-    else hi = mid;
-  }
-  return lo;
-}
 
 // a x b with every product rounded on its own (__dmul_rn is never contracted into an FMA): the cross product of
 // parallel vectors is then exactly zero, as on the CPU, so the phi = 0 convention sees the same geometries there
@@ -148,12 +139,8 @@ __global__ void __launch_bounds__(kPT) tfdPairKernel(int nMols, const int64_t* u
     if (u >= total) break;
     const int     m  = upperIndex(unitStart, nMols + 1, u);
     const MolDesc md = mols[m];
-    // local unit -> tile (ti, tj), tj <= ti, row-major over the lower triangle
-    const int64_t loc = u - unitStart[m];
-    int           ti  = static_cast<int>((sqrt(8.0 * static_cast<double>(loc) + 1.0) - 1.0) * 0.5);
-    while (static_cast<int64_t>(ti) * (ti + 1) / 2 > loc) --ti;
-    while (static_cast<int64_t>(ti + 1) * (ti + 2) / 2 <= loc) ++ti;
-    const int tj    = static_cast<int>(loc - static_cast<int64_t>(ti) * (ti + 1) / 2);
+    int ti, tj;
+    lowerTriangleTile(u - unitStart[m], ti, tj);
     const int R     = md.R, F = md.F;
     const int nRows = min(R, md.nConf - ti * R), nCols = min(R, md.nConf - tj * R);
     float*    sRow  = reinterpret_cast<float*>(smem);
@@ -309,7 +296,7 @@ extern "C" int b200mol_tfd_matrices(int32_t nMols, const int32_t* h_mol_conf_sta
       featTotal += static_cast<int64_t>(md.nConf) * md.F;
       outTotal += static_cast<int64_t>(md.nConf) * (md.nConf - 1) / 2;
       workStart[m + 1] = workStart[m] + static_cast<int64_t>(md.nConf) * md.nTors;
-      unitStart[m + 1] = unitStart[m] + static_cast<int64_t>(md.T) * (md.T + 1) / 2;
+      unitStart[m + 1] = unitStart[m] + lowerTriangleUnits(md.T);
       if (md.T > 0) smemMax = std::max(smemMax, unitSmem(md.R, md.F, md.nTors));
     }
     if (outTotal == 0) return;

@@ -37,6 +37,7 @@ import numpy as np
 import torch
 
 from nvmolkit_b200 import _lib
+from nvmolkit_b200._hostutil import device_conformer_order
 from nvmolkit_b200._interop import require_cuda, stream_ctx, stream_ptr
 from nvmolkit_b200.types import Device3DResult
 
@@ -441,21 +442,9 @@ def GetTFDMatrices(mols, useWeights: bool = True, maxDev: str = "equal", symmRad
 
     xyz = coordinates.values.torch()
     dev = xyz.device
-    mol_idx = coordinates.mol_indices.torch().cpu().numpy().astype(np.int64)
-    conf_idx = coordinates.conf_indices.torch().cpu().numpy().astype(np.int64)
-    starts_t = coordinates.atom_starts.torch()
-    sizes = np.diff(starts_t.cpu().numpy().astype(np.int64))
-    if len(mol_idx) and (mol_idx.min() < 0 or mol_idx.max() >= len(mols)):
-        raise ValueError("coordinates: molecule index out of range")
-    expect = np.asarray(atom_counts, np.int64)[mol_idx]
-    if np.any(sizes != expect):
-        bad = int(np.nonzero(sizes != expect)[0][0])
-        raise ValueError(f"coordinates: conformer {bad} has {int(sizes[bad])} atoms, molecule {int(mol_idx[bad])} has "
-                         f"{int(expect[bad])}")
+    order, counts, starts_t = device_conformer_order(coordinates, atom_counts)
     stream_ptr(stream)
     require_cuda()
-    order = np.lexsort((conf_idx, mol_idx)).astype(np.int32)
-    counts = np.bincount(mol_idx, minlength=len(mols)).astype(np.int64)
     with torch.cuda.device(dev), stream_ctx(stream):
         d_order = torch.from_numpy(order).to(dev)
         cas = starts_t.to(device=dev, dtype=torch.int32).contiguous()
