@@ -64,6 +64,10 @@ int b200mol_free_async(void* d_ptr, void* stream);
  *   "similarity_popcount_band"     1 (default): a neighbour pass in popcount order (superposed, its fallbacks, the
  *                                  pilot) skips, per row group of 8,192 fingerprints, the tile columns whose popcounts
  *                                  no row of the group can reach a neighbour with; 0: visits them. Results identical
+ *   "topk_slab_cols"               0 (default): b200mol_similarity_topk warms its bars on the first 4,096 library
+ *                                  fingerprints and sends the rest through the tensor tile in column slabs that double,
+ *                                  up to 512 MB of expanded operand; > 0: warm-up (at least B200MOL_TOPK_MAX) and every
+ *                                  slab take this many fingerprints. Results identical
  *   "butina_min_round_commits"     a parallel Butina round that commits fewer clusters than this hands over to the
  *                                  one-cluster-per-step loop (default 32; 0 = rounds only, >= 1e9 = stepwise only)
  *   "etkdg_hessian_fp64"           0 (default): the embedder keeps its BFGS inverse Hessian in fp32 and sweeps it in fp32
@@ -78,7 +82,9 @@ int b200mol_set_option(const char* key, long long value);
  * (1 after a candidate-list overflow made it fall back), "similarity_candidates_last": how many candidates it listed, and
  * what the tensor-core count passes of the last neighbour pass walked after its pilot: "similarity_units_planned_last"
  * (work units the host sized the grids for), "similarity_units_last" and "similarity_tiles_last" (units and tiles the
- * kernels counted; these two synchronise the device). */
+ * kernels counted; these two synchronise the device). Of the last b200mol_similarity_topk: "topk_slabs_last" (column slabs
+ * that went through the tensor tile), "topk_candidates_last" (pairs its epilogue listed) and "topk_rows_redone_last" (rows
+ * of a slab whose candidates did not fit and that the SIMT scan redid); the last two synchronise the device. */
 int b200mol_get_option(const char* key, long long* value);
 /* Per-phase CUDA-event timing inside the library (off by default). Phases: "neighbor_pass" (the N^2 tile kernel
  * alone), "csr_build", "cluster_loop", "bfgs". b200mol_profile_read waits for the phase's stop event. */
@@ -120,6 +126,19 @@ int b200mol_similarity_cross_host(const uint32_t* h_a, size_t nA, const uint32_t
  * materialised. Replaces the Triton kernel _update_neighbor_count_kernel (nvmolkit/_fusedButina.py:99-179, 249-289). */
 int b200mol_tanimoto_count_ge(const uint32_t* d_x, size_t nX, const uint32_t* d_y, size_t nY, int words, int metric,
                               double cutoff, int sign, int32_t* d_counts, void* stream);
+
+/* Exact k-nearest-neighbour search, the similarity matrix never materialised: row q of d_values / d_indices ([nQ][k],
+ * caller-allocated) holds the first k columns of row q of the matrix b200mol_tanimoto_cross / b200mol_cosine_cross would
+ * write for the same inputs, ordered by (value descending, column index ascending): values bit-identical to the matrix
+ * entries, ties to the lowest index, the result a pure function of the inputs. d_lib = NULL searches the queries
+ * themselves (self-matches included). 1 <= k <= min(nLib, B200MOL_TOPK_MAX), metric = B200MOL_METRIC_*; inputs are
+ * borrowed. Asynchronous on `stream`, no host synchronisation; scratch is stream-ordered: 8 * words bytes per query
+ * (expanded operand), at most 512 MB of expanded library slab, and 4 * min(1792, max(256, 8 k)) bytes of candidate slots
+ * per query. Inputs of fewer than "similarity_tensor_min_pairs" pairs, or with at most 4,096 library fingerprints, are
+ * scanned by a SIMT kernel; larger ones run on the wgmma tile. Both give the same bits. */
+#define B200MOL_TOPK_MAX 256
+int b200mol_similarity_topk(const uint32_t* d_q, size_t nQ, const uint32_t* d_lib, size_t nLib, int words, int metric,
+                            int k, double* d_values /* [nQ][k] */, int32_t* d_indices /* [nQ][k] */, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Butina clustering.  Definition (RDKit ML.Cluster.Butina.ClusterData(reordering=True), the CPU baseline the

@@ -317,6 +317,9 @@ extern unsigned long long g_candidatesLast;
 extern int g_popcountBand;
 extern unsigned long long g_unitsPlanned;
 void readWalkCounters(unsigned long long* units, unsigned long long* tiles);
+extern long long          g_topkSlabCols;
+extern unsigned long long g_topkSlabsLast;
+void readTopkStats(unsigned long long* candidates, unsigned long long* redone);
 long long g_tensorMinPairs = 1ll << 24;  // pair count from which the passes run on the tensor-core tile (< 0: never)
 
 void launchThreshTable(int maxS, double cutoff, uint16_t* thresh, cudaStream_t s) {
@@ -451,6 +454,10 @@ extern "C" int b200mol_set_option(const char* key, long long value) {
       g_pipelineChunks = static_cast<int>(value);
     }
     else if (k == "similarity_popcount_band") g_popcountBand = value != 0;
+    else if (k == "topk_slab_cols") {
+      B200_REQUIRE(value >= 0 && value < (1ll << 31), "topk_slab_cols must be in [0, 2^31)");
+      g_topkSlabCols = value;
+    }
     else if (k == "similarity_tensor_cluster") {
       B200_REQUIRE(value >= 0 && value <= 3, "similarity_tensor_cluster must be 0, 1, 2 or 3");
       g_tensorCluster = static_cast<int>(value);
@@ -484,6 +491,13 @@ extern "C" int b200mol_get_option(const char* key, long long* value) {
       unsigned long long units = 0, tiles = 0;
       readWalkCounters(&units, &tiles);
       *value = static_cast<long long>(k == "similarity_units_last" ? units : tiles);
+    }
+    else if (k == "topk_slab_cols") *value = g_topkSlabCols;
+    else if (k == "topk_slabs_last") *value = static_cast<long long>(g_topkSlabsLast);  // read-only
+    else if (k == "topk_candidates_last" || k == "topk_rows_redone_last") {  // read-only; synchronises the device
+      unsigned long long listed = 0, redone = 0;
+      readTopkStats(&listed, &redone);
+      *value = static_cast<long long>(k == "topk_candidates_last" ? listed : redone);
     }
     else if (k == "butina_min_round_commits") *value = g_butinaMinCommits;
     else fail(B200MOL_ERR_INVALID, "unknown option '%s'", key);

@@ -90,6 +90,13 @@ struct TcParams {
   // neighbour of any of its rows (popcountBandKernel). The walk skips the tile columns at and past it.
   const uint32_t*     bandEnd;
   unsigned long long* walked;  // [0] += units walked (once per CTA pair), [1] += tiles a CTA ran; nullptr: not counted
+  // Top-k search (topk.cu): per query row its running bar {c, |A| + |B|, column, float bits of a lower bound of the value}
+  // of the current k-th best; an accumulator that could beat it leaves as its column index in the row's candidate slots.
+  const int4* topkBar;
+  uint32_t*   topkCand;   // [n][topkCap] caller's column indices
+  uint32_t*   topkCount;  // [n] slots asked for (may pass topkCap: the row is then redone, nothing of it is merged)
+  uint32_t    topkCap;
+  uint32_t    topkColBase;  // caller's index of the Y operand's first row (the library is searched in column slabs)
 };
 
 // The popcount band. A pair with popcounts a, b and intersection c <= min(a, b) can only be a neighbour if
@@ -100,7 +107,7 @@ struct TcParams {
 // row group whose largest popcount is A, no column past the first one this cuts can be a neighbour of any of its rows.
 __host__ __device__ __forceinline__ bool bandCuts(const uint16_t* tmin, int A, int b) { return tmin[A + b] > A; }
 
-enum TcMode : int { kTcCount = 0, kTcTanimoto = 1, kTcCosine = 2 };
+enum TcMode : int { kTcCount = 0, kTcTanimoto = 1, kTcCosine = 2, kTcTopkTanimoto = 3, kTcTopkCosine = 4 };
 }  // namespace
 int g_tensorCluster = 1;  // count tile in clusters of two CTAs with a multicast column operand (option "similarity_tensor_cluster":
                           // 0 one CTA per tile, 1 the pair, 2 the pair too (kept for callers written for the CTA-pair MMA
@@ -559,6 +566,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
   extern __shared__ __align__(1024) uint8_t smemRaw[];
   static_assert(!CL || MODE == kTcCount, "the two-CTA cluster is wired for the count tile");
   constexpr bool COUNT = MODE == kTcCount;
+  constexpr bool TOPK  = MODE == kTcTopkTanimoto || MODE == kTcTopkCosine;
   constexpr bool ST    = CL == 3;  // row operand stationary
   using Walk           = UnitWalk<CL != 0, ST ? kRunStat : 1>;
   constexpr int  kStg       = ST ? kStagesStat : kStages;
@@ -814,6 +822,66 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
           if (hits0) atomicAdd(p.counts + r0, p.sign * hits0);
           if (hits1) atomicAdd(p.counts + r1, p.sign * hits1);
           B200_TC_T1(tCand, 4);
+        } else if constexpr (TOPK) {
+          // Top-k filter: can the pair beat the row's bar, the key of its current k-th best? Conservative - the select
+          // kernel (topk.cu) re-counts every survivor and orders them exactly - but tight, so that survivors stay rare.
+          // The bar's column lies before the slab (the list holds earlier columns only), so a tie never wins.
+          // Tanimoto, in integers: c / (s - c) > cB / (sB - cB)  <=>  c sB > cB s  (s = |A| + |B|; both sides < 2^26).
+          // Equal ratios round to equal fp64 values and distinct ratios with denominators <= 8192 differ by more than
+          // 2^-26, far above an ulp, so this integer order is the order of the fp64 values the select kernel compares.
+          // Cosine, c / sqrt(|A| |B|), has no integer form: float(c) >= tauLow sqrt|A| sqrt|B| with tauLow a few 1e-5
+          // (relative) below the bar, which covers the float roundings; ties and near ties survive.
+          constexpr bool COS = MODE == kTcTopkCosine;
+          const bool in0 = r0 < p.n, in1 = r1 < p.n;
+          // per row: margin(c, column) = c f - g term(column) must exceed t. Past the end nothing does.
+          int   f0 = 0, g0 = 0, t0 = 0x7fffffff, f1 = 0, g1 = 0, t1 = 0x7fffffff;
+          float rt0 = 3.0e38f, rt1 = 3.0e38f;
+          if (in0) {
+            const int4 b = __ldg(p.topkBar + r0);
+            f0 = b.y, g0 = b.x, t0 = b.x * pa0;
+            rt0 = __int_as_float(b.w) * sqrtf(static_cast<float>(pa0));
+          }
+          if (in1) {
+            const int4 b = __ldg(p.topkBar + r1);
+            f1 = b.y, g1 = b.x, t1 = b.x * pa1;
+            rt1 = __int_as_float(b.w) * sqrtf(static_cast<float>(pa1));
+          }
+          // does accumulator e of a column block (popcount pb, sqrt(pb) as float bits sq) pass? (cosine: the count through
+          // the 2^23 trick, exact and no I2F)
+          auto pass = [&](int e, int a, int pb, int sq) {
+            if constexpr (COS) return fmaf(-(e < 2 ? rt0 : rt1), __int_as_float(sq), __int_as_float(0x4b000000 | a) - 8388608.0f) >= 0.0f;
+            else return a * (e < 2 ? f0 : f1) - (e < 2 ? g0 : g1) * pb > (e < 2 ? t0 : t1);
+          };
+          bool any = false;
+#pragma unroll
+          for (int j = 0; j < 32; ++j) {
+            const int4 ci = cm[4 * j];
+            any |= pass(0, static_cast<int>(acc[4 * j]), ci.x, ci.y) | pass(1, static_cast<int>(acc[4 * j + 1]), ci.z, ci.w) |
+                   pass(2, static_cast<int>(acc[4 * j + 2]), ci.x, ci.y) | pass(3, static_cast<int>(acc[4 * j + 3]), ci.z, ci.w);
+          }
+          if (__any_sync(0xffffffffu, any)) {
+            // survivors as bits 4 (j % 8) + e of sv[j / 8] in one unrolled pass; each lane then lists its own in a rolled loop
+            uint32_t sv[4] = {0, 0, 0, 0};
+#pragma unroll
+            for (int j = 0; j < 32; ++j) {
+              const int4 ci  = ldsFresh(cm + 4 * j);
+              uint32_t   nib = 0;
+#pragma unroll
+              for (int e = 0; e < 4; ++e)
+                if (pass(e, static_cast<int>(acc[4 * j + e]), (e & 1) ? ci.z : ci.x, (e & 1) ? ci.w : ci.y) && (e < 2 ? in0 : in1) &&
+                    c0 + 8 * j + (e & 1) < p.nY)
+                  nib |= 1u << e;
+              sv[j >> 3] |= nib << (4 * (j & 7));
+            }
+#pragma unroll
+            for (int w = 0; w < 4; ++w)
+              for (uint32_t bits = sv[w]; bits; bits &= bits - 1) {
+                const int      b = __ffs(bits) - 1, e = b & 3;
+                const uint32_t r = e < 2 ? r0 : r1, c = c0 + 8 * (8 * w + (b >> 2)) + (e & 1);
+                const uint32_t at = atomicAdd(p.topkCount + r, 1u);
+                if (at < p.topkCap) p.topkCand[static_cast<size_t>(r) * p.topkCap + at] = p.topkColBase + c;
+              }
+          }
         } else {
           // fp64 Tanimoto / cosine straight from the accumulators: a quad of lanes writes 64 contiguous bytes of a row
 #pragma unroll
@@ -1356,6 +1424,73 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
     if (nCand) launchVerify(cand.get(), nCand, s);
   }
   return true;
+}
+
+// ---- top-k search (topk.cu): the 0/1 expansion and one tile pass of the queries over a column slab of the library ----
+namespace {
+// {popcount, float bits of sqrt(popcount) (cosine) or 0} per operand row, whole tiles; rows past the end: popcount 0 and a
+// square root no accumulator reaches
+__global__ void topkMetaKernel(const int32_t* __restrict__ pop, size_t n, size_t nPad, int cosine, int2* __restrict__ out) {
+  const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= nPad) return;
+  if (i >= n) out[i] = make_int2(0, cosine ? __float_as_int(3.0e38f) : 0);
+  else out[i] = make_int2(pop[i], cosine ? __float_as_int(sqrtf(static_cast<float>(pop[i]))) : 0);
+}
+}  // namespace
+
+void launchExpandBits(const uint32_t* fp, size_t n, int words, uint8_t* out, cudaStream_t s) {
+  const size_t nw = n * static_cast<size_t>(words);
+  if (nw == 0) return;
+  expandBitsKernel<<<static_cast<unsigned>((nw + 255) / 256), 256, 0, s>>>(fp, nw, reinterpret_cast<uint4*>(out));
+  B200_LAUNCHED();
+}
+
+bool topkTileEligible(int words) { return (words * 32) % kTK == 0 && words * 32 <= 4096; }
+
+void launchTopkTile(bool cosine, const uint8_t* expQ, size_t nQ, const int32_t* popQ, const uint8_t* expLib, size_t nCols,
+                    const int32_t* popCols, int words, const int4* bar, uint32_t* cand, uint32_t* count, uint32_t cap,
+                    uint32_t colBase, cudaStream_t s) {
+  const int rowBytes = words * 32;
+  TcParams  p{};
+  p.n           = static_cast<uint32_t>(nQ);
+  p.nY          = static_cast<uint32_t>(nCols);
+  p.kChunks     = rowBytes / kTK;
+  p.tilesM      = static_cast<uint32_t>((nQ + kTM - 1) / kTM);
+  p.tilesN      = static_cast<uint32_t>((nCols + kTN - 1) / kTN);
+  p.groupStride = 1;
+  p.superS = p.superC = 1;
+  p.rowSpan     = kTM;
+  p.colSpan     = kTN;
+  p.groupTiles  = kGroupRows / kTM;
+  p.topkBar     = bar;
+  p.topkCand    = cand;
+  p.topkCount   = count;
+  p.topkCap     = cap;
+  p.topkColBase = colBase;
+  const size_t  rowsPad = static_cast<size_t>(p.tilesM) * kTM, colsPad = static_cast<size_t>(p.tilesN) * kTN;
+  Scratch<int2> rowMeta(rowsPad, s), colMeta(colsPad, s);
+  topkMetaKernel<<<static_cast<unsigned>((rowsPad + 255) / 256), 256, 0, s>>>(popQ, nQ, rowsPad, 0, rowMeta.get());
+  B200_LAUNCHED();
+  topkMetaKernel<<<static_cast<unsigned>((colsPad + 255) / 256), 256, 0, s>>>(popCols, nCols, colsPad, cosine ? 1 : 0, colMeta.get());
+  B200_LAUNCHED();
+  p.rowMeta = rowMeta.get();
+  p.colMeta = colMeta.get();
+  CUtensorMap tmA, tmB;
+  makeTensorMap2D(&tmA, expQ, nQ, rowBytes, kTM, kTK, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1);
+  makeTensorMap2D(&tmB, expLib, nCols, rowBytes, kTN, kTK, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1);
+  const size_t smemBytes = static_cast<size_t>(kStages) * kStageBytes + 1024;
+  static bool  configured[kMaxDevices] = {};
+  if (!configured[currentDeviceSlot()]) {
+    B200_CUDA(cudaFuncSetAttribute(simTensorKernel<kTcTopkTanimoto, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smemBytes)));
+    B200_CUDA(cudaFuncSetAttribute(simTensorKernel<kTcTopkCosine, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smemBytes)));
+    configured[currentDeviceSlot()] = true;
+  }
+  const uint64_t units = countUnits<false>(p, nullptr);
+  if (units == 0) return;
+  const int grid = static_cast<int>(std::min<uint64_t>(static_cast<uint64_t>(smCount()), units));
+  if (cosine) simTensorKernel<kTcTopkCosine, 0><<<grid, kThreadsTC, smemBytes, s>>>(tmA, tmB, p);
+  else simTensorKernel<kTcTopkTanimoto, 0><<<grid, kThreadsTC, smemBytes, s>>>(tmA, tmB, p);
+  B200_LAUNCHED();
 }
 
 }  // namespace b200
