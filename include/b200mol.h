@@ -68,6 +68,12 @@ int b200mol_free_async(void* d_ptr, void* stream);
  *                                  fingerprints and sends the rest through the tensor tile in column slabs that double,
  *                                  up to 512 MB of expanded operand; > 0: warm-up (at least B200MOL_TOPK_MAX) and every
  *                                  slab take this many fingerprints. Results identical
+ *   "maxmin_mode"                  b200mol_maxmin_pick: 0 (default) dense (every pick updates every item), 1 deferred
+ *                                  (RDKit's lazy bound: a round catches up only the items that could still win).
+ *                                  Results identical
+ *   "maxmin_resident_rows"         -1 (default): b200mol_maxmin_pick keeps the pool's fingerprints in shared memory
+ *                                  whenever they fit; 0: always reads them from L2 / HBM; > 0: keeps pools of at most
+ *                                  this many rows (that fit). Results identical
  *   "butina_min_round_commits"     a parallel Butina round that commits fewer clusters than this hands over to the
  *                                  one-cluster-per-step loop (default 32; 0 = rounds only, >= 1e9 = stepwise only)
  *   "etkdg_hessian_fp64"           0 (default): the embedder keeps its BFGS inverse Hessian in fp32 and sweeps it in fp32
@@ -84,7 +90,10 @@ int b200mol_set_option(const char* key, long long value);
  * (work units the host sized the grids for), "similarity_units_last" and "similarity_tiles_last" (units and tiles the
  * kernels counted; these two synchronise the device). Of the last b200mol_similarity_topk: "topk_slabs_last" (column slabs
  * that went through the tensor tile), "topk_candidates_last" (pairs its epilogue listed) and "topk_rows_redone_last" (rows
- * of a slab whose candidates did not fit and that the SIMT scan redid); the last two synchronise the device. */
+ * of a slab whose candidates did not fit and that the SIMT scan redid); the last two synchronise the device. Of the last
+ * b200mol_maxmin_pick: "maxmin_resident_last" (1: the pool was kept in shared memory), "maxmin_distances_last" (pair
+ * distances it evaluated) and "maxmin_popcount_skips_last" (pairs the popcount bound ruled out unread); the last two
+ * synchronise the device. */
 int b200mol_get_option(const char* key, long long* value);
 /* Per-phase CUDA-event timing inside the library (off by default). Phases: "neighbor_pass" (the N^2 tile kernel
  * alone), "csr_build", "cluster_loop", "bfgs". b200mol_profile_read waits for the phase's stop event. */
@@ -139,6 +148,21 @@ int b200mol_tanimoto_count_ge(const uint32_t* d_x, size_t nX, const uint32_t* d_
 #define B200MOL_TOPK_MAX 256
 int b200mol_similarity_topk(const uint32_t* d_q, size_t nQ, const uint32_t* d_lib, size_t nLib, int words, int metric,
                             int k, double* d_values /* [nQ][k] */, int32_t* d_indices /* [nQ][k] */, void* stream);
+
+/* MaxMin diversity picking (RDKit MaxMinPicker::LazyBitVectorPick / LazyBitVectorPickWithThreshold) over the pool
+ * d_fp[0 .. nPool) ([nPool][words], 16-byte aligned). d(i, j) = 1 - s(i, j), s the fp64 value b200mol_tanimoto_cross /
+ * b200mol_cosine_cross store for the pair (metric = B200MOL_METRIC_*), so two empty fingerprints are at distance 1.
+ * d_picks[0 .. nFirst) = h_first (host memory, 1 <= nFirst <= pickSize, distinct pool indices; a seeded random first
+ * pick is the caller's to draw); each further pick is the unpicked item with the largest min over the picks of d(i, p),
+ * ties to the lowest index. threshold >= 0: the loop stops before adding a pick whose max-min is <= threshold, and
+ * d_picks holds -1 past the stop; threshold < 0: no stop. *d_threshold = the max-min of the last pick the loop added,
+ * -1 when it added none. 1 <= pickSize <= nPool < 2^31. Asynchronous on `stream`, no host synchronisation (h_first is
+ * uploaded by one cudaMemcpyAsync from pageable memory); the pick loop is one cooperative kernel. Scratch is
+ * stream-ordered: 4 bytes per pool item (popcounts), 12 bytes per CTA, and, when a CTA's slice of the pool does not fit
+ * in shared memory (above about 1.9M items), 16 bytes per pool item of per-item state. */
+int b200mol_maxmin_pick(const uint32_t* d_fp, size_t nPool, int words, int metric, const int32_t* h_first, int nFirst,
+                        int pickSize, double threshold, int32_t* d_picks /* [pickSize] */, double* d_threshold /* [1] */,
+                        void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Butina clustering.  Definition (RDKit ML.Cluster.Butina.ClusterData(reordering=True), the CPU baseline the

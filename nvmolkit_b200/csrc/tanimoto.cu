@@ -320,6 +320,10 @@ void readWalkCounters(unsigned long long* units, unsigned long long* tiles);
 extern long long          g_topkSlabCols;
 extern unsigned long long g_topkSlabsLast;
 void readTopkStats(unsigned long long* candidates, unsigned long long* redone);
+extern int       g_maxminMode;
+extern long long g_maxminResidentRows;
+extern int       g_maxminResidentLast;
+void readMaxminStats(unsigned long long* evaluated, unsigned long long* skipped);
 long long g_tensorMinPairs = 1ll << 24;  // pair count from which the passes run on the tensor-core tile (< 0: never)
 
 void launchThreshTable(int maxS, double cutoff, uint16_t* thresh, cudaStream_t s) {
@@ -458,6 +462,11 @@ extern "C" int b200mol_set_option(const char* key, long long value) {
       B200_REQUIRE(value >= 0 && value < (1ll << 31), "topk_slab_cols must be in [0, 2^31)");
       g_topkSlabCols = value;
     }
+    else if (k == "maxmin_mode") {
+      B200_REQUIRE(value == 0 || value == 1, "maxmin_mode must be 0 (dense) or 1 (deferred)");
+      g_maxminMode = static_cast<int>(value);
+    }
+    else if (k == "maxmin_resident_rows") g_maxminResidentRows = value < 0 ? -1 : value;
     else if (k == "similarity_tensor_cluster") {
       B200_REQUIRE(value >= 0 && value <= 3, "similarity_tensor_cluster must be 0, 1, 2 or 3");
       g_tensorCluster = static_cast<int>(value);
@@ -498,6 +507,14 @@ extern "C" int b200mol_get_option(const char* key, long long* value) {
       unsigned long long listed = 0, redone = 0;
       readTopkStats(&listed, &redone);
       *value = static_cast<long long>(k == "topk_candidates_last" ? listed : redone);
+    }
+    else if (k == "maxmin_mode") *value = g_maxminMode;
+    else if (k == "maxmin_resident_rows") *value = g_maxminResidentRows;
+    else if (k == "maxmin_resident_last") *value = g_maxminResidentLast;  // read-only
+    else if (k == "maxmin_distances_last" || k == "maxmin_popcount_skips_last") {  // read-only; synchronises the device
+      unsigned long long evaluated = 0, skipped = 0;
+      readMaxminStats(&evaluated, &skipped);
+      *value = static_cast<long long>(k == "maxmin_distances_last" ? evaluated : skipped);
     }
     else if (k == "butina_min_round_commits") *value = g_butinaMinCommits;
     else fail(B200MOL_ERR_INVALID, "unknown option '%s'", key);
