@@ -74,6 +74,8 @@ int b200mol_free_async(void* d_ptr, void* stream);
  *   "maxmin_resident_rows"         -1 (default): b200mol_maxmin_pick keeps the pool's fingerprints in shared memory
  *                                  whenever they fit; 0: always reads them from L2 / HBM; > 0: keeps pools of at most
  *                                  this many rows (that fit). Results identical
+ *   "leader_window_rows"           0 (default): b200mol_leader_pick sizes each window of the pool so that about 8,192 items
+ *                                  survive its bulk pass; > 0: every window takes this many items. Results identical
  *   "butina_min_round_commits"     a parallel Butina round that commits fewer clusters than this hands over to the
  *                                  one-cluster-per-step loop (default 32; 0 = rounds only, >= 1e9 = stepwise only)
  *   "etkdg_hessian_fp64"           0 (default): the embedder keeps its BFGS inverse Hessian in fp32 and sweeps it in fp32
@@ -93,7 +95,10 @@ int b200mol_set_option(const char* key, long long value);
  * of a slab whose candidates did not fit and that the SIMT scan redid); the last two synchronise the device. Of the last
  * b200mol_maxmin_pick: "maxmin_resident_last" (1: the pool was kept in shared memory), "maxmin_distances_last" (pair
  * distances it evaluated) and "maxmin_popcount_skips_last" (pairs the popcount bound ruled out unread); the last two
- * synchronise the device. */
+ * synchronise the device. Of the last b200mol_leader_pick: "leader_windows_last" (windows of the pool it walked),
+ * "leader_bulk_pairs_last" (window x pick pairs sent through the count pass), "leader_window_pairs_last" and
+ * "leader_block_pairs_last" (pairs the resolver compared against earlier picks of the same window / of the same block;
+ * these two synchronise the device). */
 int b200mol_get_option(const char* key, long long* value);
 /* Per-phase CUDA-event timing inside the library (off by default). Phases: "neighbor_pass" (the N^2 tile kernel
  * alone), "csr_build", "cluster_loop", "bfgs". b200mol_profile_read waits for the phase's stop event. */
@@ -163,6 +168,21 @@ int b200mol_similarity_topk(const uint32_t* d_q, size_t nQ, const uint32_t* d_li
 int b200mol_maxmin_pick(const uint32_t* d_fp, size_t nPool, int words, int metric, const int32_t* h_first, int nFirst,
                         int pickSize, double threshold, int32_t* d_picks /* [pickSize] */, double* d_threshold /* [1] */,
                         void* stream);
+
+/* Leader (sphere-exclusion) diversity picking (RDKit LeaderPicker::LazyBitVectorPick) over the pool d_fp[0 .. nPool)
+ * ([nPool][words], 16-byte aligned). d(i, j) = 1 - s(i, j) as for b200mol_maxmin_pick; item j is covered by pick p iff
+ * d(p, j) <= threshold (the neighbour predicate of b200mol_tanimoto_count_ge with cutoff = threshold). d_picks[0 .. nFirst)
+ * = h_first (host memory, distinct pool indices, 0 <= nFirst <= pickSize; h_first may be null when nFirst = 0); every
+ * item that is a first pick or is covered by one leaves the pool; then, repeatedly, the lowest-index item left becomes
+ * the next pick, and it and every item it covers leave the pool, until the pool is empty or there are pickSize picks.
+ * *h_n_picks = the number of picks; d_picks past it is left as it was. 1 <= pickSize <= nPool < 2^31, 0 <= threshold <= 1.
+ * Picks are bitwise repeatable. Stream-ordered on `stream`, but the call synchronises it once per window of the pool
+ * (to size the next window from the survivor count) and returns after the last: *h_n_picks is valid on return. Scratch
+ * is stream-ordered: 5 bytes per pool item, 8 bytes per window item, 132 KB for the resolver's block, the picks' fingerprints (growing by doubling) and
+ * what the count pass takes per window. */
+int b200mol_leader_pick(const uint32_t* d_fp, size_t nPool, int words, int metric, double threshold, const int32_t* h_first,
+                        int nFirst, int pickSize /* >= 1: the cap */, int32_t* d_picks /* [pickSize] */,
+                        int32_t* h_n_picks, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Butina clustering.  Definition (RDKit ML.Cluster.Butina.ClusterData(reordering=True), the CPU baseline the

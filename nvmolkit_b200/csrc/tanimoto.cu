@@ -324,6 +324,10 @@ extern int       g_maxminMode;
 extern long long g_maxminResidentRows;
 extern int       g_maxminResidentLast;
 void readMaxminStats(unsigned long long* evaluated, unsigned long long* skipped);
+extern long long          g_leaderWindowRows;
+extern long long          g_leaderWindowsLast;
+extern unsigned long long g_leaderBulkPairsLast;
+void readLeaderStats(unsigned long long* window, unsigned long long* inBlock);
 long long g_tensorMinPairs = 1ll << 24;  // pair count from which the passes run on the tensor-core tile (< 0: never)
 
 void launchThreshTable(int maxS, double cutoff, uint16_t* thresh, cudaStream_t s) {
@@ -467,6 +471,10 @@ extern "C" int b200mol_set_option(const char* key, long long value) {
       g_maxminMode = static_cast<int>(value);
     }
     else if (k == "maxmin_resident_rows") g_maxminResidentRows = value < 0 ? -1 : value;
+    else if (k == "leader_window_rows") {
+      B200_REQUIRE(value >= 0 && value < (1ll << 31), "leader_window_rows must be in [0, 2^31)");
+      g_leaderWindowRows = value;
+    }
     else if (k == "similarity_tensor_cluster") {
       B200_REQUIRE(value >= 0 && value <= 3, "similarity_tensor_cluster must be 0, 1, 2 or 3");
       g_tensorCluster = static_cast<int>(value);
@@ -515,6 +523,14 @@ extern "C" int b200mol_get_option(const char* key, long long* value) {
       unsigned long long evaluated = 0, skipped = 0;
       readMaxminStats(&evaluated, &skipped);
       *value = static_cast<long long>(k == "maxmin_distances_last" ? evaluated : skipped);
+    }
+    else if (k == "leader_window_rows") *value = g_leaderWindowRows;
+    else if (k == "leader_windows_last") *value = g_leaderWindowsLast;                                   // read-only
+    else if (k == "leader_bulk_pairs_last") *value = static_cast<long long>(g_leaderBulkPairsLast);  // read-only
+    else if (k == "leader_window_pairs_last" || k == "leader_block_pairs_last") {  // read-only; synchronises the device
+      unsigned long long window = 0, inBlock = 0;
+      readLeaderStats(&window, &inBlock);
+      *value = static_cast<long long>(k == "leader_window_pairs_last" ? window : inBlock);
     }
     else if (k == "butina_min_round_commits") *value = g_butinaMinCommits;
     else fail(B200MOL_ERR_INVALID, "unknown option '%s'", key);

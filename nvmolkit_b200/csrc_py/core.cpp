@@ -123,6 +123,7 @@ PYBIND11_MODULE(_core, m) {
   DEF(b200mol_tanimoto_count_ge);
   DEF(b200mol_similarity_topk);
   DEF(b200mol_maxmin_pick);
+  DEF(b200mol_leader_pick);
   DEF(b200mol_butina_fused);
   DEF(b200mol_neighbor_edges);
   DEF(b200mol_butina_from_edges);

@@ -1,8 +1,10 @@
 """Diversity picking on fingerprints on the GPU. API of RDKit's ``rdkit.SimDivFilters.rdSimDivPickers.MaxMinPicker``
-(``LazyBitVectorPick`` / ``LazyBitVectorPickWithThreshold``), plus ``metric`` and ``stream``."""
+(``LazyBitVectorPick`` / ``LazyBitVectorPickWithThreshold``) and ``LeaderPicker`` (``LazyBitVectorPick``), plus
+``metric`` and ``stream``."""
 
 from __future__ import annotations
 
+import ctypes
 import secrets
 
 import torch
@@ -137,3 +139,54 @@ class MaxMinPicker:
         max-min distance of the last pick the loop added, -1.0 when it added none (the first picks filled
         ``pickSize``, or the first candidate was already within the threshold)."""
         return _pick(fingerprints, poolSize, pickSize, float(threshold), firstPicks, seed, metric, stream)
+
+
+def _leader_args(n: int, words: int, poolSize, threshold, pickSize, firstPicks, metric) -> tuple[int, float, list]:
+    """``MaxMinPicker``'s checks with ``pickSize = 0`` read as ``poolSize``, plus the threshold (in [0, 1], not NaN);
+    returns (the pick cap, the threshold, the first picks)."""
+    cap = poolSize if type(pickSize) is int and pickSize == 0 else pickSize
+    first = _check_args(n, words, poolSize, cap, firstPicks, metric)
+    try:
+        thr = float(threshold)
+    except (TypeError, ValueError):
+        raise ValueError(f"threshold must be a number in [0, 1], got {threshold!r}") from None
+    if not 0.0 <= thr <= 1.0:  # (also refuses NaN)
+        raise ValueError(f"threshold must be in [0, 1], got {thr}")
+    return cap, thr, first
+
+
+class LeaderPicker:
+    """Leader (sphere-exclusion) diversity picking of packed fingerprints on the GPU (RDKit's ``LeaderPicker``).
+
+    The pool and the distance are ``MaxMinPicker``'s: the first ``poolSize`` rows of ``fingerprints``, and ``1 - s``
+    with s the fp64 value ``crossTanimotoSimilarity`` / ``crossCosineSimilarity`` returns for the pair. Item j is covered
+    by pick p when ``1 - s(p, j) <= threshold``. Picks start with ``firstPicks`` in their order, and every item that is a
+    first pick or is covered by one leaves the pool; then, repeatedly, the lowest-index item left becomes the next pick,
+    and it and every item it covers leave the pool, until the pool is empty or there are ``pickSize`` picks
+    (``pickSize = 0``: no limit). Picks after the first ones therefore come in ascending index order. This restates
+    RDKit's ``LeaderPicker::lazyPick`` (each pick is the head of the remaining list, which is compacted to the items with
+    distance ``> threshold``); the tests pin this restatement, not RDKit itself.
+
+    Differences from RDKit: two empty fingerprints are at distance 1 here (similarity 0, the convention of the
+    similarity calls), at 0 in RDKit; a pick always leaves the pool itself, so an empty fingerprint is never picked twice.
+    A threshold outside [0, 1] or NaN, more ``firstPicks`` than a non-zero ``pickSize``, or a repeated first pick is a
+    ValueError. ``numThreads`` is accepted, so that RDKit call sites run unchanged, and ignored."""
+
+    def LazyBitVectorPick(self, fingerprints, poolSize, threshold, pickSize=0, firstPicks=(), numThreads=1,
+                          metric="tanimoto", stream=None) -> AsyncGpuResult:
+        """int32 ``[nPicks]`` pool indices in pick order.
+
+        The pick count is only known at the end, so this call synchronises ``stream``: it walks the pool in windows and
+        reads back each window's survivor and pick counts to size the next one. The result is complete on return."""
+        del numThreads  # (RDKit's thread count: the GPU call has none to set)
+        sptr = stream_ptr(stream)  # validates `stream` first, like the other calls (TypeError)
+        fp = fingerprint_matrix(fingerprints, "fingerprints")
+        cap, thr, first = _leader_args(fp.shape[0], fp.shape[1], poolSize, threshold, pickSize, firstPicks, metric)
+        require_cuda()
+        h_first = torch.tensor(first, dtype=torch.int32)
+        n = ctypes.c_int32(0)
+        with stream_ctx(stream):
+            picks = torch.empty(cap, dtype=torch.int32, device=fp.device)
+            _lib.call("b200mol_leader_pick", fp.data_ptr(), poolSize, fp.shape[1], _lib.METRIC[metric], thr,
+                      h_first.data_ptr() if first else None, len(first), cap, picks.data_ptr(), ctypes.addressof(n), sptr)
+        return AsyncGpuResult(picks[:n.value])
