@@ -154,6 +154,27 @@ int b200mol_tanimoto_count_ge(const uint32_t* d_x, size_t nX, const uint32_t* d_
 int b200mol_similarity_topk(const uint32_t* d_q, size_t nQ, const uint32_t* d_lib, size_t nLib, int words, int metric,
                             int k, double* d_values /* [nQ][k] */, int32_t* d_indices /* [nQ][k] */, void* stream);
 
+/* Threshold (range) similarity search, the similarity matrix never materialised: row q of the CSR result (d_indptr
+ * [nQ + 1], d_indices / d_values [nnz]) lists exactly the columns j for which the fp64 value b200mol_tanimoto_cross /
+ * b200mol_cosine_cross would store for (q, j) is >= threshold, in ascending column order, with values bit-identical to
+ * those matrix entries; the result is a pure function of the inputs. d_lib = NULL searches the queries against
+ * themselves (nLib is then ignored): the same result as passing them twice, self-matches included (1.0 for a non-empty
+ * fingerprint, 0 for an empty one), from the symmetric pass over half the pairs. 0 < threshold <= 1, metric =
+ * B200MOL_METRIC_*, nQ, nLib < 2^31, inputs 16-byte aligned and borrowed; arguments are checked before any device work.
+ * *h_nnz = the true total nnz, always. d_indptr, d_indices and d_values are written only when nnz <= cap (the caller
+ * sizes them for cap); otherwise nothing is written and the caller calls again with cap >= *h_nnz.
+ * The output size is data-dependent, so the call SYNCHRONISES `stream`: once to read the listed-pair total, and once
+ * more in the rare case that the pass listed more pairs than its buffer held and is rerun; the CSR is then written
+ * stream-ordered on `stream`. Tanimoto runs the thresholded graph pass of the fused Butina path (symmetric for a self
+ * search; superposed and in popcount order on the tensor-core tile), cosine a list mode of the tile (SIMT below
+ * "similarity_tensor_min_pairs" pairs). Scratch is stream-ordered: 16 bytes per listed pair (the pair and its value; a
+ * self search lists each off-diagonal pair once), 24 bytes per result entry plus CUB's radix-sort temporary storage
+ * (about another 16 bytes per entry), 12 bytes per fingerprint, and what the pass itself takes (the tensor tile: 8 bits
+ * per fingerprint bit of expanded operand). */
+int b200mol_similarity_threshold(const uint32_t* d_q, size_t nQ, const uint32_t* d_lib /* NULL = self */, size_t nLib, int words,
+                                 int metric, double threshold, int64_t* d_indptr /* [nQ + 1] */, int32_t* d_indices /* [cap] */,
+                                 double* d_values /* [cap] */, uint64_t cap, uint64_t* h_nnz, void* stream);
+
 /* MaxMin diversity picking (RDKit MaxMinPicker::LazyBitVectorPick / LazyBitVectorPickWithThreshold) over the pool
  * d_fp[0 .. nPool) ([nPool][words], 16-byte aligned). d(i, j) = 1 - s(i, j), s the fp64 value b200mol_tanimoto_cross /
  * b200mol_cosine_cross store for the pair (metric = B200MOL_METRIC_*), so two empty fingerprints are at distance 1.

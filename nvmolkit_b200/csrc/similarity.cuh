@@ -12,6 +12,8 @@ enum SimMode : int {
   kMaterialiseCosine   = 1,
   kCountTanimoto       = 2,  // thresholded neighbour counts (+ optional edge list)
   kCountCosine         = 3,
+  kListCosine          = 4,  // edges only: every pair with sim >= cutoff, possibly with false positives (tensor tile:
+                             // a float bound, unordered; the SIMT fallback runs kCountCosine and lists exactly)
 };
 
 struct SimLaunch {
@@ -24,12 +26,13 @@ struct SimLaunch {
   double* out = nullptr;  // [nX][nY]
   // count
   double   cutoff      = 0.0;      // neighbour iff 1 - sim <= cutoff (fp64)
+  bool     atLeast     = false;    // ... or, when set, iff sim >= cutoff (fp64; the threshold search)
   int      sign        = 1;        // counts += sign * hits
   int32_t* rowCounts   = nullptr;  // [nX]
   bool     symmetric   = false;    // x == y: visit tiles tn >= tm only, skip the diagonal pairs, update both endpoints
   uint32_t groupOffset = 0;        // multi-GPU row sharding: this call covers tile-row groups (32 x 128 rows each)
   uint32_t groupStride = 1;        //   groupOffset, groupOffset + groupStride, ...
-  int2*    edges       = nullptr;  // optional (symmetric only): (i<j) neighbour pairs appended here
+  int2*    edges       = nullptr;  // optional: neighbour pairs (i, j) appended here (symmetric: i < j)
   unsigned long long* edgeCursor = nullptr;  // device counter; entries beyond edgeCap are dropped (cursor still advances)
   unsigned long long  edgeCap    = 0;
 };

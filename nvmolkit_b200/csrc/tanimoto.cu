@@ -40,6 +40,7 @@ struct TileParams {
   double*        out;
   const uint16_t* thresh;  // Tanimoto count: min intersection for a hit, indexed by |A|+|B|
   double          cutoff;
+  int             atLeast;  // the predicate is sim >= cutoff (else 1 - sim <= cutoff)
   int             sign;
   int32_t*        rowCounts;
   int             symmetric;
@@ -64,7 +65,8 @@ __global__ void rowPopcountKernel(const uint32_t* __restrict__ fp, size_t n, int
 // `1.0 - sim <= cutoff` holds with sim = (c == 0 || u == 0) ? 0 : c/u, u = s - c. 0xFFFF = never.
 // The predicate is monotone in c, so the hot loop tests `c >= thresh[s]` with integers and stays bit-identical to the
 // fp64 evaluation a CPU makes.
-__global__ void threshTableKernel(int maxS, double cutoff, uint16_t* __restrict__ thresh) {
+// atLeast: the threshold search's predicate `sim >= cutoff` instead (cutoff in (0, 1]: c = 0 never passes).
+__global__ void threshTableKernel(int maxS, double cutoff, int atLeast, uint16_t* __restrict__ thresh) {
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
   if (s > maxS) return;
   // explicit round-to-nearest intrinsics: never contracted into an FMA, so the result is the two-rounding value a CPU
@@ -72,12 +74,17 @@ __global__ void threshTableKernel(int maxS, double cutoff, uint16_t* __restrict_
   auto passes = [&](int c) {
     const int    u   = s - c;
     const double sim = (c == 0 || u == 0) ? 0.0 : __ddiv_rn(static_cast<double>(c), static_cast<double>(u));
-    return __dsub_rn(1.0, sim) <= cutoff;
+    return atLeast ? sim >= cutoff : __dsub_rn(1.0, sim) <= cutoff;
   };
   // c/(s - c) grows with c and correctly rounded division and subtraction keep the order, so the smallest passing c is
-  // found by bisection over [0, s/2] (a linear scan cost 0.2 ms per table: 2048 dependent fp64 divisions per thread)
+  // found by bisection over [0, s/2] ([1, s/2] for atLeast) (a linear scan cost 0.2 ms per table: 2048 dependent fp64
+  // divisions per thread)
   int found = 0xFFFF;
-  int lo = 0, hi = s / 2;
+  int lo = atLeast ? 1 : 0, hi = s / 2;
+  if (hi < lo) {
+    thresh[s] = static_cast<uint16_t>(found);
+    return;
+  }
   if (passes(hi)) {
     while (lo < hi) {
       const int mid = (lo + hi) >> 1;
@@ -228,7 +235,7 @@ __global__ void __launch_bounds__(kThreads, 2)
             (c == 0) ? 0.0
                      : __ddiv_rn(static_cast<double>(c),
                                  __dsqrt_rn(__dmul_rn(static_cast<double>(pa[i]), static_cast<double>(pb[j]))));
-          h = (__dsub_rn(1.0, sim) <= p.cutoff);
+          h = p.atLeast ? sim >= p.cutoff : (__dsub_rn(1.0, sim) <= p.cutoff);
         }
         if (ok && h) hits |= 1ull << (i * 8 + j);
       }
@@ -330,8 +337,8 @@ extern unsigned long long g_leaderBulkPairsLast;
 void readLeaderStats(unsigned long long* window, unsigned long long* inBlock);
 long long g_tensorMinPairs = 1ll << 24;  // pair count from which the passes run on the tensor-core tile (< 0: never)
 
-void launchThreshTable(int maxS, double cutoff, uint16_t* thresh, cudaStream_t s) {
-  threshTableKernel<<<(maxS + 1 + 127) / 128, 128, 0, s>>>(maxS, cutoff, thresh);
+void launchThreshTable(int maxS, double cutoff, bool atLeast, uint16_t* thresh, cudaStream_t s) {
+  threshTableKernel<<<(maxS + 1 + 127) / 128, 128, 0, s>>>(maxS, cutoff, atLeast ? 1 : 0, thresh);
   B200_LAUNCHED();
 }
 
@@ -370,6 +377,7 @@ void launchSimilarity(SimMode mode, const SimLaunch& q, cudaStream_t s) {
   tp.tilesN     = static_cast<uint32_t>((q.nY + kBN - 1) / kBN);
   tp.out        = q.out;
   tp.cutoff     = q.cutoff;
+  tp.atLeast    = q.atLeast ? 1 : 0;
   tp.sign       = q.sign;
   tp.rowCounts  = q.rowCounts;
   tp.symmetric  = q.symmetric ? 1 : 0;
@@ -396,7 +404,7 @@ void launchSimilarity(SimMode mode, const SimLaunch& q, cudaStream_t s) {
   if (mode == kCountTanimoto) {
     const int maxS = 2 * q.words * 32;
     thresh         = Scratch<uint16_t>(maxS + 1, s);
-    threshTableKernel<<<(maxS + 1 + 127) / 128, 128, 0, s>>>(maxS, q.cutoff, thresh.get());
+    threshTableKernel<<<(maxS + 1 + 127) / 128, 128, 0, s>>>(maxS, q.cutoff, q.atLeast ? 1 : 0, thresh.get());
     B200_LAUNCHED();
     tp.thresh = thresh.get();
   }
@@ -407,7 +415,8 @@ void launchSimilarity(SimMode mode, const SimLaunch& q, cudaStream_t s) {
     case kMaterialiseTanimoto: launchTile<kMaterialiseTanimoto>(tmX, tmY, tp, smemBytes, s); break;
     case kMaterialiseCosine: launchTile<kMaterialiseCosine>(tmX, tmY, tp, smemBytes, s); break;
     case kCountTanimoto: launchTile<kCountTanimoto>(tmX, tmY, tp, smemBytes, s); break;
-    case kCountCosine: launchTile<kCountCosine>(tmX, tmY, tp, smemBytes, s); break;
+    case kCountCosine:
+    case kListCosine: launchTile<kCountCosine>(tmX, tmY, tp, smemBytes, s); break;  // (exact: lists no false positive)
   }
 }
 

@@ -107,7 +107,7 @@ struct TcParams {
 // row group whose largest popcount is A, no column past the first one this cuts can be a neighbour of any of its rows.
 __host__ __device__ __forceinline__ bool bandCuts(const uint16_t* tmin, int A, int b) { return tmin[A + b] > A; }
 
-enum TcMode : int { kTcCount = 0, kTcTanimoto = 1, kTcCosine = 2, kTcTopkTanimoto = 3, kTcTopkCosine = 4 };
+enum TcMode : int { kTcCount = 0, kTcTanimoto = 1, kTcCosine = 2, kTcTopkTanimoto = 3, kTcTopkCosine = 4, kTcListCosine = 5 };
 }  // namespace
 int g_tensorCluster = 1;  // count tile in clusters of two CTAs with a multicast column operand (option "similarity_tensor_cluster":
                           // 0 one CTA per tile, 1 the pair, 2 the pair too (kept for callers written for the CTA-pair MMA
@@ -342,6 +342,15 @@ __global__ void __launch_bounds__(kBandThreads) popcountBandKernel(const int32_t
   }
 }
 
+// The cosine list tile's metadata: {popcount, float bits of scale sqrt(popcount)} per operand row, whole tiles; rows past
+// the end get popcount 0 and 3e38, which no count reaches
+__global__ void listMetaKernel(const int32_t* __restrict__ pop, size_t n, size_t nPad, float scale, int2* __restrict__ out) {
+  const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= nPad) return;
+  if (i >= n) out[i] = make_int2(0, __float_as_int(3.0e38f));
+  else out[i] = make_int2(pop[i], __float_as_int(scale * sqrtf(static_cast<float>(pop[i]))));
+}
+
 __global__ void recipTableKernel(double* __restrict__ r, int len) {  // r[u] = RN(1 / u), r[0] = 0
   const int u = blockIdx.x * blockDim.x + threadIdx.x;
   if (u <= len) r[u] = u ? __drcp_rn(static_cast<double>(u)) : 0.0;
@@ -567,6 +576,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
   static_assert(!CL || MODE == kTcCount, "the two-CTA cluster is wired for the count tile");
   constexpr bool COUNT = MODE == kTcCount;
   constexpr bool TOPK  = MODE == kTcTopkTanimoto || MODE == kTcTopkCosine;
+  constexpr bool LIST  = MODE == kTcListCosine;  // edges only, through the same per-warp staging as the count mode
   constexpr bool ST    = CL == 3;  // row operand stationary
   using Walk           = UnitWalk<CL != 0, ST ? kRunStat : 1>;
   constexpr int  kStg       = ST ? kStagesStat : kStages;
@@ -579,7 +589,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
   __shared__ uint64_t metaFull[2], metaEmpty[2];
   __shared__ __align__(16) int2 colMeta[2][kTN];
   __shared__ __align__(16) int2 rowMeta[2][kTM];
-  __shared__ int2 pairSlots[COUNT ? 8 : 1][COUNT ? kStagePairs : 1];  // count mode: each epilogue warp's PairStage
+  __shared__ int2 pairSlots[COUNT || LIST ? 8 : 1][COUNT || LIST ? kStagePairs : 1];  // count / list: each epilogue warp's PairStage
   __shared__ uint32_t walkCount[2];  // units the producer walked, tiles it ran (in shared memory: no register to spare)
 
   const uint32_t rank      = CL ? clusterCtaRank() : 0u;
@@ -882,6 +892,49 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
                 if (at < p.topkCap) p.topkCand[static_cast<size_t>(r) * p.topkCap + at] = p.topkColBase + c;
               }
           }
+        } else if constexpr (LIST) {
+          // Cosine listing (threshold search, threshold.cu): can c / sqrt(|A| |B|) reach t? Tested as
+          // float(c) >= tLow sqrt|A| sqrt|B| with tLow 1e-5 (relative) below t, far more than the few 2^-24 the float
+          // square roots and products can err by, so every pair whose fp64 value is >= t is listed; the assembly re-counts
+          // each listed pair and drops the near misses. rowMeta .y = float bits of tLow sqrt|A|, colMeta .y = those of
+          // sqrt|B| (3e38 past the end). An empty intersection never reaches t > 0.
+          const float rt0 = __int_as_float(ra0.y), rt1 = __int_as_float(ra1.y);
+          auto pass = [&](int e, int a, int sq) {  // (the count through the 2^23 trick, exact and no I2F)
+            return a != 0 && fmaf(-(e < 2 ? rt0 : rt1), __int_as_float(sq), __int_as_float(0x4b000000 | a) - 8388608.0f) >= 0.0f;
+          };
+          bool any = false;
+#pragma unroll
+          for (int j = 0; j < 32; ++j) {
+            const int4 ci = cm[4 * j];
+            any |= pass(0, static_cast<int>(acc[4 * j]), ci.y) | pass(1, static_cast<int>(acc[4 * j + 1]), ci.w) |
+                   pass(2, static_cast<int>(acc[4 * j + 2]), ci.y) | pass(3, static_cast<int>(acc[4 * j + 3]), ci.w);
+          }
+          if (__any_sync(0xffffffffu, any)) {
+            // survivors as bits 4 (j % 8) + e of sv[j / 8] in one unrolled pass, listed in a rolled loop over the column
+            // blocks that hold any (as the superposed count epilogue does)
+            uint32_t sv[4] = {0, 0, 0, 0}, blocks = 0;
+#pragma unroll
+            for (int j = 0; j < 32; ++j) {
+              const int4 ci  = ldsFresh(cm + 4 * j);
+              uint32_t   nib = 0;
+#pragma unroll
+              for (int e = 0; e < 4; ++e)
+                if (pass(e, static_cast<int>(acc[4 * j + e]), (e & 1) ? ci.w : ci.y)) nib |= 1u << e;
+              sv[j >> 3] |= nib << (4 * (j & 7));
+              if (nib) blocks |= 1u << j;
+            }
+            for (uint32_t todo = __reduce_or_sync(0xffffffffu, blocks); todo; todo &= todo - 1) {
+              const int      j   = __ffs(todo) - 1;
+              const uint32_t nib = ((j < 8 ? sv[0] : j < 16 ? sv[1] : j < 24 ? sv[2] : sv[3]) >> (4 * (j & 7))) & 0xFu;
+              uint32_t       bits = 0;
+#pragma unroll
+              for (int e = 0; e < 4; ++e) {
+                const uint32_t r = e < 2 ? r0 : r1, c = c0 + 8 * j + (e & 1);
+                if ((nib >> e) & 1u && r < p.n && c < p.nY && (!p.symmetric || r < c)) bits |= 1u << e;
+              }
+              if (__any_sync(0xffffffffu, bits != 0)) pairs.add(p, pairSlots[warp - 4], bits, r0, r1, c0 + 8 * j, lane);
+            }
+          }
         } else {
           // fp64 Tanimoto / cosine straight from the accumulators: a quad of lanes writes 64 contiguous bytes of a row
 #pragma unroll
@@ -931,7 +984,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
       }
       aPhase ^= 1;
     }
-    if constexpr (COUNT) {
+    if constexpr (COUNT || LIST) {
       B200_TC_T0(tFlush);
       pairs.flush(p, pairSlots[warp - 4], lane);  // (n stays 0 when the pass lists nothing)
       B200_TC_T1(tFlush, 4);
@@ -949,7 +1002,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
 }  // namespace
 
 void launchRowPopcount(const uint32_t* fp, size_t n, int words, int32_t* pop, cudaStream_t s);
-void launchThreshTable(int maxS, double cutoff, uint16_t* thresh, cudaStream_t s);
+void launchThreshTable(int maxS, double cutoff, bool atLeast, uint16_t* thresh, cudaStream_t s);
 
 // A fingerprint set in popcount order: row i of fp is the caller's row perm[i], pop its popcount; ascending, ties in the
 // caller's order (CUB's radix sort is stable), so the same input always gives the same order.
@@ -1155,9 +1208,10 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
     p.recipG = recip.get();
   }
   {
-    // a pair passes iff 1 - c / (|A| + |B| - c) <= cutoff, i.e. c >= alpha (|A| + |B|); the pre-filter's alpha is rounded
-    // DOWN (and its products too), so it never rejects what the exact fp64 table accepts
-    const double a  = q.cutoff < 2.0 ? (1.0 - q.cutoff) / (2.0 - q.cutoff) : 0.0;
+    // a pair passes iff 1 - c / (|A| + |B| - c) <= cutoff, i.e. c >= alpha (|A| + |B|) - or, for the threshold search's
+    // c / (|A| + |B| - c) >= t, with alpha = t / (1 + t); the pre-filter's alpha is rounded DOWN (and its products
+    // too), so it never rejects what the exact fp64 table accepts
+    const double a  = q.atLeast ? q.cutoff / (1.0 + q.cutoff) : q.cutoff < 2.0 ? (1.0 - q.cutoff) / (2.0 - q.cutoff) : 0.0;
     float        af = static_cast<float>(a);
     if (static_cast<double>(af) > a) af = nextafterf(af, -1.0f);
     p.alpha = nextafterf(af, -1.0f);  // (one more ulp: fp64 rounding inside the table's predicate)
@@ -1214,12 +1268,22 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
   // tile of a CTA pair may lie one tile row past the end)
   const size_t  rowsPad = (static_cast<size_t>(p.tilesM) + 1) * kTM, colsPad = static_cast<size_t>(p.tilesN) * kTN;
   Scratch<int2> rowMeta(rowsPad, s), colMeta(colsPad, s);
-  tileMetaKernel<<<static_cast<unsigned>((rowsPad + 255) / 256), 256, 0, s>>>(popXs, q.nX, superS, nSuper, rowsPad, p.alpha, 1,
-                                                                             rowMeta.get());
-  B200_LAUNCHED();
-  tileMetaKernel<<<static_cast<unsigned>((colsPad + 255) / 256), 256, 0, s>>>(popYs, q.nY, superC, nSuperY, colsPad, p.alpha, -1,
-                                                                             colMeta.get());
-  B200_LAUNCHED();
+  if (mode == kListCosine) {
+    // the list tile's bound: tLow = t (1 - 1e-5), rounded down
+    float tLow = static_cast<float>(q.cutoff * (1.0 - 1e-5));
+    if (static_cast<double>(tLow) > q.cutoff * (1.0 - 1e-5)) tLow = nextafterf(tLow, 0.0f);
+    listMetaKernel<<<static_cast<unsigned>((rowsPad + 255) / 256), 256, 0, s>>>(popXs, q.nX, rowsPad, tLow, rowMeta.get());
+    B200_LAUNCHED();
+    listMetaKernel<<<static_cast<unsigned>((colsPad + 255) / 256), 256, 0, s>>>(popYs, q.nY, colsPad, 1.0f, colMeta.get());
+    B200_LAUNCHED();
+  } else {
+    tileMetaKernel<<<static_cast<unsigned>((rowsPad + 255) / 256), 256, 0, s>>>(popXs, q.nX, superS, nSuper, rowsPad, p.alpha, 1,
+                                                                               rowMeta.get());
+    B200_LAUNCHED();
+    tileMetaKernel<<<static_cast<unsigned>((colsPad + 255) / 256), 256, 0, s>>>(popYs, q.nY, superC, nSuperY, colsPad, p.alpha, -1,
+                                                                               colMeta.get());
+    B200_LAUNCHED();
+  }
   p.rowMeta = rowMeta.get();
   p.colMeta = colMeta.get();
   // candidates of a superposed pass: (super row, super column) pairs the exact kernel re-examines. Sized for the
@@ -1238,7 +1302,7 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
   const int         maxS = 2 * bits;
   Scratch<uint16_t> thresh(static_cast<size_t>(maxS + 1), s);
   if (mode == kCountTanimoto) {
-    launchThreshTable(maxS, q.cutoff, thresh.get(), s);
+    launchThreshTable(maxS, q.cutoff, q.atLeast, thresh.get(), s);
     p.threshLen = maxS + 1;
   }
   p.thresh = thresh.get();
@@ -1279,6 +1343,7 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
     optIn(simTensorKernel<kTcCount, 3>);
     optIn(simTensorKernel<kTcTanimoto, 0>);
     optIn(simTensorKernel<kTcCosine, 0>);
+    optIn(simTensorKernel<kTcListCosine, 0>);
     configured[currentDeviceSlot()] = true;
   }
   // units a call owns: tiles, or vertical tile pairs (same enumeration as the kernel's UnitWalk)
@@ -1398,6 +1463,9 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
                                          q.edgeCursor, q.edgeCap);
       B200_LAUNCHED();
     }
+  } else if (mode == kListCosine) {
+    PhaseTimer t("threshold_list_tc", s);
+    simTensorKernel<kTcListCosine, 0><<<blocks, kThreadsTC, smemBytes, s>>>(tmA, tmB, p);
   } else if (mode == kMaterialiseTanimoto) {
     PhaseTimer t("cross_tc", s);
     simTensorKernel<kTcTanimoto, 0><<<blocks, kThreadsTC, smemBytes, s>>>(tmA, tmB, p);

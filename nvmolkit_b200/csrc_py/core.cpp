@@ -122,6 +122,7 @@ PYBIND11_MODULE(_core, m) {
   DEF(b200mol_similarity_cross_host);
   DEF(b200mol_tanimoto_count_ge);
   DEF(b200mol_similarity_topk);
+  DEF(b200mol_similarity_threshold);
   DEF(b200mol_maxmin_pick);
   DEF(b200mol_leader_pick);
   DEF(b200mol_butina_fused);

@@ -2,6 +2,8 @@
 
 from __future__ import annotations
 
+import ctypes as C
+
 import numpy as np
 import torch
 
@@ -77,6 +79,73 @@ def topKTanimotoSimilarity(fingerprint_group_one, fingerprint_group_two=None, k=
 def topKCosineSimilarity(fingerprint_group_one, fingerprint_group_two=None, k=10, stream=None):
     """Cosine twin of ``topKTanimotoSimilarity``: rows of ``crossCosineSimilarity``."""
     return _topk("cosine", fingerprint_group_one, fingerprint_group_two, k, stream)
+
+
+def _check_threshold(threshold) -> float:
+    if isinstance(threshold, bool) or not isinstance(threshold, (int, float, np.integer, np.floating)):
+        raise ValueError(f"threshold must be a real number, got {type(threshold).__name__}")
+    t = float(threshold)
+    if not 0.0 < t <= 1.0:  # (NaN fails too)
+        raise ValueError(f"threshold must be in (0, 1] (got {threshold}); threshold 0 is the dense matrix: use the "
+                         "cross*Similarity calls")
+    return t
+
+
+def _threshold(metric: str, one, two, threshold, stream):
+    sptr = stream_ptr(stream)  # validates `stream` first, like the matrix calls (TypeError)
+    t = _check_threshold(threshold)
+    require_cuda()
+    a = fingerprint_matrix(one, "fingerprint_group_one")
+    b = None if two is None else fingerprint_matrix(two, "fingerprint_group_two")
+    if b is not None and a.shape[1] != b.shape[1]:
+        raise ValueError(f"fingerprint widths differ: {a.shape[1]} vs {b.shape[1]} words")
+    n_q, n_lib = a.shape[0], (a.shape[0] if b is None else b.shape[0])
+    with stream_ctx(stream):
+        if n_q == 0 or n_lib == 0:  # no pair (and an empty tensor's address may be 0, the C-ABI's "no library")
+            return (AsyncGpuResult(torch.zeros(n_q + 1, dtype=torch.int64, device=a.device)),
+                    AsyncGpuResult(torch.empty(0, dtype=torch.int32, device=a.device)),
+                    AsyncGpuResult(torch.empty(0, dtype=torch.float64, device=a.device)))
+        indptr = torch.empty(n_q + 1, dtype=torch.int64, device=a.device)
+        # a first guess at the result size; a larger result is reported and the call is made once more with room for it
+        cap = min(max(1 << 20, 64 * n_q), n_q * n_lib)
+        for _ in range(2):
+            indices = torch.empty(cap, dtype=torch.int32, device=a.device)
+            values = torch.empty(cap, dtype=torch.float64, device=a.device)
+            nnz = C.c_uint64(0)
+            _lib.call("b200mol_similarity_threshold", a.data_ptr(), n_q, None if b is None else b.data_ptr(), n_lib,
+                      a.shape[1], _lib.METRIC[metric], t, indptr.data_ptr(), indices.data_ptr(), values.data_ptr(), cap,
+                      C.byref(nnz), sptr)
+            if nnz.value <= cap:
+                break
+            cap = int(nnz.value)
+        # keep inputs alive until the stream has consumed them
+        a.record_stream(torch.cuda.current_stream())
+        if b is not None:
+            b.record_stream(torch.cuda.current_stream())
+    n = int(nnz.value)
+    return AsyncGpuResult(indptr), AsyncGpuResult(indices[:n]), AsyncGpuResult(values[:n])
+
+
+def thresholdTanimotoSimilarity(fingerprint_group_one, fingerprint_group_two=None, *, threshold, stream=None):
+    """Every pair at or above a Tanimoto threshold, as CSR: ``(indptr, indices, values)``, int64 ``[Q + 1]``, int32
+    ``[nnz]`` and fp64 ``[nnz]``. Row q (a fingerprint of group one) lists exactly the columns j (of group two; of group
+    one itself, self-matches included, when None) whose ``crossTanimotoSimilarity`` entry is ``>= threshold``, in
+    ascending column order, with values bit-identical to those matrix entries. The matrix is never stored.
+    ``0 < threshold <= 1``. The result size is data-dependent, so the call synchronises ``stream`` (the arrays it returns
+    are then written on ``stream``). As a sparse matrix::
+
+        indptr, indices, values = (r.torch() for r in thresholdTanimotoSimilarity(q, lib, threshold=0.7))
+        m = torch.sparse_csr_tensor(indptr, indices, values, size=(len(q), len(lib)))
+        m = scipy.sparse.csr_matrix((values.cpu().numpy(), indices.cpu().numpy(), indptr.cpu().numpy()),
+                                    shape=(len(q), len(lib)))
+    """
+    return _threshold("tanimoto", fingerprint_group_one, fingerprint_group_two, threshold, stream)
+
+
+def thresholdCosineSimilarity(fingerprint_group_one, fingerprint_group_two=None, *, threshold, stream=None):
+    """Cosine twin of ``thresholdTanimotoSimilarity``: the entries of ``crossCosineSimilarity`` that are
+    ``>= threshold``."""
+    return _threshold("cosine", fingerprint_group_one, fingerprint_group_two, threshold, stream)
 
 
 def _cross_host(metric: str, one, two, max_device_bytes: int = 0) -> np.ndarray:
