@@ -5,6 +5,7 @@ There is no CPU fallback: if the CUDA library is missing, or a call fails, this 
 
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import os
 
@@ -194,3 +195,17 @@ def stats_read(reset: bool = True) -> dict:
 
 def set_option(key: str, value: int) -> None:
     check(load().b200mol_set_option(key.encode(), int(value)))
+
+
+@contextlib.contextmanager
+def options(**values):
+    """Set library options for the body of a ``with`` block, then put back the values they had, also on an exception."""
+    saved = {}
+    try:
+        for key, value in values.items():
+            saved[key] = get_option(key)
+            set_option(key, value)
+        yield
+    finally:
+        for key, value in reversed(saved.items()):
+            set_option(key, value)

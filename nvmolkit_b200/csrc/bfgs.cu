@@ -14,6 +14,7 @@
 //     b200mol_schedule_waves) into per-warp shared-memory accumulators and reduced in a fixed order, the sweep's
 //     row / column sums likewise -> a minimisation is bit-reproducible run to run.
 #include "bfgs_device.cuh"
+#include "options.cuh"
 #include "profile.cuh"
 
 namespace b200 {

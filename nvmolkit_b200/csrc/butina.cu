@@ -24,6 +24,7 @@
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
+#include "options.cuh"
 #include "profile.cuh"
 #include "similarity.cuh"
 

@@ -119,6 +119,27 @@ inline int currentDeviceSlot() {
 
 inline cudaStream_t asStream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
 
+// Statistics counters of the kernels: `__device__ unsigned long long counters[N]`. The library is compiled without -rdc,
+// so a __device__ symbol is visible in its own translation unit only: these are instantiated in the file that defines it.
+template <size_t N>
+unsigned long long* deviceCounters(unsigned long long (&counters)[N]) {
+  void* ptr = nullptr;
+  B200_CUDA(cudaGetSymbolAddress(&ptr, counters));
+  return static_cast<unsigned long long*>(ptr);
+}
+template <size_t N>
+void resetDeviceCounters(unsigned long long (&counters)[N], cudaStream_t s) {
+  B200_CUDA(cudaMemsetAsync(deviceCounters(counters), 0, sizeof(counters), s));
+}
+// Word i once all work on the device has finished (synchronises the device).
+template <size_t N>
+unsigned long long readDeviceCounter(const unsigned long long (&counters)[N], int i) {
+  unsigned long long v[N] = {};
+  B200_CUDA(cudaDeviceSynchronize());
+  B200_CUDA(cudaMemcpyFromSymbol(v, counters, sizeof(v)));
+  return v[i];
+}
+
 // RAII: while alive, accesses of kernels launched on `s` to [ptr, ptr + bytes) are marked PERSISTING in L2 (the rest
 // streaming): the inverse-Hessian slabs of the minimiser kernels are re-read every iteration while the term tables only
 // stream through. Best effort - failures of the attribute calls are ignored (the kernels are correct without it).

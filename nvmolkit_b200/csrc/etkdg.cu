@@ -21,12 +21,11 @@
 // and lets a host Scheduler re-dispatch failures (src/etkdg_impl.cpp:111-159,286-312).
 #include "bfgs_device.cuh"
 #include "dgprep_device.cuh"
+#include "options.cuh"
 #include "profile.cuh"
 
 namespace b200 {
-extern int g_bfgsCtasPerSm;
-extern int g_bfgsL2Persist;
-int        g_etkdgHessianFp64 = 0;  // option "etkdg_hessian_fp64": the embedder's inverse Hessian in fp64 (default fp32)
+int g_etkdgHessianFp64 = 0;  // option "etkdg_hessian_fp64": the embedder's inverse Hessian in fp64 (default fp32)
 unsigned long long* pathBStats();
 namespace {
 

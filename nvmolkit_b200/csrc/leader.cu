@@ -49,6 +49,7 @@
 #include <cub/device/device_scan.cuh>
 #include <vector>
 
+#include "options.cuh"
 #include "similarity.cuh"
 
 namespace cg = cooperative_groups;
@@ -288,12 +289,7 @@ size_t resolveSmem(int chunks) {
 
 }  // namespace
 
-void readLeaderStats(unsigned long long* window, unsigned long long* inBlock) {
-  unsigned long long v[2] = {0, 0};
-  B200_CUDA(cudaDeviceSynchronize());
-  B200_CUDA(cudaMemcpyFromSymbol(v, g_leaderStat, sizeof(v)));
-  *window = v[0], *inBlock = v[1];
-}
+unsigned long long readLeaderStat(int i) { return readDeviceCounter(g_leaderStat, i); }
 
 }  // namespace b200
 
@@ -326,11 +322,7 @@ extern "C" int b200mol_leader_pick(const uint32_t* d_fp, size_t nPool, int words
     const bool   fixed = g_leaderWindowRows > 0;
     const int    maxWindow = static_cast<int>(std::min<long long>(n, fixed ? g_leaderWindowRows : kMaxWindow));
     g_leaderWindowsLast = 0, g_leaderBulkPairsLast = 0;
-    {
-      void* ptr = nullptr;
-      B200_CUDA(cudaGetSymbolAddress(&ptr, g_leaderStat));
-      B200_CUDA(cudaMemsetAsync(ptr, 0, sizeof(unsigned long long) * 2, s));
-    }
+    resetDeviceCounters(g_leaderStat, s);
 
     Scratch<int32_t> pop(nPool, s), counts(static_cast<size_t>(maxWindow) + 1, s), surv(maxWindow, s), count(2, s);
     Scratch<uint8_t> isFirst(nPool, s), covered(kBlock, s);

@@ -37,6 +37,7 @@
 #include <algorithm>
 #include <vector>
 
+#include "options.cuh"
 #include "similarity.cuh"
 
 namespace cg = cooperative_groups;
@@ -353,12 +354,7 @@ size_t staticSmem(const void* fn) {
 
 }  // namespace
 
-void readMaxminStats(unsigned long long* evaluated, unsigned long long* skipped) {
-  unsigned long long v[2] = {0, 0};
-  B200_CUDA(cudaDeviceSynchronize());
-  B200_CUDA(cudaMemcpyFromSymbol(v, g_maxminStat, sizeof(v)));
-  *evaluated = v[0], *skipped = v[1];
-}
+unsigned long long readMaxminStat(int i) { return readDeviceCounter(g_maxminStat, i); }
 
 }  // namespace b200
 
@@ -393,11 +389,7 @@ extern "C" int b200mol_maxmin_pick(const uint32_t* d_fp, size_t nPool, int words
     launchRowPopcount(d_fp, nPool, words, pop.get(), s);
     B200_CUDA(cudaMemcpyAsync(d_picks, h_first, sizeof(int32_t) * nFirst, cudaMemcpyHostToDevice, s));
     if (pickSize > nFirst) B200_CUDA(cudaMemsetAsync(d_picks + nFirst, 0xFF, sizeof(int32_t) * (pickSize - nFirst), s));
-    {
-      void* ptr = nullptr;
-      B200_CUDA(cudaGetSymbolAddress(&ptr, g_maxminStat));
-      B200_CUDA(cudaMemsetAsync(ptr, 0, sizeof(unsigned long long) * 2, s));
-    }
+    resetDeviceCounters(g_maxminStat, s);
 
     const int blocks = std::max(1, std::min(smCount(), (n + kMinSlice - 1) / kMinSlice));
     const int slice  = (n + blocks - 1) / blocks;

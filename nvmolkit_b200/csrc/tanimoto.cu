@@ -10,6 +10,7 @@
 // written from scratch (the reference stages with scalar 4-byte loads and an emulated b1 mma.sync).
 #include <cub/device/device_scan.cuh>
 
+#include "options.cuh"
 #include "profile.cuh"
 #include "similarity.cuh"
 #include "tma.cuh"
@@ -310,32 +311,6 @@ void launchTile(const CUtensorMap& tmX, const CUtensorMap& tmY, const TileParams
 }  // namespace
 
 bool launchSimilarityTensor(SimMode mode, const SimLaunch& q, cudaStream_t s);
-extern int g_bfgsCtasPerSm;
-extern int g_bfgsL2Persist;
-extern int g_etkdgHessianFp64;
-extern int g_butinaMinCommits;
-extern int g_tensorCluster;
-extern int g_superpose;
-extern int g_superposeLast;
-extern int g_superposeCols;
-extern int g_superposeAuto;
-extern int g_pipelineChunks;
-extern unsigned long long g_candidatesLast;
-extern int g_popcountBand;
-extern unsigned long long g_unitsPlanned;
-void readWalkCounters(unsigned long long* units, unsigned long long* tiles);
-extern long long          g_topkSlabCols;
-extern unsigned long long g_topkSlabsLast;
-void readTopkStats(unsigned long long* candidates, unsigned long long* redone);
-extern int       g_maxminMode;
-extern long long g_maxminResidentRows;
-extern int       g_maxminResidentLast;
-void readMaxminStats(unsigned long long* evaluated, unsigned long long* skipped);
-extern long long          g_leaderWindowRows;
-extern long long          g_leaderWindowsLast;
-extern unsigned long long g_leaderBulkPairsLast;
-void readLeaderStats(unsigned long long* window, unsigned long long* inBlock);
-long long g_tensorMinPairs = 1ll << 24;  // pair count from which the passes run on the tensor-core tile (< 0: never)
 
 void launchThreshTable(int maxS, double cutoff, bool atLeast, uint16_t* thresh, cudaStream_t s) {
   threshTableKernel<<<(maxS + 1 + 127) / 128, 128, 0, s>>>(maxS, cutoff, atLeast ? 1 : 0, thresh);
@@ -443,106 +418,6 @@ extern "C" int b200mol_profile_read(const char* phase, float* ms) {
     B200_REQUIRE(it != g_phases.end() && it->second.recorded, "phase '%s' was not recorded", phase);
     B200_CUDA(cudaEventSynchronize(it->second.stop));
     B200_CUDA(cudaEventElapsedTime(ms, it->second.start, it->second.stop));
-  });
-}
-
-extern "C" int b200mol_set_option(const char* key, long long value) {
-  return guarded([&] {
-    B200_REQUIRE(key, "null key");
-    const std::string k(key);
-    if (k == "similarity_tensor_min_pairs") g_tensorMinPairs = value;
-    else if (k == "bfgs_ctas_per_sm") {
-      B200_REQUIRE(value >= 1 && value <= 8, "bfgs_ctas_per_sm must be in [1, 8]");
-      g_bfgsCtasPerSm = static_cast<int>(value);
-    }
-    else if (k == "bfgs_l2_persist") g_bfgsL2Persist = value != 0;
-    else if (k == "etkdg_hessian_fp64") g_etkdgHessianFp64 = value != 0;
-    else if (k == "similarity_superpose") {
-      B200_REQUIRE(value == 1 || value == 2 || value == 4, "similarity_superpose must be 1, 2 or 4");
-      g_superpose = static_cast<int>(value);
-    }
-    else if (k == "similarity_superpose_cols") {
-      B200_REQUIRE(value == 1 || value == 2 || value == 4, "similarity_superpose_cols must be 1, 2 or 4");
-      g_superposeCols = static_cast<int>(value);
-    }
-    else if (k == "similarity_superpose_auto") g_superposeAuto = value != 0;
-    else if (k == "similarity_pipeline_chunks") {
-      B200_REQUIRE(value >= 1 && value <= 8, "similarity_pipeline_chunks must be in [1, 8]");
-      g_pipelineChunks = static_cast<int>(value);
-    }
-    else if (k == "similarity_popcount_band") g_popcountBand = value != 0;
-    else if (k == "topk_slab_cols") {
-      B200_REQUIRE(value >= 0 && value < (1ll << 31), "topk_slab_cols must be in [0, 2^31)");
-      g_topkSlabCols = value;
-    }
-    else if (k == "maxmin_mode") {
-      B200_REQUIRE(value == 0 || value == 1, "maxmin_mode must be 0 (dense) or 1 (deferred)");
-      g_maxminMode = static_cast<int>(value);
-    }
-    else if (k == "maxmin_resident_rows") g_maxminResidentRows = value < 0 ? -1 : value;
-    else if (k == "leader_window_rows") {
-      B200_REQUIRE(value >= 0 && value < (1ll << 31), "leader_window_rows must be in [0, 2^31)");
-      g_leaderWindowRows = value;
-    }
-    else if (k == "similarity_tensor_cluster") {
-      B200_REQUIRE(value >= 0 && value <= 3, "similarity_tensor_cluster must be 0, 1, 2 or 3");
-      g_tensorCluster = static_cast<int>(value);
-    }
-    else if (k == "butina_min_round_commits") {
-      B200_REQUIRE(value >= 0, "butina_min_round_commits must be >= 0");
-      g_butinaMinCommits = static_cast<int>(value > 1000000000 ? 1000000000 : value);  // huge = stepwise loop only
-    }
-    else fail(B200MOL_ERR_INVALID, "unknown option '%s'", key);
-  });
-}
-
-extern "C" int b200mol_get_option(const char* key, long long* value) {
-  return guarded([&] {
-    B200_REQUIRE(key && value, "null pointer");
-    const std::string k(key);
-    if (k == "similarity_tensor_min_pairs") *value = g_tensorMinPairs;
-    else if (k == "bfgs_ctas_per_sm") *value = g_bfgsCtasPerSm;
-    else if (k == "bfgs_l2_persist") *value = g_bfgsL2Persist;
-    else if (k == "etkdg_hessian_fp64") *value = g_etkdgHessianFp64;
-    else if (k == "similarity_tensor_cluster") *value = g_tensorCluster;
-    else if (k == "similarity_superpose") *value = g_superpose;
-    else if (k == "similarity_superpose_cols") *value = g_superposeCols;
-    else if (k == "similarity_superpose_auto") *value = g_superposeAuto;
-    else if (k == "similarity_pipeline_chunks") *value = g_pipelineChunks;
-    else if (k == "similarity_candidates_last") *value = static_cast<long long>(g_candidatesLast);
-    else if (k == "similarity_superpose_last") *value = g_superposeLast;  // read-only: pairs per accumulator of the last pass
-    else if (k == "similarity_popcount_band") *value = g_popcountBand;
-    else if (k == "similarity_units_planned_last") *value = static_cast<long long>(g_unitsPlanned);  // read-only
-    else if (k == "similarity_units_last" || k == "similarity_tiles_last") {  // read-only; synchronises the device
-      unsigned long long units = 0, tiles = 0;
-      readWalkCounters(&units, &tiles);
-      *value = static_cast<long long>(k == "similarity_units_last" ? units : tiles);
-    }
-    else if (k == "topk_slab_cols") *value = g_topkSlabCols;
-    else if (k == "topk_slabs_last") *value = static_cast<long long>(g_topkSlabsLast);  // read-only
-    else if (k == "topk_candidates_last" || k == "topk_rows_redone_last") {  // read-only; synchronises the device
-      unsigned long long listed = 0, redone = 0;
-      readTopkStats(&listed, &redone);
-      *value = static_cast<long long>(k == "topk_candidates_last" ? listed : redone);
-    }
-    else if (k == "maxmin_mode") *value = g_maxminMode;
-    else if (k == "maxmin_resident_rows") *value = g_maxminResidentRows;
-    else if (k == "maxmin_resident_last") *value = g_maxminResidentLast;  // read-only
-    else if (k == "maxmin_distances_last" || k == "maxmin_popcount_skips_last") {  // read-only; synchronises the device
-      unsigned long long evaluated = 0, skipped = 0;
-      readMaxminStats(&evaluated, &skipped);
-      *value = static_cast<long long>(k == "maxmin_distances_last" ? evaluated : skipped);
-    }
-    else if (k == "leader_window_rows") *value = g_leaderWindowRows;
-    else if (k == "leader_windows_last") *value = g_leaderWindowsLast;                                   // read-only
-    else if (k == "leader_bulk_pairs_last") *value = static_cast<long long>(g_leaderBulkPairsLast);  // read-only
-    else if (k == "leader_window_pairs_last" || k == "leader_block_pairs_last") {  // read-only; synchronises the device
-      unsigned long long window = 0, inBlock = 0;
-      readLeaderStats(&window, &inBlock);
-      *value = static_cast<long long>(k == "leader_window_pairs_last" ? window : inBlock);
-    }
-    else if (k == "butina_min_round_commits") *value = g_butinaMinCommits;
-    else fail(B200MOL_ERR_INVALID, "unknown option '%s'", key);
   });
 }
 

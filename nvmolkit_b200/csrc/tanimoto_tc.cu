@@ -32,6 +32,7 @@
 #include <cub/device/device_radix_sort.cuh>
 #include <vector>
 
+#include "options.cuh"
 #include "profile.cuh"
 #include "similarity.cuh"
 #include "tma.cuh"
@@ -1051,21 +1052,11 @@ unsigned long long g_unitsPlanned = 0;
 namespace {
 __device__ unsigned long long g_walkedDev[2];  // [0] units, [1] tiles (TcParams::walked)
 }
-static unsigned long long* walkCounters() {
-  void* ptr = nullptr;
-  B200_CUDA(cudaGetSymbolAddress(&ptr, g_walkedDev));
-  return static_cast<unsigned long long*>(ptr);
-}
 static void resetWalkCounters(cudaStream_t s) {
   g_unitsPlanned = 0;
-  B200_CUDA(cudaMemsetAsync(walkCounters(), 0, 2 * sizeof(unsigned long long), s));
+  resetDeviceCounters(g_walkedDev, s);
 }
-void readWalkCounters(unsigned long long* units, unsigned long long* tiles) {
-  unsigned long long v[2] = {0, 0};
-  B200_CUDA(cudaDeviceSynchronize());
-  B200_CUDA(cudaMemcpyFromSymbol(v, g_walkedDev, sizeof(v)));
-  *units = v[0], *tiles = v[1];
-}
+unsigned long long readWalkCounter(int i) { return readDeviceCounter(g_walkedDev, i); }
 
 static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, int superS, int superC, bool ordered,
                              bool* overflow, unsigned long long* pilotCand = nullptr, double* pilotPairs = nullptr);
@@ -1321,7 +1312,7 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
     p.bandEnd = band.get();
   }
   const uint32_t* bandH = banded ? bandHost.data() : nullptr;
-  if (count) p.walked = walkCounters();
+  if (count) p.walked = deviceCounters(g_walkedDev);
 
   CUtensorMap tmA, tmB;
   makeTensorMap2D(&tmA, expX.get(), nSuper, rowBytes, kTM, kTK, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1);

@@ -23,12 +23,12 @@
 // anything back, so all of it is enqueued unconditionally and the redo kernels return at once for unmarked rows.
 #include <algorithm>
 
+#include "options.cuh"
 #include "similarity.cuh"
 
 namespace b200 {
 
 long long          g_topkSlabCols = 0;  // option "topk_slab_cols": columns per slab (and of the warm-up); 0 = automatic
-extern long long   g_tensorMinPairs;
 unsigned long long g_topkSlabsLast = 0;  // slabs the last call ran through the tensor tile ("topk_slabs_last")
 
 namespace {
@@ -207,20 +207,9 @@ __global__ void __launch_bounds__(kSelThreads) topkSelectKernel(const TopkArgs a
   }
 }
 
-void resetStats(cudaStream_t s) {
-  void* ptr = nullptr;
-  B200_CUDA(cudaGetSymbolAddress(&ptr, g_topkStat));
-  B200_CUDA(cudaMemsetAsync(ptr, 0, sizeof(g_topkStat), s));
-}
-
 }  // namespace
 
-void readTopkStats(unsigned long long* candidates, unsigned long long* redone) {
-  unsigned long long v[2] = {0, 0};
-  B200_CUDA(cudaDeviceSynchronize());
-  B200_CUDA(cudaMemcpyFromSymbol(v, g_topkStat, sizeof(v)));
-  *candidates = v[0], *redone = v[1];
-}
+unsigned long long readTopkStat(int i) { return readDeviceCounter(g_topkStat, i); }
 
 static void topkSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t nLib, int words, bool cosine, int k, double* values,
                        int32_t* indices, cudaStream_t s) {
@@ -235,7 +224,7 @@ static void topkSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t
   Scratch<int4>     bar(nQ, s);
   B200_CUDA(cudaMemsetAsync(count.get(), 0, nQ * sizeof(uint32_t), s));
   B200_CUDA(cudaMemsetAsync(redo.get(), 0, nQ * sizeof(uint32_t), s));
-  resetStats(s);
+  resetDeviceCounters(g_topkStat, s);
   g_topkSlabsLast = 0;
 
   TopkArgs a{};

@@ -14,6 +14,8 @@ Tight comparisons use p = 2, or p = 4 up to three iterations: further on, a diff
 can flip a near-tie in the line search's acceptance test and send the two minimisers down different, equally valid paths.
 """
 
+import contextlib
+
 import numpy as np
 import pytest
 import torch
@@ -33,11 +35,8 @@ def ctas_per_sm(request, cuda):
     """Default CTA count, or one CTA per SM with more systems than CTAs: each slab then serves several systems."""
     from nvmolkit_b200 import _lib
 
-    old = _lib.get_option("bfgs_ctas_per_sm")
-    if request.param:
-        _lib.set_option("bfgs_ctas_per_sm", 1)
-    yield request.param
-    _lib.set_option("bfgs_ctas_per_sm", old)
+    with _lib.options(bfgs_ctas_per_sm=1) if request.param else contextlib.nullcontext():
+        yield request.param
 
 
 def _batch_sizes(sizes, reuse, seed):

@@ -1,6 +1,8 @@
 """MaxMin diversity picking on the GPU: picks equal (==) to the CPU oracles and the threshold bit-equal, in both modes,
 with the pool resident in shared memory and streamed."""
 
+import contextlib
+
 import numpy as np
 import pytest
 import torch
@@ -43,12 +45,10 @@ def _dev(a):
 @pytest.fixture
 def path(cuda):
     """path(mode, resident_rows): force a mode and a fingerprint placement until the test ends."""
-    def force(mode, resident):
-        _lib.set_option("maxmin_mode", mode)
-        _lib.set_option("maxmin_resident_rows", resident)
-    yield force
-    _lib.set_option("maxmin_mode", 0)
-    _lib.set_option("maxmin_resident_rows", -1)
+    with contextlib.ExitStack() as scopes:
+        def force(mode, resident):
+            scopes.enter_context(_lib.options(maxmin_mode=mode, maxmin_resident_rows=resident))
+        yield force
 
 
 def _pick(fp, pool, pick, first=(), threshold=None, metric="tanimoto", **kw):

@@ -1,6 +1,8 @@
 """Leader diversity picking on the GPU: picks equal (==) to the CPU oracle, with the bulk pass on the SIMT tile and on
 the tensor-core tile, and with windows forced small so that windows and resolver blocks cut through the picks."""
 
+import contextlib
+
 import numpy as np
 import pytest
 import torch
@@ -44,12 +46,10 @@ def _dev(a):
 @pytest.fixture
 def path(cuda):
     """path(min_pairs, window_rows): force the bulk pass's tile and the window size until the test ends."""
-    def force(min_pairs, window):
-        _lib.set_option("similarity_tensor_min_pairs", min_pairs)
-        _lib.set_option("leader_window_rows", window)
-    yield force
-    _lib.set_option("similarity_tensor_min_pairs", 1 << 24)
-    _lib.set_option("leader_window_rows", 0)
+    with contextlib.ExitStack() as scopes:
+        def force(min_pairs, window):
+            scopes.enter_context(_lib.options(similarity_tensor_min_pairs=min_pairs, leader_window_rows=window))
+        yield force
 
 
 def _pick(fp, pool, threshold, pick=0, first=(), metric="tanimoto", **kw):

@@ -190,11 +190,8 @@ def pair_tile(cuda, request):
     """The tile a small X-vs-Y count runs on: SIMT, or tensor variant 0, 1 or 3 (unsuperposed: acc = c)."""
     from nvmolkit_b200 import _lib
 
-    _lib.set_option("similarity_tensor_min_pairs", request.param[0])
-    _lib.set_option("similarity_tensor_cluster", request.param[1])
-    yield request.param
-    _lib.set_option("similarity_tensor_cluster", 1)
-    _lib.set_option("similarity_tensor_min_pairs", 1 << 24)
+    with _lib.options(similarity_tensor_min_pairs=request.param[0], similarity_tensor_cluster=request.param[1]):
+        yield request.param
 
 
 @pytest.mark.gpu
@@ -260,15 +257,12 @@ def superposition(cuda, request):
     from nvmolkit_b200 import _lib
 
     if request.param is None:
-        _lib.set_option("similarity_tensor_min_pairs", -1)
+        tile = _lib.options(similarity_tensor_min_pairs=-1)
     else:
-        _lib.set_option("similarity_tensor_min_pairs", 0)
-        _lib.set_option("similarity_superpose", request.param[0])
-        _lib.set_option("similarity_superpose_cols", request.param[1])
-    yield request.param
-    _lib.set_option("similarity_superpose", 4)
-    _lib.set_option("similarity_superpose_cols", 4)
-    _lib.set_option("similarity_tensor_min_pairs", 1 << 24)
+        tile = _lib.options(similarity_tensor_min_pairs=0, similarity_superpose=request.param[0],
+                            similarity_superpose_cols=request.param[1])
+    with tile:
+        yield request.param
 
 
 @pytest.mark.gpu

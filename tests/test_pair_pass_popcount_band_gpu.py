@@ -64,16 +64,9 @@ def variant(cuda, request):
     from nvmolkit_b200 import _lib
 
     cl, s, c = request.param
-    _lib.set_option("similarity_tensor_min_pairs", 0)
-    _lib.set_option("similarity_tensor_cluster", cl)
-    _lib.set_option("similarity_superpose", s)
-    _lib.set_option("similarity_superpose_cols", c)
-    yield request.param
-    _lib.set_option("similarity_tensor_cluster", 1)
-    _lib.set_option("similarity_superpose", 4)
-    _lib.set_option("similarity_superpose_cols", 4)
-    _lib.set_option("similarity_tensor_min_pairs", 1 << 24)
-    _lib.set_option("similarity_popcount_band", 1)
+    with _lib.options(similarity_tensor_min_pairs=0, similarity_tensor_cluster=cl, similarity_superpose=s,
+                      similarity_superpose_cols=c):
+        yield request.param
 
 
 def _boundary_set(bits, cutoff, delta, seed):
@@ -117,8 +110,8 @@ def _units_model(fp, cutoff, cl, s, c, band):
 def _pass(fp, cutoff, cuda, band):
     from nvmolkit_b200 import _lib
 
-    _lib.set_option("similarity_popcount_band", band)
-    deg, edges = P._neighbor_edges(fp, cutoff, cuda)
+    with _lib.options(similarity_popcount_band=band):
+        deg, edges = P._neighbor_edges(fp, cutoff, cuda)
     return deg, edges, _lib.get_option("similarity_units_last"), _lib.get_option("similarity_units_planned_last")
 
 
@@ -202,19 +195,14 @@ def test_wide_popcount_spread_clusters_equal_the_pass_without_band(cuda):
     pop = P._popcounts(fp)
     assert pop.min() < 40 and pop.max() > 150
     dev = A._dev(fp, cuda)
-    _lib.set_option("similarity_tensor_min_pairs", 0)
-    try:
-        out = {}
-        for band in (1, 0):
-            _lib.set_option("similarity_popcount_band", band)
+    out = {}
+    for band in (1, 0):
+        with _lib.options(similarity_tensor_min_pairs=0, similarity_popcount_band=band):
             deg, edges = P._neighbor_edges(fp, 0.3, cuda)
             units = _lib.get_option("similarity_units_last")
             assert units == _lib.get_option("similarity_units_planned_last")
             ids, cen = fused_butina_device(dev, 0.3)
-            out[band] = (deg, np.sort(edges[:, 0] * len(fp) + edges[:, 1]), ids.cpu().numpy(), cen.cpu().numpy(), units)
-    finally:
-        _lib.set_option("similarity_popcount_band", 1)
-        _lib.set_option("similarity_tensor_min_pairs", 1 << 24)
+        out[band] = (deg, np.sort(edges[:, 0] * len(fp) + edges[:, 1]), ids.cpu().numpy(), cen.cpu().numpy(), units)
     (deg, key, ids, cen, units), (deg0, key0, ids0, cen0, units0) = out[1], out[0]
     assert units < 0.7 * units0, (units, units0)  # the band skips over 30 % of the triangle's units
     assert (deg == deg0).all() and len(key) == len(key0) and (key == key0).all()
@@ -230,12 +218,9 @@ def test_wide_popcount_spread_sharded_pass_equals_one_pass(cuda, world):
     from nvmolkit_b200 import _lib
 
     fp = _wide(40_000, seed=world)
-    _lib.set_option("similarity_tensor_min_pairs", 0)
-    try:
+    with _lib.options(similarity_tensor_min_pairs=0):
         ids, cen, edges, deg, per_rank = A._sharded_butina_one_gpu(fp, 0.3, world, cuda)
         ids1, cen1, edges1, deg1, _ = A._sharded_butina_one_gpu(fp, 0.3, 1, cuda)
-    finally:
-        _lib.set_option("similarity_tensor_min_pairs", 1 << 24)
     assert (deg == deg1).all() and (ids == ids1).all() and (cen == cen1).all()
     key = np.sort(edges[:, 0].astype(np.int64) * len(fp) + edges[:, 1])
     key1 = np.sort(edges1[:, 0].astype(np.int64) * len(fp) + edges1[:, 1])
@@ -250,15 +235,8 @@ def test_superposed_pass_lists_the_candidates_the_banded_model_predicts(cuda):
 
     fp = S.clustered_fingerprints(400, 50, seed=S.SEED)[:16384]
     fp = np.ascontiguousarray(fp[P._stable_order(fp)])
-    _lib.set_option("similarity_tensor_min_pairs", 0)
-    _lib.set_option("similarity_superpose_auto", 0)
-    try:
-        for c in (4, 2, 1):
-            _lib.set_option("similarity_superpose_cols", c)
+    for c in (4, 2, 1):
+        with _lib.options(similarity_tensor_min_pairs=0, similarity_superpose_auto=0, similarity_superpose_cols=c):
             P._neighbor_edges(fp, 0.3, cuda)
             assert _lib.get_option("similarity_superpose_last") == 4 * c
             assert _lib.get_option("similarity_candidates_last") == M.candidates(fp, 0.3, 4, c, band=True), c
-    finally:
-        _lib.set_option("similarity_superpose_cols", 4)
-        _lib.set_option("similarity_superpose_auto", 1)
-        _lib.set_option("similarity_tensor_min_pairs", 1 << 24)

@@ -38,13 +38,9 @@ def superposition(cuda, request):
     """The tensor-core neighbour pass at rows x columns superposition, no pilot."""
     from nvmolkit_b200 import _lib
 
-    _lib.set_option("similarity_tensor_min_pairs", 0)
-    _lib.set_option("similarity_superpose", request.param[0])
-    _lib.set_option("similarity_superpose_cols", request.param[1])
-    yield request.param
-    _lib.set_option("similarity_superpose", 4)
-    _lib.set_option("similarity_superpose_cols", 4)
-    _lib.set_option("similarity_tensor_min_pairs", 1 << 24)
+    with _lib.options(similarity_tensor_min_pairs=0, similarity_superpose=request.param[0],
+                      similarity_superpose_cols=request.param[1]):
+        yield request.param
 
 
 def _neighbor_edges(fp, cutoff, cuda, group_offset=0, group_stride=1):
@@ -169,17 +165,11 @@ def test_sharded_pass_in_popcount_order_equals_the_plain_pass(cuda, world):
     from nvmolkit_b200 import _lib
 
     fp = _descending(40_000, 2048, seed=world)
-    _lib.set_option("similarity_tensor_min_pairs", 0)
-    try:
+    with _lib.options(similarity_tensor_min_pairs=0):
         ids, cen, edges, deg, per_rank = A._sharded_butina_one_gpu(fp, 0.3, world, cuda)
         assert all(c > 0 for c in per_rank)
-        _lib.set_option("similarity_superpose", 1)
-        _lib.set_option("similarity_superpose_cols", 1)
-        ids1, cen1, edges1, deg1, _ = A._sharded_butina_one_gpu(fp, 0.3, 1, cuda)
-    finally:
-        _lib.set_option("similarity_superpose", 4)
-        _lib.set_option("similarity_superpose_cols", 4)
-        _lib.set_option("similarity_tensor_min_pairs", 1 << 24)
+        with _lib.options(similarity_superpose=1, similarity_superpose_cols=1):
+            ids1, cen1, edges1, deg1, _ = A._sharded_butina_one_gpu(fp, 0.3, 1, cuda)
     assert (deg == deg1).all() and (ids == ids1).all() and (cen == cen1).all()
     key = np.sort(edges[:, 0].astype(np.int64) * len(fp) + edges[:, 1])
     key1 = np.sort(edges1[:, 0].astype(np.int64) * len(fp) + edges1[:, 1])
@@ -217,16 +207,9 @@ def _plain_graph(fp, cuda):
     from nvmolkit_b200 import _lib
     from nvmolkit_b200.clustering import fused_butina_device
 
-    _lib.set_option("similarity_superpose", 1)
-    _lib.set_option("similarity_superpose_cols", 1)
-    _lib.set_option("similarity_pipeline_chunks", 1)
-    try:
+    with _lib.options(similarity_superpose=1, similarity_superpose_cols=1, similarity_pipeline_chunks=1):
         deg, edges = _neighbor_edges(fp, 0.3, cuda)
         ids, cen = fused_butina_device(A._dev(fp, cuda), 0.3)
-    finally:
-        _lib.set_option("similarity_superpose", 4)
-        _lib.set_option("similarity_superpose_cols", 4)
-        _lib.set_option("similarity_pipeline_chunks", 4)
     return deg, np.sort(edges[:, 0] * len(fp) + edges[:, 1]), ids.cpu().numpy(), cen.cpu().numpy()
 
 
@@ -239,16 +222,11 @@ def test_pipeline_chunk_that_overflows_twice_reruns_unsuperposed_in_popcount_ord
     from nvmolkit_b200.clustering import fused_butina_device
 
     fp = _with_band(120_000, 20_000, seed=140)
-    _lib.set_option("similarity_tensor_min_pairs", 0)
-    _lib.set_option("similarity_superpose_auto", 0)
-    try:
+    with _lib.options(similarity_tensor_min_pairs=0, similarity_superpose_auto=0):
         deg, edges = _neighbor_edges(fp, 0.3, cuda)
         ids, cen = fused_butina_device(A._dev(fp, cuda), 0.3)
         assert _lib.get_option("similarity_superpose_last") == 16
         deg1, key1, ids1, cen1 = _plain_graph(fp, cuda)
-    finally:
-        _lib.set_option("similarity_superpose_auto", 1)
-        _lib.set_option("similarity_tensor_min_pairs", 1 << 24)
     assert len(key1) > 0
     _assert_graph(deg, edges, deg1, key1, len(fp), "pipelined fallback")
     assert (ids.cpu().numpy() == ids1).all() and (cen.cpu().numpy() == cen1).all()
@@ -263,8 +241,7 @@ def test_sharded_pass_where_one_rank_falls_back_to_the_plain_pass(cuda):
     fp = _with_band(24_576, 16_384, seed=2)
     n = len(fp)
     sptr = torch.cuda.current_stream().cuda_stream
-    _lib.set_option("similarity_tensor_min_pairs", 0)
-    try:
+    with _lib.options(similarity_tensor_min_pairs=0):
         total = np.zeros(n, dtype=np.int64)
         parts, ran = [], []
         for r in range(2):
@@ -283,8 +260,6 @@ def test_sharded_pass_where_one_rank_falls_back_to_the_plain_pass(cuda):
         _lib.call("b200mol_butina_from_edges", n, counts.data_ptr(), de.data_ptr(), de.shape[0], ids.data_ptr(), cen.data_ptr(),
                   ncl.data_ptr(), None, sptr)
         k = int(ncl.item())
-    finally:
-        _lib.set_option("similarity_tensor_min_pairs", 1 << 24)
     assert len(key1) > 0
     _assert_graph(total.astype(np.int32), all_edges, deg1, key1, n, "sharded fallback")
     assert (ids.cpu().numpy() == ids1).all() and (cen[:k].cpu().numpy() == cen1).all()
@@ -302,12 +277,7 @@ def test_pilot_on_the_bench_generator_picks_what_the_model_predicts(cuda):
     dev = A._dev(fp, cuda)
     ids, cen = fused_butina_device(dev, 0.3)
     chosen = _lib.get_option("similarity_superpose_last")
-    try:
-        _lib.set_option("similarity_superpose", 1)
-        _lib.set_option("similarity_superpose_cols", 1)
+    with _lib.options(similarity_superpose=1, similarity_superpose_cols=1):
         ids1, cen1 = fused_butina_device(dev, 0.3)
-    finally:
-        _lib.set_option("similarity_superpose", 4)
-        _lib.set_option("similarity_superpose_cols", 4)
     assert chosen == model["chosen"][0] * model["chosen"][1], (chosen, model)
     assert torch.equal(ids, ids1) and torch.equal(cen, cen1)

@@ -315,11 +315,8 @@ def test_butina_parallel_rounds_keep_the_greedy_order(cuda, min_commits, n, degr
     d = np.minimum(d, d.T)
     np.fill_diagonal(d, 0.0)
     cutoff = 1.0 - (1.0 - degree / n) ** 0.5  # P(min(u, v) <= c) = degree / n
-    _lib.set_option("butina_min_round_commits", min_commits)
-    try:
+    with _lib.options(butina_min_round_commits=min_commits):
         ids, cen = butina(torch.from_numpy(d).to(cuda), cutoff, return_centroids=True)
-    finally:
-        _lib.set_option("butina_min_round_commits", 32)
     ids_cpu, cen_cpu = oracle.butina_dense(d, cutoff)
     assert (ids.numpy() == ids_cpu).all() and (cen.numpy() == cen_cpu).all()
 
@@ -337,15 +334,9 @@ def force_tensor_path(cuda, request):
     row x column superposition of the Butina neighbour pass (4 x 4 = default ... 1 x 1 = off)."""
     from nvmolkit_b200 import _lib
 
-    _lib.set_option("similarity_tensor_min_pairs", 0)
-    _lib.set_option("similarity_tensor_cluster", request.param[0])
-    _lib.set_option("similarity_superpose", request.param[1])
-    _lib.set_option("similarity_superpose_cols", request.param[2])
-    yield request.param
-    _lib.set_option("similarity_tensor_cluster", 1)
-    _lib.set_option("similarity_superpose", 4)
-    _lib.set_option("similarity_superpose_cols", 4)
-    _lib.set_option("similarity_tensor_min_pairs", 1 << 24)
+    with _lib.options(similarity_tensor_min_pairs=0, similarity_tensor_cluster=request.param[0],
+                      similarity_superpose=request.param[1], similarity_superpose_cols=request.param[2]):
+        yield request.param
 
 
 @pytest.mark.parametrize("bits", [128, 512, 2048] + TENSOR_WIDTHS)
@@ -434,21 +425,13 @@ def test_row_stationary_tile_reloads_its_row_operand(cuda, superpose):
     fp = S.clustered_fingerprints(180, 50, bits=1024, seed=98)
     counts = torch.zeros(len(fp), dtype=torch.int32, device=cuda)
     dfp = _dev(fp, cuda)
-    _lib.set_option("similarity_tensor_min_pairs", 0)
-    _lib.set_option("similarity_tensor_cluster", 3)
-    _lib.set_option("similarity_superpose", superpose)
-    _lib.set_option("similarity_superpose_cols", superpose)
-    try:
+    with _lib.options(similarity_tensor_min_pairs=0, similarity_tensor_cluster=3, similarity_superpose=superpose,
+                      similarity_superpose_cols=superpose):
         _lib.call("b200mol_tanimoto_count_ge", dfp.data_ptr(), len(fp), dfp.data_ptr(), len(fp), 32, 0, 0.3, 1,
                   counts.data_ptr(), torch.cuda.current_stream().cuda_stream)
         from nvmolkit_b200.clustering import fused_butina_device
 
         ids, cen = fused_butina_device(dfp, 0.3)
-    finally:
-        _lib.set_option("similarity_tensor_cluster", 1)
-        _lib.set_option("similarity_superpose", 4)
-        _lib.set_option("similarity_superpose_cols", 4)
-        _lib.set_option("similarity_tensor_min_pairs", 1 << 24)
     assert (counts.cpu().numpy() == oracle.count_ge(fp, fp, 0.3)).all()
     ids_cpu, cen_cpu = oracle.butina_fp(fp, 0.3)
     assert (ids.cpu().numpy() == ids_cpu).all() and (cen.cpu().numpy() == cen_cpu).all()
@@ -461,25 +444,17 @@ def test_pilot_chosen_superposition_gives_the_unsuperposed_answer(cuda):
     from nvmolkit_b200 import _lib
     from nvmolkit_b200.clustering import fused_butina_device
 
-    _lib.set_option("similarity_tensor_min_pairs", 0)
-    try:
+    with _lib.options(similarity_tensor_min_pairs=0, similarity_superpose=4, similarity_superpose_cols=4):
         chosen = []
         for dens in (0.08, 0.012):
             fp = S.random_fingerprints(70_000, p=dens, seed=5, near_dups=30_000)
             dev = _dev(fp, cuda)
             ids, cen = fused_butina_device(dev, 0.35)
             chosen.append(_lib.get_option("similarity_superpose_last"))
-            _lib.set_option("similarity_superpose", 1)
-            _lib.set_option("similarity_superpose_cols", 1)
-            ids1, cen1 = fused_butina_device(dev, 0.35)
-            _lib.set_option("similarity_superpose", 4)
-            _lib.set_option("similarity_superpose_cols", 4)
+            with _lib.options(similarity_superpose=1, similarity_superpose_cols=1):
+                ids1, cen1 = fused_butina_device(dev, 0.35)
             assert torch.equal(ids, ids1) and torch.equal(cen, cen1)
         assert chosen == [4, 16], chosen  # sparse rows carry 4 x 4 sums, dense ones only rows
-    finally:
-        _lib.set_option("similarity_superpose", 4)
-        _lib.set_option("similarity_superpose_cols", 4)
-        _lib.set_option("similarity_tensor_min_pairs", 1 << 24)
 
 
 def test_pipelined_verification_gives_the_same_graph(cuda):
@@ -490,22 +465,15 @@ def test_pipelined_verification_gives_the_same_graph(cuda):
     from nvmolkit_b200 import _lib
     from nvmolkit_b200.clustering import fused_butina_device
 
-    _lib.set_option("similarity_tensor_min_pairs", 0)
-    try:
-        for centres, members, auto in ((2700, 50, 1), (338, 400, 0)):
-            dev = _dev(S.clustered_fingerprints(centres, members, seed=centres), cuda)
-            _lib.set_option("similarity_superpose_auto", auto)
-            _lib.set_option("similarity_pipeline_chunks", 4)
+    for centres, members, auto in ((2700, 50, 1), (338, 400, 0)):
+        dev = _dev(S.clustered_fingerprints(centres, members, seed=centres), cuda)
+        with _lib.options(similarity_tensor_min_pairs=0, similarity_superpose_auto=auto, similarity_pipeline_chunks=4):
             ids, cen = fused_butina_device(dev, 0.3)
             listed = _lib.get_option("similarity_candidates_last")
-            _lib.set_option("similarity_pipeline_chunks", 1)
-            ids1, cen1 = fused_butina_device(dev, 0.3)
-            assert torch.equal(ids, ids1) and torch.equal(cen, cen1), (centres, members)
-            assert listed > 0
-    finally:
-        _lib.set_option("similarity_superpose_auto", 1)
-        _lib.set_option("similarity_pipeline_chunks", 4)
-        _lib.set_option("similarity_tensor_min_pairs", 1 << 24)
+            with _lib.options(similarity_pipeline_chunks=1):
+                ids1, cen1 = fused_butina_device(dev, 0.3)
+        assert torch.equal(ids, ids1) and torch.equal(cen, cen1), (centres, members)
+        assert listed > 0
 
 
 def test_superposed_pass_falls_back_when_its_candidate_list_overflows(cuda):
@@ -516,12 +484,9 @@ def test_superposed_pass_falls_back_when_its_candidate_list_overflows(cuda):
     from nvmolkit_b200.clustering import fused_butina_device
 
     one = np.repeat(S.random_fingerprints(1, seed=3), 12000, axis=0)
-    _lib.set_option("similarity_tensor_min_pairs", 0)
-    try:
+    with _lib.options(similarity_tensor_min_pairs=0):
         ids, cen = fused_butina_device(_dev(one, cuda), 0.3)
         assert _lib.get_option("similarity_superpose_last") == 1
-    finally:
-        _lib.set_option("similarity_tensor_min_pairs", 1 << 24)
     assert (ids.cpu().numpy() == 0).all() and cen.cpu().numpy().tolist() == [11999]
 
 
@@ -594,19 +559,11 @@ def test_sharded_pipelined_pass_equals_the_plain_pass(cuda):
     from nvmolkit_b200 import _lib
 
     fp = S.clustered_fingerprints(5400, 50, seed=11)
-    _lib.set_option("similarity_tensor_min_pairs", 0)
-    try:
+    with _lib.options(similarity_tensor_min_pairs=0):
         ids, cen, edges, deg, per_rank = _sharded_butina_one_gpu(fp, 0.3, 2, cuda)
         assert all(c > 0 for c in per_rank)
-        _lib.set_option("similarity_pipeline_chunks", 1)
-        _lib.set_option("similarity_superpose", 1)
-        _lib.set_option("similarity_superpose_cols", 1)
-        ids1, cen1, edges1, deg1, _ = _sharded_butina_one_gpu(fp, 0.3, 1, cuda)
-    finally:
-        _lib.set_option("similarity_pipeline_chunks", 4)
-        _lib.set_option("similarity_superpose", 4)
-        _lib.set_option("similarity_superpose_cols", 4)
-        _lib.set_option("similarity_tensor_min_pairs", 1 << 24)
+        with _lib.options(similarity_pipeline_chunks=1, similarity_superpose=1, similarity_superpose_cols=1):
+            ids1, cen1, edges1, deg1, _ = _sharded_butina_one_gpu(fp, 0.3, 1, cuda)
     assert (deg == deg1).all() and (ids == ids1).all() and (cen == cen1).all()
     key = np.sort(edges[:, 0].astype(np.int64) * len(fp) + edges[:, 1])
     key1 = np.sort(edges1[:, 0].astype(np.int64) * len(fp) + edges1[:, 1])
@@ -622,13 +579,8 @@ def test_sharded_neighbor_pass_equals_oracle(cuda, world, centres, members, tens
     from nvmolkit_b200 import _lib
 
     fp = S.clustered_fingerprints(centres, members, seed=centres + world)
-    _lib.set_option("similarity_tensor_min_pairs", 0 if tensor else -1)
-    _lib.set_option("similarity_tensor_cluster", tensor if tensor else 1)
-    try:
+    with _lib.options(similarity_tensor_min_pairs=0 if tensor else -1, similarity_tensor_cluster=tensor if tensor else 1):
         ids, cen, edges, deg, per_rank = _sharded_butina_one_gpu(fp, 0.3, world, cuda)
-    finally:
-        _lib.set_option("similarity_tensor_min_pairs", 1 << 24)
-        _lib.set_option("similarity_tensor_cluster", 1)
     ids_cpu, cen_cpu = oracle.butina_fp(fp, 0.3)
     want_deg = oracle.count_ge(fp, fp, 0.3) - 1  # neighbours other than the point itself
     assert (deg == want_deg).all()

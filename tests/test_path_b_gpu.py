@@ -306,9 +306,8 @@ def embedder_hessian(request):
     """The embedder's BFGS inverse Hessian in fp32 (default) and in fp64 (option etkdg_hessian_fp64, the reference's type)."""
     from nvmolkit_b200 import _lib
 
-    _lib.set_option("etkdg_hessian_fp64", request.param)
-    yield request.param
-    _lib.set_option("etkdg_hessian_fp64", 0)
+    with _lib.options(etkdg_hessian_fp64=request.param):
+        yield request.param
 
 
 def test_etkdg_embed_produces_conformers_the_cpu_accepts(cuda, embedder_hessian):

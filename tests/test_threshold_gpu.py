@@ -1,5 +1,6 @@
 """Threshold similarity search on the GPU: indptr, indices and values equal (==) to the CPU oracle on every path."""
 
+import contextlib
 import ctypes as C
 
 import numpy as np
@@ -15,8 +16,6 @@ pytestmark = pytest.mark.gpu
 
 SEARCH = {"tanimoto": thresholdTanimotoSimilarity, "cosine": thresholdCosineSimilarity}
 SIMT, TENSOR = "simt", "tensor"
-OPTIONS = {"similarity_tensor_min_pairs": 1 << 24, "similarity_superpose": 4, "similarity_superpose_cols": 4,
-           "similarity_popcount_band": 1, "similarity_tensor_cluster": 1}
 
 
 def _fingerprints(seed, n, words, density=0.08):
@@ -32,14 +31,12 @@ def _dev(a):
 @pytest.fixture
 def opts(cuda):
     """opts(key=value, ...): set library options until the test ends; opts(SIMT) / opts(TENSOR) forces a tile."""
-    def force(which=None, **kw):
-        if which is not None:
-            _lib.set_option("similarity_tensor_min_pairs", -1 if which == SIMT else 0)
-        for k, v in kw.items():
-            _lib.set_option(k, v)
-    yield force
-    for k, v in OPTIONS.items():
-        _lib.set_option(k, v)
+    with contextlib.ExitStack() as scopes:
+        def force(which=None, **kw):
+            if which is not None:
+                scopes.enter_context(_lib.options(similarity_tensor_min_pairs=-1 if which == SIMT else 0))
+            scopes.enter_context(_lib.options(**kw))
+        yield force
 
 
 def _search(metric, q, lib, t, **kw):

@@ -1,5 +1,7 @@
 """Top-k similarity search on the GPU: values and indices equal (==) to the CPU oracle on both kernel paths."""
 
+import contextlib
+
 import numpy as np
 import pytest
 import torch
@@ -28,12 +30,10 @@ def _dev(a):
 @pytest.fixture
 def path(cuda):
     """path(SIMT) / path(TENSOR, slab): force one kernel path (and the tensor path's slab size) until the test ends."""
-    def force(which, slab=256):
-        _lib.set_option("similarity_tensor_min_pairs", -1 if which == SIMT else 0)
-        _lib.set_option("topk_slab_cols", slab)
-    yield force
-    _lib.set_option("similarity_tensor_min_pairs", 1 << 24)
-    _lib.set_option("topk_slab_cols", 0)
+    with contextlib.ExitStack() as scopes:
+        def force(which, slab=256):
+            scopes.enter_context(_lib.options(similarity_tensor_min_pairs=-1 if which == SIMT else 0, topk_slab_cols=slab))
+        yield force
 
 
 def _search(metric, q, lib, k, **kw):

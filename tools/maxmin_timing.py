@@ -82,12 +82,12 @@ def main() -> None:
             row["torch_loop_ms"] = ms_loop
             row["torch_loop_us_per_pick"] = 1e3 * ms_loop / (pick - 1)
             for mode, label in ((0, "dense"), (1, "deferred")):
-                _lib.set_option("maxmin_mode", mode)
-                times = []
-                for it in range(1 + REPEATS):
-                    ms, p = timed(lambda: picker.LazyBitVectorPick(d, pool, pick, [0]).torch())
-                    if it:
-                        times.append(ms)
+                with _lib.options(maxmin_mode=mode):
+                    times = []
+                    for it in range(1 + REPEATS):
+                        ms, p = timed(lambda: picker.LazyBitVectorPick(d, pool, pick, [0]).torch())
+                        if it:
+                            times.append(ms)
                 assert torch.equal(p.cpu(), want), f"{label} picks differ from the torch loop ({pool}, {pick})"
                 ev, sk = _lib.get_option("maxmin_distances_last"), _lib.get_option("maxmin_popcount_skips_last")
                 row[f"{label}_ms"] = statistics.median(times)
@@ -96,7 +96,6 @@ def main() -> None:
                 row[f"{label}_distances"] = ev
                 row[f"{label}_popcount_skip_rate"] = sk / max(1, ev + sk)
                 row[f"{label}_resident"] = _lib.get_option("maxmin_resident_last")
-            _lib.set_option("maxmin_mode", 0)
             visited = row["dense_distances"] / max(1e-9, 1.0 - row["dense_popcount_skip_rate"])  # pairs dense visits
             row["dense_pairs_visited"] = visited
             row["deferred_fraction_evaluated"] = row["deferred_distances"] / visited
