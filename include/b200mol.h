@@ -76,6 +76,9 @@ int b200mol_free_async(void* d_ptr, void* stream);
  *                                  this many rows (that fit). Results identical
  *   "leader_window_rows"           0 (default): b200mol_leader_pick sizes each window of the pool so that about 8,192 items
  *                                  survive its bulk pass; > 0: every window takes this many items. Results identical
+ *   "rmsd_match_chunk"             0 (default): b200mol_conformer_rmsd_mapped keeps the column operands of as many mappings
+ *                                  per molecule resident at once as fit 1 GiB; > 0: at most this many (fewer passes
+ *                                  over the pairs against less scratch). Results identical
  *   "butina_min_round_commits"     a parallel Butina round that commits fewer clusters than this hands over to the
  *                                  one-cluster-per-step loop (default 32; 0 = rounds only, >= 1e9 = stepwise only)
  *   "etkdg_hessian_fp64"           0 (default): the embedder keeps its BFGS inverse Hessian in fp32 and sweeps it in fp32
@@ -98,7 +101,8 @@ int b200mol_set_option(const char* key, long long value);
  * synchronise the device. Of the last b200mol_leader_pick: "leader_windows_last" (windows of the pool it walked),
  * "leader_bulk_pairs_last" (window x pick pairs sent through the count pass), "leader_window_pairs_last" and
  * "leader_block_pairs_last" (pairs the resolver compared against earlier picks of the same window / of the same block;
- * these two synchronise the device). */
+ * these two synchronise the device). Of the last b200mol_conformer_rmsd_mapped: "rmsd_match_chunks_last" (chunks of
+ * mappings it ran). */
 int b200mol_get_option(const char* key, long long* value);
 /* Per-phase CUDA-event timing inside the library (off by default). Phases: "neighbor_pass" (the N^2 tile kernel
  * alone), "csr_build", "cluster_loop", "bfgs". b200mol_profile_read waits for the phase's stop event. */
@@ -531,6 +535,22 @@ int b200mol_tfd_matrices(int32_t nMols, const int32_t* h_mol_conf_start, const i
 int b200mol_conformer_rmsd(int32_t nMols, const int32_t* h_mol_conf_start, const int32_t* h_mol_atoms,
                            const int32_t* d_conf_order, const int32_t* d_conf_atom_start, const double* d_xyz,
                            int32_t prealigned, double* d_out, void* stream);
+/* Symmetry-aware conformer RMSD matrices (RDKit rdMolAlign.GetAllConformerBestRMS; with one mapping, an atom selection as
+ * AllChem.GetConformerRMSMatrix(atomIds=...)). The conformer tables, output and stream are as b200mol_conformer_rmsd.
+ * Molecule m (fewer than 32768 atoms) has a mapping table of K_m = h_map_count[m] >= 1 mappings of
+ * L_m = h_map_len[m] in [1, h_mol_atoms[m]] atoms (L_m = 0 for a molecule without atoms, which has no pairs):
+ * h_map_atoms[h_map_start[m] .. h_map_start[m+1]) (int64 offsets) holds the probe list P (L_m molecule-local indices),
+ * then the reference lists Q_1 .. Q_K (L_m each); no index twice within a list. For conformers I > J:
+ *   min over k of RMSD(x_I[P], x_J[Q_k])
+ * with RMSD as b200mol_conformer_rmsd over the L_m selected atoms: after the best proper rigid superposition, each side
+ * centred on its own selected atoms, or, prealigned != 0, on the coordinates as given (RDKit CalcRMS). K = 1 with
+ * P = Q_1 = 0 .. n-1 gives b200mol_conformer_rmsd's output bit for bit. The tables are HOST arrays, checked before any
+ * device work; the call uploads them with its plan. The mappings of a molecule run in chunks of at most
+ * "rmsd_match_chunk"; a minimum is exact, so results stay bitwise repeatable and batch-independent. */
+int b200mol_conformer_rmsd_mapped(int32_t nMols, const int32_t* h_mol_conf_start, const int32_t* h_mol_atoms,
+                                  const int32_t* d_conf_order, const int32_t* d_conf_atom_start, const double* d_xyz,
+                                  const int64_t* h_map_start, const int32_t* h_map_count, const int32_t* h_map_len,
+                                  const int16_t* h_map_atoms, int32_t prealigned, double* d_out, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Distance-geometry preparation (per-molecule, matrix resident in shared memory).

@@ -26,6 +26,9 @@ extern int                g_maxminResidentLast;
 extern long long          g_leaderWindowRows;
 extern long long          g_leaderWindowsLast;
 extern unsigned long long g_leaderBulkPairsLast;
+// conformer RMSD matrices (conformer_rmsd.cu)
+extern long long g_rmsdMatchChunk;
+extern long long g_rmsdMatchChunksLast;
 // Butina clustering (butina.cu)
 extern int g_butinaMinCommits;
 // minimiser and embedder (bfgs.cu, etkdg.cu)

@@ -502,3 +502,55 @@ def embed_molecules_from_rdkit(molecules, params):
         ends, quads, signs = find_double_bonds(Chem, m)
         stereo.append(StereoInfo(chiral, cbounds, tet, fused, ends, quads, signs))
     return flat_embed_from_parts(smoothed, details, stereo, bool(getattr(params, "useBasicKnowledge", True)))
+
+
+def _terminal_groups(mol) -> List[List[int]]:
+    """Groups of conjugated terminal atoms that ``symmetrizeConjugatedTerminalGroups`` makes equivalent: per atom, its
+    neighbours of degree 1 that are N or O, joined to it by a conjugated bond, and of one element, when there are at
+    least two (the two oxygens of a carboxylate or of a nitro group)."""
+    groups = []
+    for atom in mol.GetAtoms():
+        by_element: Dict[int, List[int]] = {}
+        for bond in atom.GetBonds():
+            t = bond.GetOtherAtomIdx(atom.GetIdx())
+            other = mol.GetAtomWithIdx(t)
+            if other.GetDegree() == 1 and other.GetAtomicNum() in (7, 8) and bond.GetIsConjugated():
+                by_element.setdefault(other.GetAtomicNum(), []).append(t)
+        groups += [sorted(g) for g in by_element.values() if len(g) >= 2]
+    return groups
+
+
+def self_matches(mol, maxMatches: int = 1000000, symmetrizeConjugatedTerminalGroups: bool = True) -> List[Tuple[int, ...]]:
+    """The matches of a molecule onto itself that RDKit's ``GetBestRMS`` / ``GetAllConformerBestRMS`` enumerate:
+    ``mol.GetSubstructMatches(mol, uniquify=False, maxMatches=maxMatches, useChirality=False)``; ``match[q]`` is the atom
+    that query atom q lands on.
+
+    With ``symmetrizeConjugatedTerminalGroups`` this restates RDKit's symmetrised query on the matches instead of on a
+    query copy: every match m is followed by m composed with every permutation that reorders the atoms within each
+    group of :func:`_terminal_groups` (``m'[q] = m[s[q]]``), in lexicographic order of the permutations, duplicates
+    dropped, and the list cut at ``maxMatches``. The restatement is what the tests pin, not RDKit itself."""
+    import itertools
+
+    matches = [tuple(int(a) for a in m) for m in
+               mol.GetSubstructMatches(mol, uniquify=False, maxMatches=maxMatches, useChirality=False)]
+    groups = _terminal_groups(mol) if symmetrizeConjugatedTerminalGroups else []
+    if not groups:
+        return matches[:maxMatches]
+    n = mol.GetNumAtoms()
+    perms = []
+    for choice in itertools.product(*[list(itertools.permutations(g)) for g in groups]):
+        s = list(range(n))
+        for g, p in zip(groups, choice):
+            for a, b in zip(g, p):
+                s[a] = b
+        perms.append(s)
+    out, seen = [], set()
+    for m in matches:
+        for s in perms:
+            t = tuple(m[s[q]] for q in range(n))
+            if t not in seen:
+                seen.add(t)
+                out.append(t)
+                if len(out) == maxMatches:
+                    return out
+    return out
