@@ -170,6 +170,10 @@ __device__ bool tetrahedralFails(const b200mol_term_table& T, int mol, const dou
     const int16_t* ix = T.idx + 5 * t;
     const V3       p0 = p3(pos, ix[0]), p1 = p3(pos, ix[1]), p2 = p3(pos, ix[2]), q3 = p3(pos, ix[3]), p4 = p3(pos, ix[4]);
     if (VOLUME) {
+      // A zero-length arm (an arm atom on the centre) stays a zero vector, so its volumes are 0 and the row fails
+      // here. The reference divides by the zero length instead: NaN volumes pass these comparisons, but its
+      // centre-in-volume test then fails the row, because the centre lies in three of the four face planes. The
+      // verdict is the same either way.
       auto unit = [](V3 v) {
         const double l = sqrt(ff::dot(v, v));
         return l > 0.0 ? v * (1.0 / l) : v;

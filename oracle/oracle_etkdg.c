@@ -72,6 +72,9 @@ static void crs(const double* a, const double* b, double* c) {
   c[2] = a[0] * b[1] - a[1] * b[0];
 }
 static double dt(const double* a, const double* b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
+/* A zero vector stays zero (as in csrc/etkdg.cu): a tetrahedral volume through a zero-length arm is 0 and the row
+ * fails the volume test. A division by the zero length would give NaN volumes that pass it, but the centre-in-volume
+ * test would still fail the row (the centre lies in three face planes), so the verdict does not depend on it. */
 static void   unit(double* v) {
   const double l = sqrt(dt(v, v));
   if (l > 0.0) {
