@@ -552,6 +552,29 @@ int b200mol_conformer_rmsd_mapped(int32_t nMols, const int32_t* h_mol_conf_start
                                   const int64_t* h_map_start, const int32_t* h_map_count, const int32_t* h_map_len,
                                   const int16_t* h_map_atoms, int32_t prealigned, double* d_out, void* stream);
 
+/* Weighted rigid alignment of conformers (RDKit rdMolAlign.AlignMol / GetAlignmentTransform / AlignMolConformers, i.e.
+ * Numerics::Alignment::AlignPoints; the reference library has no alignment). Conformer c owns h_conf_atoms[c] atoms from
+ * d_conf_atom_start[c] of d_xyz[.][3] (f64), c < nConfs. Job j aligns probe conformer h_job_probe[j] onto reference
+ * conformer h_job_ref[j] through pair list h_job_list[j]: list l holds the L >= 1 pairs
+ * h_list_pairs[2 i], h_list_pairs[2 i + 1] (probe atom, reference atom; conformer-local) for
+ * i in [h_list_start[l], h_list_start[l+1]) (int64, h_list_start[0] = 0), with weights h_list_weights[i] (finite, >= 0,
+ * summing to W > 0 per list; NULL = all 1). Lists are shared by jobs (AlignMolConformers: one list per molecule).
+ * With weighted centroids p_bar, r_bar and covariance S = sum w (p - p_bar)(r - r_bar)^T (reflect != 0: every probe
+ * point p replaced by -p first), lambda = largest eigenvalue estimate of Horn's quaternion matrix N(S) after at most
+ * maxIters >= 1 cyclic Jacobi sweeps (converged in fp64 at 50), q its eigenvector, R = R(q) (N = 0: R = I):
+ *   d_rmsd[j] = sqrt(max(0, sum w |p - p_bar|^2 + sum w |r - r_bar|^2 - 2 lambda) / L)   (divided by L, not by W)
+ *   d_transform[16 j ..] (optional, NULL = not written) = [[+-R, t], [0 0 0 1]] row-major, acting on column vectors,
+ *     t = r_bar - R p_bar (reflected p_bar), the sign - when reflect: RDKit's Transform3D layout.
+ * move != 0: every atom of the probe conformer (not just the listed ones) is replaced by its image under the transform,
+ * in place in d_xyz; then no conformer may be the probe of two jobs or both a probe and a reference. Sums run on
+ * coordinates shifted by each job's first pair, so molecules far from the origin keep their accuracy. All tables are
+ * HOST arrays, checked before any device work and uploaded in one cudaMemcpyAsync; the kernel runs on `stream`.
+ * Results are bitwise repeatable and independent of the other jobs of the call. */
+int b200mol_align(int32_t nJobs, const int32_t* h_job_probe, const int32_t* h_job_ref, const int32_t* h_job_list,
+                  int32_t nConfs, const int32_t* h_conf_atoms, const int32_t* d_conf_atom_start, double* d_xyz,
+                  int32_t nLists, const int64_t* h_list_start, const int32_t* h_list_pairs, const double* h_list_weights,
+                  int32_t reflect, int32_t maxIters, int32_t move, double* d_rmsd, double* d_transform, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Distance-geometry preparation (per-molecule, matrix resident in shared memory).
  * Matrices are concatenated: matrix m occupies d_x[starts[m] .. starts[m+1]) = n_m * n_m doubles, row-major.

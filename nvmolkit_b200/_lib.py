@@ -77,6 +77,8 @@ SIGNATURES = {
     "b200mol_conformer_rmsd": (C.c_int, [C.c_int32, _vp, _vp, _vp, _vp, _vp, C.c_int32, _vp, _vp]),
     "b200mol_conformer_rmsd_mapped": (C.c_int, [C.c_int32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_int32, _vp,
                                                 _vp]),
+    "b200mol_align": (C.c_int, [C.c_int32, _vp, _vp, _vp, C.c_int32, _vp, _vp, _vp, C.c_int32, _vp, _vp, _vp, C.c_int32,
+                                C.c_int32, C.c_int32, _vp, _vp, _vp]),
     "b200mol_morgan": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, _vp,
                                  _vp]),
 }

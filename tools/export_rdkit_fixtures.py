@@ -17,6 +17,9 @@ and commit the resulting .npz. `tests/test_rdkit_fixtures.py` then replays it (s
     (TorsionFingerprints.CalculateTorsionLists / CalculateTorsionWeights) in the flat layout of b200mol_tfd_matrices,
     the tables nvmolkit_b200.tfd.tfd_torsions builds for the same molecules, ETKDG conformers and
     TorsionFingerprints.GetTFDMatrix on them
+  * alignment (to tests/golden/rdkit_align.npz, replayed by tests/test_mol_align_rdkit.py): rdMolAlign.AlignMolConformers
+    RMS lists and aligned coordinates over all atoms, heavy-atom atomIds, weights and reflect; rdMolAlign.AlignMol RMSDs
+    and moved coordinates and GetAlignmentTransform matrices with atom maps, weights and reflect
 
 The default molecule set is a small drug-like SMILES list embedded below (aspirin, ibuprofen, caffeine, ...); pass
 --smiles benchmarks/data/chembl_10k.smi of the reference checkout for the BASELINE configs' real input.
@@ -154,6 +157,7 @@ def main() -> None:
     np.savez_compressed(args.out, **out)
     print(f"wrote {args.out}: {len(mols)} molecules, {len(hmols)} with conformers, RDKit {rdkit.__version__}")
     export_tfd(hmols, os.path.join(os.path.dirname(os.path.abspath(args.out)), "rdkit_tfd.npz"))
+    export_align(hmols, os.path.join(os.path.dirname(os.path.abspath(args.out)), "rdkit_align.npz"))
 
 
 def export_tfd(hmols, path: str, n_confs: int = 6) -> None:
@@ -194,6 +198,62 @@ def export_tfd(hmols, path: str, n_confs: int = 6) -> None:
         out[f"adapter_{k}"] = getattr(ours, k)
     np.savez_compressed(path, **out)
     print(f"wrote {path}: {len(mols)} molecules")
+
+
+def export_align(hmols, path: str, n_confs: int = 5) -> None:
+    """RDKit's alignment on ETKDG conformers. AlignMolConformers case k: ``amc{k}_before`` / ``_after`` [C, n, 3],
+    ``_rms`` [C - 1], ``_atomids`` (empty: all atoms), ``_weights`` (empty: none), ``_reflect``. AlignMol /
+    GetAlignmentTransform case k: ``am{k}_prb``, ``_ref``, ``_map`` [L, 2], ``_weights``, ``_reflect``, ``_rmsd``,
+    ``_transform`` [4, 4] and ``_moved`` (the probe after AlignMol)."""
+    import rdkit
+    from rdkit import Chem
+    from rdkit.Chem import rdDistGeom, rdMolAlign
+
+    out = {"rdkit_version": np.array(rdkit.__version__)}
+    rng = np.random.default_rng(5)
+    k = j = 0
+    confmols = []
+    for m in hmols:
+        mh = Chem.Mol(m)
+        mh.RemoveAllConformers()
+        p = rdDistGeom.ETKDGv3()
+        p.randomSeed = 11
+        if len(rdDistGeom.EmbedMultipleConfs(mh, n_confs, p)) < 2:
+            continue
+        confmols.append(mh)
+        n = mh.GetNumAtoms()
+        heavy = [a.GetIdx() for a in mh.GetAtoms() if a.GetAtomicNum() > 1]
+        for ids, weighted, reflect in ((None, False, False), (heavy, False, False), (None, True, False),
+                                       (heavy, True, True)):
+            work = Chem.Mol(mh)
+            L = n if ids is None else len(ids)
+            w = rng.uniform(0.5, 2.0, L).tolist() if weighted else []
+            out[f"amc{k}_before"] = np.array([c.GetPositions() for c in work.GetConformers()])
+            rms = []
+            rdMolAlign.AlignMolConformers(work, atomIds=ids or [], weights=w, reflect=reflect, RMSlist=rms)
+            out[f"amc{k}_after"] = np.array([c.GetPositions() for c in work.GetConformers()])
+            out[f"amc{k}_rms"], out[f"amc{k}_atomids"] = np.array(rms), np.array(ids or [], np.int64)
+            out[f"amc{k}_weights"], out[f"amc{k}_reflect"] = np.array(w, np.float64), np.array(reflect)
+            k += 1
+    for a, b in zip(confmols, confmols[1:] + confmols[:1]):  # a probe onto another molecule through a heavy-atom map
+        L = min(a.GetNumHeavyAtoms(), b.GetNumHeavyAtoms(), 8)
+        amap = list(zip(rng.permutation([x.GetIdx() for x in a.GetAtoms() if x.GetAtomicNum() > 1])[:L].tolist(),
+                        rng.permutation([x.GetIdx() for x in b.GetAtoms() if x.GetAtomicNum() > 1])[:L].tolist()))
+        for weighted, reflect in ((False, False), (True, False), (True, True)):
+            w = rng.uniform(0.5, 2.0, L).tolist() if weighted else []
+            prb = Chem.Mol(a)
+            rmsd, T = rdMolAlign.GetAlignmentTransform(prb, b, atomMap=amap, weights=w, reflect=reflect)
+            out[f"am{j}_prb"], out[f"am{j}_ref"] = prb.GetConformer().GetPositions(), b.GetConformer().GetPositions()
+            out[f"am{j}_map"], out[f"am{j}_weights"] = np.array(amap, np.int64), np.array(w, np.float64)
+            out[f"am{j}_reflect"], out[f"am{j}_transform"] = np.array(reflect), np.asarray(T, np.float64)
+            out[f"am{j}_rmsd"] = np.array(rdMolAlign.AlignMol(prb, b, atomMap=amap, weights=w, reflect=reflect))
+            out[f"am{j}_moved"] = prb.GetConformer().GetPositions()
+            if abs(float(out[f"am{j}_rmsd"]) - rmsd) > 1e-12:
+                raise RuntimeError("AlignMol and GetAlignmentTransform disagree")
+            j += 1
+    out["n_amc"], out["n_am"] = np.array(k), np.array(j)
+    np.savez_compressed(path, **out)
+    print(f"wrote {path}: {k} AlignMolConformers and {j} AlignMol cases")
 
 
 if __name__ == "__main__":
