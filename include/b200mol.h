@@ -575,6 +575,30 @@ int b200mol_align(int32_t nJobs, const int32_t* h_job_probe, const int32_t* h_jo
                   int32_t nLists, const int64_t* h_list_start, const int32_t* h_list_pairs, const double* h_list_weights,
                   int32_t reflect, int32_t maxIters, int32_t move, double* d_rmsd, double* d_transform, void* stream);
 
+/* Symmetry-aware alignment of conformers (RDKit rdMolAlign.GetBestRMS / GetBestAlignmentTransform / CalcRMS; the
+ * reference library has no alignment). Conformers as in b200mol_align. Job j compares probe conformer h_job_probe[j]
+ * with reference conformer h_job_ref[j] through mapping set s = h_job_set[j]: K_s = h_set_count[s] >= 1 mappings of
+ * L_s = h_set_len[s] >= 1 atoms, h_set_atoms[h_set_start[s] .. h_set_start[s+1]) (int64 offsets, h_set_start[0] = 0,
+ * (K_s + 1) L_s entries) holding the probe list P, then the reference lists Q_1 .. Q_K (conformer-local indices below
+ * 32768, none twice within a list; the layout of b200mol_conformer_rmsd_mapped). Mapping k pairs P[i] with Q_k[i],
+ * with weight h_set_weights[W_s + i] (W_s = sum of L over the sets before s; finite, >= 0, summing to > 0 per set;
+ * NULL = all 1). Sets are shared by jobs: one per molecule pair, whatever its number of conformers.
+ *   mode 0 (align): per mapping the RMSD of b200mol_align (reflect, maxIters as there); d_rmsd[j] = the smallest,
+ *     d_best[j] (optional) = the first mapping that has it, d_transform[16 j ..] (optional) = its transform, and,
+ *     move != 0, every atom of the probe conformer moved by it (then no conformer may be the probe of two jobs or both a
+ *     probe and a reference).
+ *   mode 1 (in place, RDKit CalcRMS): per mapping sqrt(sum w |p - r|^2 / L) on the coordinates as given, the smallest in
+ *     d_rmsd[j] and its first mapping in d_best[j]; move, reflect and d_transform must be 0.
+ * All tables are HOST arrays, checked before any device work and uploaded in one cudaMemcpyAsync; the kernel runs on
+ * `stream`. Results are bitwise repeatable and independent of the other jobs of the call; K = 1 gives b200mol_align's
+ * bits. */
+int b200mol_best_align(int32_t nJobs, const int32_t* h_job_probe, const int32_t* h_job_ref, const int32_t* h_job_set,
+                       int32_t nConfs, const int32_t* h_conf_atoms, const int32_t* d_conf_atom_start, double* d_xyz,
+                       int32_t nSets, const int64_t* h_set_start, const int32_t* h_set_count, const int32_t* h_set_len,
+                       const int16_t* h_set_atoms, const double* h_set_weights, int32_t mode, int32_t reflect,
+                       int32_t maxIters, int32_t move, double* d_rmsd, int32_t* d_best, double* d_transform,
+                       void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Distance-geometry preparation (per-molecule, matrix resident in shared memory).
  * Matrices are concatenated: matrix m occupies d_x[starts[m] .. starts[m+1]) = n_m * n_m doubles, row-major.

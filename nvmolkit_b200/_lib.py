@@ -79,6 +79,8 @@ SIGNATURES = {
                                                 _vp]),
     "b200mol_align": (C.c_int, [C.c_int32, _vp, _vp, _vp, C.c_int32, _vp, _vp, _vp, C.c_int32, _vp, _vp, _vp, C.c_int32,
                                 C.c_int32, C.c_int32, _vp, _vp, _vp]),
+    "b200mol_best_align": (C.c_int, [C.c_int32, _vp, _vp, _vp, C.c_int32, _vp, _vp, _vp, C.c_int32, _vp, _vp, _vp, _vp,
+                                     _vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _vp, _vp, _vp, _vp]),
     "b200mol_morgan": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, _vp,
                                  _vp]),
 }

@@ -98,24 +98,35 @@ def _atom_ids_lists(atomIds, n: int, what: str):
     return ids, ids[None, :]
 
 
-def _map_lists(mapping, n: int, what: str):
-    """GetBestRMS's ``map`` (mappings of (probeAtom, refAtom) pairs) -> (P, Q), each mapping sorted by probe atom."""
+def _map_lists(mapping, n: int, what: str, n_ref: Optional[int] = None, order: bool = False):
+    """GetBestRMS's ``map`` (mappings of (probeAtom, refAtom) pairs) -> (P, Q), each mapping sorted by probe atom; probe
+    atoms index ``n`` atoms and reference atoms ``n_ref`` (default ``n``). With ``order``, also the sort of the first
+    mapping's pairs, and every mapping must list its probe atoms in that mapping's order (so that one weight per pair
+    means one weight per probe atom)."""
+    n_ref = n if n_ref is None else n_ref
     if mapping is None or len(mapping) == 0:
         raise ValueError(f"{what} must be a non-empty list of mappings")
-    probe, refs = None, []
+    probe, refs, first = None, [], None
     for k, pairs in enumerate(mapping):
         arr = np.asarray(pairs)
         if arr.ndim != 2 or arr.shape[1] != 2 or len(arr) == 0 or not np.issubdtype(arr.dtype, np.integer):
             raise ValueError(f"{what}[{k}] must be a non-empty list of (probeAtom, refAtom) pairs")
-        arr = arr[np.argsort(arr[:, 0], kind="stable")].astype(np.int64)
+        if order:
+            if first is None:
+                first = arr[:, 0].copy()
+            elif not np.array_equal(arr[:, 0], first):
+                raise ValueError(f"{what}[{k}] lists its probe atoms in another order than {what}[0], so its weights "
+                                 "would fall on other atoms")
+        sort = np.argsort(arr[:, 0], kind="stable")
+        arr = arr[sort].astype(np.int64)
         p = _check_list(arr[:, 0], n, f"{what}[{k}] probe atoms")
-        q = _check_list(arr[:, 1], n, f"{what}[{k}] reference atoms")
+        q = _check_list(arr[:, 1], n_ref, f"{what}[{k}] reference atoms")
         if probe is None:
-            probe = p
+            probe, perm = p, sort
         elif not np.array_equal(p, probe):
             raise ValueError(f"{what}[{k}] covers other probe atoms than {what}[0]")
         refs.append(q)
-    return probe, np.stack(refs)
+    return (probe, np.stack(refs), perm) if order else (probe, np.stack(refs))
 
 
 def _self_match_lists(mol, maxMatches: int, symmetrize: bool, m: int):

@@ -153,6 +153,7 @@ PYBIND11_MODULE(_core, m) {
   DEF(b200mol_conformer_rmsd);
   DEF(b200mol_conformer_rmsd_mapped);
   DEF(b200mol_align);
+  DEF(b200mol_best_align);
   DEF(b200mol_allgather_counts);
   DEF(b200mol_allgather_results);
 #undef DEF

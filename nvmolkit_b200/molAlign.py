@@ -1,4 +1,5 @@
-"""Conformer alignment on the GPU (RDKit ``rdMolAlign.AlignMolConformers``, ``AlignMol`` and ``GetAlignmentTransform``).
+"""Conformer alignment on the GPU (RDKit ``rdMolAlign.AlignMolConformers``, ``AlignMol`` and ``GetAlignmentTransform``;
+and, over atom mappings, ``GetBestRMS``, ``GetBestAlignmentTransform`` and ``CalcRMS``).
 
 Every call is one launch of ``b200mol_align`` (``csrc/align.cu``): one alignment job per probe conformer, the weighted
 rigid superposition of its listed atoms onto a reference conformer's (Horn's quaternion method, as RDKit's
@@ -30,6 +31,44 @@ Differences from RDKit:
   ``tests/golden/rdkit_align.npz`` where RDKit exists, and the tests replay it when it is present.
 * Argument errors (a ``None`` molecule, an unknown conformer id, empty, repeated or out-of-range atom indices, a weights
   length mismatch, bad weights, ``maxIters < 1``) raise ValueError, and a bad ``stream`` TypeError, before any device work.
+
+:func:`GetBestRMS`, :func:`GetBestAlignmentTransform` and :func:`CalcRMS` (and their batch forms) compare a probe
+conformer with a reference conformer of another molecule object over K atom mappings, in one launch of
+``b200mol_best_align`` (``csrc/best_align.cu``). Semantics, restated from RDKit's ``MolAlign.cpp``:
+
+* Mappings: ``ref.GetSubstructMatches(prb, uniquify=False, maxMatches=maxMatches, useChirality=False)``; match t pairs
+  probe atom q with reference atom t[q]. With ``symmetrizeConjugatedTerminalGroups`` every match is followed by its
+  compositions with the permutations of the probe's conjugated terminal groups (the order, duplicate removal and
+  ``maxMatches`` cut of :func:`~nvmolkit_b200.rdkit_adapter.probe_ref_matches`). No match raises ValueError("No
+  sub-structure match found between the reference and probe mol"). A user ``map`` (mappings of (probeAtom, refAtom)
+  pairs) replaces the matches, and then ``maxMatches`` and the symmetrisation are ignored.
+* ``GetBestRMS``: every mapping is aligned as ``AlignMol`` aligns (50 Jacobi sweeps); the result is the first mapping
+  with the strictly smallest RMSD, and the probe conformer is moved by its transform, every atom.
+  ``GetBestAlignmentTransform``: the same search with ``reflect`` and ``maxIters``; nothing moves; it returns (RMSD,
+  transform, the mapping as ((probeAtom, refAtom), ...)). ``CalcRMS``: min over k of sqrt(sum w |p - r_k|^2 / L) on the
+  coordinates as given; nothing moves.
+* Weights are one per pair in the mapping's order (one per probe atom for the matches), checked as for ``AlignMol``.
+
+Differences from RDKit for these three:
+
+* RDKit symmetrises a copy of the query before matching, so a probe and a reference that draw a carboxylate or a nitro
+  group with different bond orders match in RDKit; the restatement here finds no match for them and raises.
+  ``tools/export_rdkit_fixtures.py`` writes ``tests/golden/rdkit_best_align.npz`` where RDKit exists, and
+  ``tests/test_mol_align_best_rdkit.py`` replays it when it is present; until then the restatement and these semantics
+  are not checked against RDKit.
+* A user ``map`` is sorted by probe atom, and every mapping must cover the same probe atoms; with weights, every mapping
+  must also list them in the same order. The match tuple of ``GetBestAlignmentTransform`` lists pairs by probe atom.
+* ``numThreads`` is accepted and ignored. Mapping tables take molecules of fewer than 32768 atoms.
+* A probe conformer that is its own pair's reference conformer (``GetBestRMS(mol, mol)`` with the default ids) is
+  compared with a copy of itself taken before anything moves, so the RMSD is ~0, as in RDKit. A conformer moved as the
+  probe of one pair may not be the reference of another pair of the same call, nor moved twice (ValueError).
+* With ``coordinates=Device3DResult`` the call builds one temporary device buffer of the result's coordinates followed
+  by the references, and with ``GetBestRMSBatch`` copies the result's part back: every conformer of the result makes
+  that round trip (48 B per atom of device traffic and a second copy of ``values`` in device memory), not only the
+  listed probes.
+* Batch forms (:func:`GetBestRMSBatch`, :func:`CalcRMSBatch`, :func:`GetBestAlignmentTransformBatch`) take many probe
+  conformers per molecule pair, find the pair's matches once, and can read and move the probes of a
+  :class:`~nvmolkit_b200.types.Device3DResult` on the device.
 """
 
 from __future__ import annotations
@@ -46,7 +85,8 @@ from nvmolkit_b200.conformerRmsd import _check_list, _check_mols, _check_stream
 from nvmolkit_b200.types import AsyncGpuResult, Device3DResult
 
 __all__ = ["AlignMolConformers", "AlignMolConformersBatch", "AlignMol", "AlignMolBatch", "GetAlignmentTransform",
-           "GetAlignmentTransformBatch"]
+           "GetAlignmentTransformBatch", "GetBestRMS", "GetBestRMSBatch", "CalcRMS", "CalcRMSBatch",
+           "GetBestAlignmentTransform", "GetBestAlignmentTransformBatch"]
 
 
 def _check_iters(maxIters) -> int:
@@ -394,3 +434,280 @@ def GetAlignmentTransform(prbMol, refMol, prbCid: int = -1, refCid: int = -1, at
     rmsd, trans = GetAlignmentTransformBatch([prbMol], [refMol], [prbCid], [refCid], [atomMap], [weights], reflect,
                                              maxIters, stream=stream)
     return float(rmsd.numpy()[0]), trans.numpy()[0]
+
+
+# ---------------------------------------------------------------------------------------------- GetBestRMS
+_NO_MATCH = "No sub-structure match found between the reference and probe mol"
+
+
+def _pair_lists(prb, ref, mapping, maxMatches: int, symmetrize: bool, weights, what: str):
+    """(P, Q, weights in P's order or None) of one molecule pair: the user's ``map``, or the probe's matches inside the
+    reference (:func:`~nvmolkit_b200.rdkit_adapter.probe_ref_matches`), P = every probe atom and Q = the matches."""
+    from nvmolkit_b200.conformerRmsd import _map_lists
+
+    n_p, n_r = prb.GetNumAtoms(), ref.GetNumAtoms()
+    if max(n_p, n_r) >= 32768:
+        raise ValueError(f"{what}: mapping tables take molecules of fewer than 32768 atoms")
+    if mapping is not None and len(mapping):
+        if weights is None or len(weights) == 0:
+            P, Q = _map_lists(mapping, n_p, f"{what} map", n_r)
+            return P, Q, None
+        P, Q, perm = _map_lists(mapping, n_p, f"{what} map", n_r, order=True)
+        return P, Q, _weights(weights, len(P), f"{what} weights")[perm]
+    from nvmolkit_b200.rdkit_adapter import probe_ref_matches
+
+    w = _weights(weights, n_p, f"{what} weights")
+    matches = probe_ref_matches(prb, ref, maxMatches, symmetrize)
+    if not matches:
+        raise ValueError(_NO_MATCH)
+    Q = np.array(matches, np.int64)
+    if Q.ndim != 2 or Q.shape[1] != n_p:
+        raise ValueError(f"{what}: every match must cover all {n_p} probe atoms")
+    return np.arange(n_p, dtype=np.int64), Q, w
+
+
+def _run_best(probe, ref, sets, conf_atoms, d_cas: torch.Tensor, xyz: torch.Tensor, lists, mode: int, reflect: bool,
+              maxIters: int, move: bool, transform: bool, stream):
+    """One ``b200mol_best_align`` launch on ``stream``: (RMSD [n], best mapping [n], transforms [n, 4, 4] or None).
+    ``lists[s] = (P, Q, weights or None)``: mapping set s."""
+    from nvmolkit_b200.conformerRmsd import MapTables
+
+    probe, ref, sets = (np.ascontiguousarray(x, np.int32) for x in (probe, ref, sets))
+    conf_atoms = np.ascontiguousarray(conf_atoms, np.int32)
+    maps = MapTables([(p, q) for p, q, _ in lists])
+    weights = None
+    if any(w is not None for _, _, w in lists):
+        weights = np.ascontiguousarray(np.concatenate([np.ones(len(p)) if w is None else w for p, _, w in lists]),
+                                       np.float64)
+    n = len(probe)
+    rmsd = torch.empty(n, dtype=torch.float64, device=xyz.device)
+    best = torch.empty(n, dtype=torch.int32, device=xyz.device)
+    trans = torch.empty((n, 4, 4), dtype=torch.float64, device=xyz.device) if transform else None
+    _lib.call("b200mol_best_align", n, probe.ctypes.data, ref.ctypes.data, sets.ctypes.data, len(conf_atoms),
+              conf_atoms.ctypes.data, d_cas.data_ptr(), xyz.data_ptr(), len(lists), maps.start.ctypes.data,
+              maps.count.ctypes.data, maps.length.ctypes.data, maps.atoms.ctypes.data,
+              None if weights is None else weights.ctypes.data, mode, 1 if reflect else 0, maxIters, 1 if move else 0,
+              rmsd.data_ptr() if n else None, best.data_ptr() if n else None,
+              trans.data_ptr() if transform and n else None, stream_ptr(stream))
+    return rmsd, best, trans
+
+
+def _best_batch(prbMols, refMols, prbIds, refIds, maps, maxMatches, symmetrize, weights, reflect, maxIters, mode: int,
+                move: bool, transform: bool, coordinates, stream):
+    """The jobs of every molecule pair in one launch: (per-pair sizes, RMSD, best mapping, transforms or None, the
+    mapping sets)."""
+    _check_stream(stream)
+    prbMols, refMols = _check_mols(prbMols), _check_mols(refMols)
+    maxIters = _check_iters(maxIters)
+    if int(maxMatches) < 1:
+        raise ValueError(f"maxMatches must be >= 1, got {maxMatches}")
+    n = len(prbMols)
+    if len(refMols) != n:
+        raise ValueError(f"refMols holds {len(refMols)} molecules, prbMols {n}")
+    prbIds, maps, weights = (_per_mol(a, n, w) for a, w in ((prbIds, "prbIds"), (maps, "maps"), (weights, "weights")))
+    refIds = [-1] * n if refIds is None else _per_mol(refIds, n, "refIds")
+
+    if coordinates is not None:
+        if not isinstance(coordinates, Device3DResult):
+            raise TypeError(f"coordinates must be a Device3DResult, got {type(coordinates).__name__}")
+        if coordinates.n_mols != n:
+            raise ValueError(f"coordinates hold {coordinates.n_mols} molecules, prbMols has {n}")
+        values = coordinates.values.torch()
+        if values.dtype != torch.float64 or values.ndim != 2 or values.shape[1] != 3 or not values.is_contiguous():
+            raise ValueError("coordinates.values must be a contiguous float64 (n, 3) tensor")
+        atom_counts = np.array([m.GetNumAtoms() for m in prbMols], np.int64)
+        order, dev_counts, starts_t = device_conformer_order(coordinates, atom_counts)
+        conf_idx = coordinates.conf_indices.torch().cpu().numpy().astype(np.int64)[order]
+        dev_first = np.concatenate([[0], np.cumsum(dev_counts)]).astype(np.int64)
+        n_dev = len(order)
+        dev_atoms = np.empty(n_dev, np.int64)
+        dev_atoms[order] = np.repeat(atom_counts, dev_counts)
+    else:
+        n_dev = 0
+
+    # RDKit conformers get slots n_dev, n_dev + 1, ...; device conformer c of the result is slot c
+    slots, blocks, confs = {}, [], []
+
+    def slot(mol, conf):
+        key = (id(mol), conf.GetId())
+        if key not in slots:
+            slots[key] = n_dev + len(blocks)
+            blocks.append(np.asarray(conf.GetPositions(), np.float64).reshape(-1, 3))
+            confs.append(conf)
+        return slots[key]
+
+    cache, lists = {}, []
+    probe, ref, sets, sizes = [], [], [], []
+    for m, (prb, refm) in enumerate(zip(prbMols, refMols)):
+        rc = _conformer(refm, refIds[m], f"refMols[{m}]")
+        key = (id(prb), id(refm), id(maps[m]) if maps[m] is not None and len(maps[m]) else None,
+               id(weights[m]) if weights[m] is not None and len(weights[m]) else None)
+        if key not in cache:
+            cache[key] = len(lists)
+            lists.append(_pair_lists(prb, refm, maps[m], int(maxMatches), bool(symmetrize), weights[m],
+                                     f"pair {m}"))
+        s, r = cache[key], slot(refm, rc)
+        if coordinates is None:
+            if prbIds[m] is None:
+                pcs = [c for c in prb.GetConformers() if not (prb is refm and c.GetId() == rc.GetId())]
+            else:
+                pcs = [_conformer(prb, cid, f"prbMols[{m}]") for cid in prbIds[m]]
+            ps = [slot(prb, c) for c in pcs]
+            if r in ps:  # the reference conformer is also this pair's probe: it is read from a copy taken beforehand
+                blocks.append(blocks[r - n_dev].copy())
+                confs.append(None)
+                r = n_dev + len(blocks) - 1
+        else:
+            mine = order[dev_first[m]:dev_first[m + 1]]
+            if prbIds[m] is None:
+                ps = [int(c) for c in mine]
+            else:
+                where = {int(cid): int(c) for cid, c in zip(conf_idx[dev_first[m]:dev_first[m + 1]], mine)}
+                ps = []
+                for cid in prbIds[m]:
+                    if int(cid) not in where:
+                        raise ValueError(f"coordinates: molecule {m} has no conformer with id {cid}")
+                    ps.append(where[int(cid)])
+        probe += ps
+        ref += [r] * len(ps)
+        sets += [s] * len(ps)
+        sizes.append(len(ps))
+    if move:
+        refs, moved = set(ref), set()
+        for p in probe:
+            if p in refs or p in moved:
+                raise ValueError("a probe conformer is moved twice or is also a reference")
+            moved.add(p)
+    if not probe:
+        empty = torch.zeros(0, dtype=torch.float64)
+        return sizes, empty, torch.zeros(0, dtype=torch.int32), torch.zeros((0, 4, 4), dtype=torch.float64) if transform else None, lists
+
+    require_cuda()
+    host_atoms = np.array([len(b) for b in blocks], np.int64)
+    if coordinates is None:
+        dev = torch.device("cuda", torch.cuda.current_device())
+        with torch.cuda.device(dev), stream_ctx(stream):
+            xyz = torch.from_numpy(np.ascontiguousarray(np.concatenate(blocks))).to(dev)
+            d_cas = torch.from_numpy(np.concatenate([[0], np.cumsum(host_atoms)]).astype(np.int32)).to(dev)
+            rmsd, best, trans = _run_best(probe, ref, sets, host_atoms, d_cas, xyz, lists, mode, reflect, maxIters,
+                                          move, transform, stream)
+            out = xyz.cpu().numpy() if move else None
+        if move:
+            from rdkit.Geometry import Point3D
+
+            bounds = np.concatenate([[0], np.cumsum(host_atoms)])
+            for p in sorted(set(probe)):
+                for a, (x, y, z) in enumerate(out[bounds[p]:bounds[p + 1]]):
+                    confs[p].SetAtomPosition(a, Point3D(float(x), float(y), float(z)))
+    else:
+        dev = values.device
+        n_val = values.shape[0]
+        with torch.cuda.device(dev), stream_ctx(stream):
+            refs_host = np.concatenate(blocks)
+            xyz = torch.cat([values, torch.from_numpy(np.ascontiguousarray(refs_host)).to(dev)])
+            ref_starts = torch.from_numpy((n_val + np.concatenate([[0], np.cumsum(host_atoms)[:-1]])).astype(np.int32))
+            d_cas = torch.cat([starts_t[:n_dev].to(device=dev, dtype=torch.int32), ref_starts.to(dev)]).contiguous()
+            rmsd, best, trans = _run_best(probe, ref, sets, np.concatenate([dev_atoms, host_atoms]), d_cas, xyz, lists,
+                                          mode, reflect, maxIters, move, transform, stream)
+            if move:
+                values.copy_(xyz[:n_val])
+    return sizes, rmsd, best, trans, lists
+
+
+def _split(t: Optional[torch.Tensor], sizes) -> List[AsyncGpuResult]:
+    return [AsyncGpuResult(v) for v in torch.split(t, sizes)]
+
+
+def GetBestRMSBatch(prbMols, refMols, prbIds=None, refIds=None, maps=None, maxMatches: int = 1000000,
+                    symmetrizeConjugatedTerminalGroups: bool = True, weights=None, *,
+                    coordinates: Optional[Device3DResult] = None,
+                    stream: Optional[torch.cuda.Stream] = None) -> List[AsyncGpuResult]:
+    """``GetBestRMS`` of many probe conformers per molecule pair, in one launch: every listed probe conformer of
+    ``prbMols[m]`` is aligned onto conformer ``refIds[m]`` of ``refMols[m]`` by its best mapping and moved. Returns one
+    :class:`AsyncGpuResult` per pair: the float64 RMSDs of its probes, in order.
+
+    ``prbIds[m]``: probe conformer ids, ``None`` for every conformer except the reference conformer itself;
+    ``refIds[m]``: one reference conformer id (-1: the first); ``maps[m]``: ``None`` for the probe's matches inside the
+    reference, or mappings of (probeAtom, refAtom) pairs; ``weights[m]``: one per pair, or ``None``. The matches of a
+    pair are found once, whatever its number of conformers.
+
+    ``coordinates``: a :class:`Device3DResult` whose molecule m holds the probe conformers of pair m (``prbIds`` name
+    its ``conf_indices`` values); they are moved in place on the device, asynchronously on ``stream``; the references
+    still come from ``refMols``. Its ``values`` must be a contiguous float64 (n, 3) tensor. Without it the RDKit
+    conformers are read, aligned and written back. A probe conformer may be moved once and may not be the reference of
+    another pair; a probe that is its own pair's reference is aligned onto a copy of itself."""
+    sizes, rmsd, _, _, _ = _best_batch(prbMols, refMols, prbIds, refIds, maps, maxMatches,
+                                       symmetrizeConjugatedTerminalGroups, weights, False, 50, 0, True, False,
+                                       coordinates, stream)
+    return _split(rmsd, sizes)
+
+
+def CalcRMSBatch(prbMols, refMols, prbIds=None, refIds=None, maps=None, maxMatches: int = 1000000,
+                 symmetrizeConjugatedTerminalGroups: bool = True, weights=None, *,
+                 coordinates: Optional[Device3DResult] = None,
+                 stream: Optional[torch.cuda.Stream] = None) -> List[AsyncGpuResult]:
+    """``CalcRMS`` as :func:`GetBestRMSBatch` lays it out: per probe the smallest RMSD over the mappings on the
+    coordinates as given, without alignment. Nothing is moved."""
+    sizes, rmsd, _, _, _ = _best_batch(prbMols, refMols, prbIds, refIds, maps, maxMatches,
+                                       symmetrizeConjugatedTerminalGroups, weights, False, 50, 1, False, False,
+                                       coordinates, stream)
+    return _split(rmsd, sizes)
+
+
+def GetBestAlignmentTransformBatch(prbMols, refMols, prbIds=None, refIds=None, maps=None, maxMatches: int = 1000000,
+                                   symmetrizeConjugatedTerminalGroups: bool = True, weights=None,
+                                   reflect: bool = False, maxIters: int = 50, *,
+                                   coordinates: Optional[Device3DResult] = None,
+                                   stream: Optional[torch.cuda.Stream] = None
+                                   ) -> Tuple[List[AsyncGpuResult], List[AsyncGpuResult], List[AsyncGpuResult]]:
+    """``GetBestAlignmentTransform`` as :func:`GetBestRMSBatch` lays it out; nothing is moved. Returns per pair (RMSDs,
+    float64 transforms [n, 4, 4], int32 index of the best mapping: into ``maps[m]``, or into the pair's matches)."""
+    sizes, rmsd, best, trans, _ = _best_batch(prbMols, refMols, prbIds, refIds, maps, maxMatches,
+                                              symmetrizeConjugatedTerminalGroups, weights, reflect, maxIters, 0, False,
+                                              True, coordinates, stream)
+    return _split(rmsd, sizes), _split(trans, sizes), _split(best, sizes)
+
+
+def _one(prbMol, refMol, prbId, refId, map, maxMatches, symmetrize, weights, reflect, maxIters, mode, move, transform,
+         stream):
+    _check_stream(stream)
+    if prbMol is None or refMol is None:
+        raise ValueError("prbMol and refMol must not be None")
+    prbId = _conformer(prbMol, prbId, "prbMol").GetId()
+    return _best_batch([prbMol], [refMol], [[prbId]], [refId], [map], maxMatches, symmetrize, [weights], reflect,
+                       maxIters, mode, move, transform, None, stream)
+
+
+def GetBestRMS(prbMol, refMol, prbId: int = -1, refId: int = -1, map=None, maxMatches: int = 1000000,
+               symmetrizeConjugatedTerminalGroups: bool = True, weights=None, numThreads: int = 1, *,
+               stream: Optional[torch.cuda.Stream] = None) -> float:
+    """The RMSD of conformer ``prbId`` of ``prbMol`` aligned onto conformer ``refId`` of ``refMol`` by the best of their
+    atom mappings, and the probe conformer moved by that alignment (RDKit ``rdMolAlign.GetBestRMS``)."""
+    _, rmsd, _, _, _ = _one(prbMol, refMol, prbId, refId, map, maxMatches, symmetrizeConjugatedTerminalGroups, weights,
+                            False, 50, 0, True, False, stream)
+    return float(rmsd.cpu()[0])
+
+
+def CalcRMS(prbMol, refMol, prbId: int = -1, refId: int = -1, map=None, maxMatches: int = 1000000,
+            symmetrizeConjugatedTerminalGroups: bool = True, weights=None, *,
+            stream: Optional[torch.cuda.Stream] = None) -> float:
+    """The smallest RMSD over the atom mappings between two conformers as they are, without alignment (RDKit
+    ``rdMolAlign.CalcRMS``); nothing is moved."""
+    _, rmsd, _, _, _ = _one(prbMol, refMol, prbId, refId, map, maxMatches, symmetrizeConjugatedTerminalGroups, weights,
+                            False, 50, 1, False, False, stream)
+    return float(rmsd.cpu()[0])
+
+
+def GetBestAlignmentTransform(prbMol, refMol, prbId: int = -1, refId: int = -1, map=None, maxMatches: int = 1000000,
+                              symmetrizeConjugatedTerminalGroups: bool = True, weights=None, reflect: bool = False,
+                              maxIters: int = 50, numThreads: int = 1, *, stream: Optional[torch.cuda.Stream] = None
+                              ) -> Tuple[float, np.ndarray, Tuple[Tuple[int, int], ...]]:
+    """(RMSD, 4 x 4 transform, the best mapping as ((probeAtom, refAtom), ...)) of the best alignment of ``prbMol`` onto
+    ``refMol`` over their atom mappings; nothing is moved (RDKit ``rdMolAlign.GetBestAlignmentTransform``). The pairs
+    are listed by probe atom."""
+    _, rmsd, best, trans, lists = _one(prbMol, refMol, prbId, refId, map, maxMatches,
+                                       symmetrizeConjugatedTerminalGroups, weights, reflect, maxIters, 0, False, True,
+                                       stream)
+    P, Q, _ = lists[0]
+    k = int(best.cpu()[0])
+    return float(rmsd.cpu()[0]), trans.cpu().numpy()[0], tuple((int(p), int(q)) for p, q in zip(P, Q[k]))

@@ -520,23 +520,25 @@ def _terminal_groups(mol) -> List[List[int]]:
     return groups
 
 
-def self_matches(mol, maxMatches: int = 1000000, symmetrizeConjugatedTerminalGroups: bool = True) -> List[Tuple[int, ...]]:
-    """The matches of a molecule onto itself that RDKit's ``GetBestRMS`` / ``GetAllConformerBestRMS`` enumerate:
-    ``mol.GetSubstructMatches(mol, uniquify=False, maxMatches=maxMatches, useChirality=False)``; ``match[q]`` is the atom
-    that query atom q lands on.
+def probe_ref_matches(prb, ref, maxMatches: int = 1000000, symmetrizeConjugatedTerminalGroups: bool = True
+                      ) -> List[Tuple[int, ...]]:
+    """The matches of a probe molecule inside a reference molecule that RDKit's ``GetBestRMS`` /
+    ``GetBestAlignmentTransform`` / ``CalcRMS`` enumerate: ``ref.GetSubstructMatches(prb, uniquify=False,
+    maxMatches=maxMatches, useChirality=False)``; ``match[q]`` is the reference atom that probe atom q lands on.
 
     With ``symmetrizeConjugatedTerminalGroups`` this restates RDKit's symmetrised query on the matches instead of on a
     query copy: every match m is followed by m composed with every permutation that reorders the atoms within each
-    group of :func:`_terminal_groups` (``m'[q] = m[s[q]]``), in lexicographic order of the permutations, duplicates
-    dropped, and the list cut at ``maxMatches``. The restatement is what the tests pin, not RDKit itself."""
+    group of :func:`_terminal_groups` of the probe (``m'[q] = m[s[q]]``), in lexicographic order of the permutations,
+    duplicates dropped, and the list cut at ``maxMatches``. The restatement is what the tests pin, not RDKit itself.
+    An empty list means no match."""
     import itertools
 
     matches = [tuple(int(a) for a in m) for m in
-               mol.GetSubstructMatches(mol, uniquify=False, maxMatches=maxMatches, useChirality=False)]
-    groups = _terminal_groups(mol) if symmetrizeConjugatedTerminalGroups else []
+               ref.GetSubstructMatches(prb, uniquify=False, maxMatches=maxMatches, useChirality=False)]
+    groups = _terminal_groups(prb) if symmetrizeConjugatedTerminalGroups else []
     if not groups:
         return matches[:maxMatches]
-    n = mol.GetNumAtoms()
+    n = prb.GetNumAtoms()
     perms = []
     for choice in itertools.product(*[list(itertools.permutations(g)) for g in groups]):
         s = list(range(n))
@@ -554,3 +556,9 @@ def self_matches(mol, maxMatches: int = 1000000, symmetrizeConjugatedTerminalGro
                 if len(out) == maxMatches:
                     return out
     return out
+
+
+def self_matches(mol, maxMatches: int = 1000000, symmetrizeConjugatedTerminalGroups: bool = True) -> List[Tuple[int, ...]]:
+    """The matches of a molecule onto itself that RDKit's ``GetBestRMS`` / ``GetAllConformerBestRMS`` enumerate:
+    :func:`probe_ref_matches` ``(mol, mol, maxMatches, symmetrizeConjugatedTerminalGroups)``."""
+    return probe_ref_matches(mol, mol, maxMatches, symmetrizeConjugatedTerminalGroups)

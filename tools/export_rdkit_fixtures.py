@@ -20,6 +20,12 @@ and commit the resulting .npz. `tests/test_rdkit_fixtures.py` then replays it (s
   * alignment (to tests/golden/rdkit_align.npz, replayed by tests/test_mol_align_rdkit.py): rdMolAlign.AlignMolConformers
     RMS lists and aligned coordinates over all atoms, heavy-atom atomIds, weights and reflect; rdMolAlign.AlignMol RMSDs
     and moved coordinates and GetAlignmentTransform matrices with atom maps, weights and reflect
+  * best alignment (to tests/golden/rdkit_best_align.npz, replayed by tests/test_mol_align_best_rdkit.py):
+    rdMolAlign.GetBestRMS (RMSD and moved coordinates), CalcRMS and GetBestAlignmentTransform (RMSD, transform, match)
+    of every conformer against conformer 0 of a second copy of the molecule, on heavy-atom molecules with ring flips,
+    carboxylates and a nitro group, with and without weights and symmetrizeConjugatedTerminalGroups; with each
+    molecule's atoms, bonds (conjugation included) and raw GetSubstructMatches, so that the matching restatement
+    (nvmolkit_b200.rdkit_adapter.probe_ref_matches) can be replayed without RDKit
 
 The default molecule set is a small drug-like SMILES list embedded below (aspirin, ibuprofen, caffeine, ...); pass
 --smiles benchmarks/data/chembl_10k.smi of the reference checkout for the BASELINE configs' real input.
@@ -158,6 +164,7 @@ def main() -> None:
     print(f"wrote {args.out}: {len(mols)} molecules, {len(hmols)} with conformers, RDKit {rdkit.__version__}")
     export_tfd(hmols, os.path.join(os.path.dirname(os.path.abspath(args.out)), "rdkit_tfd.npz"))
     export_align(hmols, os.path.join(os.path.dirname(os.path.abspath(args.out)), "rdkit_align.npz"))
+    export_best_align(os.path.join(os.path.dirname(os.path.abspath(args.out)), "rdkit_best_align.npz"))
 
 
 def export_tfd(hmols, path: str, n_confs: int = 6) -> None:
@@ -254,6 +261,59 @@ def export_align(hmols, path: str, n_confs: int = 5) -> None:
     out["n_amc"], out["n_am"] = np.array(k), np.array(j)
     np.savez_compressed(path, **out)
     print(f"wrote {path}: {k} AlignMolConformers and {j} AlignMol cases")
+
+
+BEST_ALIGN_SMILES = ["[O-]C(=O)c1ccccc1", "CC(C)(C)c1ccc(cc1)C(=O)[O-]", "Cc1ccc(cc1)[N+](=O)[O-]", "OC(=O)CC1CC1",
+                     "c1ccc(cc1)-c1ccccc1", "CC(=O)Oc1ccccc1C(=O)O", "OC(=O)[C@@H]1CCCN1"]
+
+
+def export_best_align(path: str, n_confs: int = 4, max_matches: int = 1000000) -> None:
+    """RDKit's GetBestRMS / CalcRMS / GetBestAlignmentTransform on heavy-atom ETKDG conformers. Molecule i:
+    ``bam{i}_z`` [n], ``_bonds`` [B, 3] (begin, end, conjugated), ``_raw`` [M, n] (``GetSubstructMatches(mol,
+    uniquify=False, maxMatches, useChirality=False)``), ``_xyz`` [C, n, 3]. Case j: ``ba{j}_mol``, ``_conf`` (the probe
+    conformer; the reference is conformer 0 of a second copy), ``_sym``, ``_weights`` (empty: none), ``_calc``
+    (CalcRMS), ``_trmsd`` / ``_transform`` / ``_match`` [L, 2] (GetBestAlignmentTransform), ``_rmsd`` / ``_moved``
+    (GetBestRMS and the probe conformer after it)."""
+    import rdkit
+    from rdkit import Chem
+    from rdkit.Chem import rdDistGeom, rdMolAlign
+
+    out = {"rdkit_version": np.array(rdkit.__version__), "max_matches": np.array(max_matches)}
+    rng = np.random.default_rng(7)
+    i = j = 0
+    for smi in BEST_ALIGN_SMILES:
+        mh = Chem.AddHs(Chem.MolFromSmiles(smi))
+        p = rdDistGeom.ETKDGv3()
+        p.randomSeed = 13
+        if len(rdDistGeom.EmbedMultipleConfs(mh, n_confs, p)) < 2:
+            continue
+        m = Chem.RemoveHs(mh)
+        n = m.GetNumAtoms()
+        ids = [c.GetId() for c in m.GetConformers()]
+        out[f"bam{i}_z"] = np.array([a.GetAtomicNum() for a in m.GetAtoms()], np.int64)
+        out[f"bam{i}_bonds"] = np.array([(b.GetBeginAtomIdx(), b.GetEndAtomIdx(), int(b.GetIsConjugated()))
+                                         for b in m.GetBonds()], np.int64).reshape(-1, 3)
+        out[f"bam{i}_raw"] = np.array(m.GetSubstructMatches(m, uniquify=False, maxMatches=max_matches,
+                                                            useChirality=False), np.int64).reshape(-1, n)
+        out[f"bam{i}_xyz"] = np.array([m.GetConformer(c).GetPositions() for c in ids])
+        for sym, weighted in ((True, False), (False, False), (True, True), (False, True)):
+            w = rng.uniform(0.5, 2.0, n).tolist() if weighted else []
+            kw = dict(maxMatches=max_matches, symmetrizeConjugatedTerminalGroups=sym, weights=w)
+            for c in range(1, len(ids)):
+                prb, ref = Chem.Mol(m), Chem.Mol(m)  # conformers of one molecule read as two objects
+                out[f"ba{j}_mol"], out[f"ba{j}_conf"] = np.array(i), np.array(c)
+                out[f"ba{j}_sym"], out[f"ba{j}_weights"] = np.array(sym), np.array(w, np.float64)
+                out[f"ba{j}_calc"] = np.array(rdMolAlign.CalcRMS(prb, ref, ids[c], ids[0], **kw))
+                rmsd, T, match = rdMolAlign.GetBestAlignmentTransform(prb, ref, ids[c], ids[0], **kw)
+                out[f"ba{j}_trmsd"], out[f"ba{j}_transform"] = np.array(rmsd), np.asarray(T, np.float64)
+                out[f"ba{j}_match"] = np.array(match, np.int64).reshape(-1, 2)
+                out[f"ba{j}_rmsd"] = np.array(rdMolAlign.GetBestRMS(prb, ref, ids[c], ids[0], **kw))
+                out[f"ba{j}_moved"] = prb.GetConformer(ids[c]).GetPositions()
+                j += 1
+        i += 1
+    out["n_bam"], out["n_ba"] = np.array(i), np.array(j)
+    np.savez_compressed(path, **out)
+    print(f"wrote {path}: {i} molecules, {j} best-alignment cases")
 
 
 if __name__ == "__main__":
