@@ -604,7 +604,8 @@ int b200mol_best_align(int32_t nJobs, const int32_t* h_job_probe, const int32_t*
  * Matrices are concatenated: matrix m occupies d_x[starts[m] .. starts[m+1]) = n_m * n_m doubles, row-major.
  * ---------------------------------------------------------------------------------------- */
 /* In-place triangle-inequality smoothing of RDKit bounds matrices ([i][j], i<j = upper bound; [j][i] = lower bound).
- * d_ok[m] = 1 consistent / 0 inconsistent (lb > ub found; matrix left partially smoothed). tol as in RDKit
+ * d_ok[m] = 1 consistent / 0 inconsistent (lb > ub found: the pivot in which it first appears is completed for every
+ * pair, later pivots are not run). tol as in RDKit
  * triangleSmoothBounds (0 = strict). Replaces triangleSmoothBoundsBatch (src/triangle_smooth.cu:132-247) and the CPU
  * call DistGeom::triangleSmoothBounds in src/embedder_utils.cpp:313,324. */
 int b200mol_triangle_smooth(double* d_bounds, const int64_t* d_matrix_starts, int32_t nMats, double tol, int8_t* d_ok,
@@ -612,14 +613,19 @@ int b200mol_triangle_smooth(double* d_bounds, const int64_t* d_matrix_starts, in
 /* Top-numEigs eigenpairs by power iteration with deflation (RDKit PowerEigenSolver: tol 1e-3, <= 1000 iterations).
  * d_mats is destroyed. d_v0 (optional) start vectors, numEigs * n_m per matrix at d_v0_starts[m]; NULL = hashed
  * counter sequence from `seed`. d_eigvals[m][numEigs]; d_eigvecs row e of matrix m at d_vec_starts[m] + e * n_m;
- * d_n_converged[m] = number of eigenpairs found. Replaces BatchedEigenSolver::solve
- * (src/symmetric_eigensolver.cu:62-247). */
+ * d_n_converged[m] = number of eigenpairs found; the outputs of eigenpairs past it are left unwritten. The two
+ * n-vectors of the iteration stay in shared memory (28160 doubles) even when the matrix itself does not fit there, so
+ * n <= 14080: a larger matrix gets d_n_converged[m] = 0 and nothing else is written for it. Replaces
+ * BatchedEigenSolver::solve (src/symmetric_eigensolver.cu:62-247). */
 int b200mol_eig_topk(double* d_mats, const int64_t* d_matrix_starts, int32_t nMats, int numEigs, const double* d_v0,
                      const int64_t* d_v0_starts, uint32_t seed, double* d_eigvals, double* d_eigvecs,
                      const int64_t* d_vec_starts, int8_t* d_n_converged, void* stream);
 /* Distance matrix -> metric matrix -> top-`dim` eigenpairs -> coordinates d_coords[(atom_starts[m]+i)*dim + j] =
  * sqrt(lambda_j) v_j[i]; d_ok[m] = 0 when an eigenvalue is not positive or did not converge (3-D AND 4-D; the
- * reference's InitialCoordinateGenerator is 3-D only, src/forcefields/coord_gen.cu:64,160). d_dist is destroyed. */
+ * reference's InitialCoordinateGenerator is 3-D only, src/forcefields/coord_gen.cu:64,160). d_dist is destroyed.
+ * Coordinates of a matrix with d_ok[m] = 0 are left unwritten. The iteration vectors, eigenpairs and row means,
+ * (3 + dim) n + dim doubles, stay in shared memory (28160 doubles), so n <= 4692 at dim 3 and n <= 4022 at dim 4:
+ * a larger matrix gets d_ok[m] = 0. */
 int b200mol_metric_embed(double* d_dist, const int64_t* d_matrix_starts, const int32_t* d_atom_starts, int32_t nMats,
                          int dim, const double* d_v0, const int64_t* d_v0_starts, uint32_t seed, double* d_coords,
                          int8_t* d_ok, void* stream);

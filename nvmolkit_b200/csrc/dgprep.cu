@@ -77,7 +77,9 @@ __global__ void __launch_bounds__(kT) eigenKernel(int mode, double* mats, const 
                                                 const long long* vecStarts, double* coords, const int* atomStarts,
                                                 int8_t* ok) {
   extern __shared__ __align__(16) double sm[];
-  __shared__ double                     red[16];
+  __shared__ double                     red[kEigRed];
+  static_assert(sizeof(red) >= kEigWarps * (sizeof(double) + sizeof(int)),
+                "powerEigen's argmax needs a double and an int per warp in `red`");
   for (int m = blockIdx.x; m < nMats; m += gridDim.x) {
     double*         g    = mats + starts[m];
     const long long size = starts[m + 1] - starts[m];
@@ -86,6 +88,10 @@ __global__ void __launch_bounds__(kT) eigenKernel(int mode, double* mats, const 
     double*         z    = sm + n;
     double*         vecs = sm + 2 * n;  // numEigs * n (mode 1 keeps them on chip)
     const int       head = 2 * n + (mode == 1 ? numEigs * n + numEigs + n : 0);
+    if (head > smemCapDoubles) {  // v, z (and in mode 1 the eigenpairs and sq0) always live on chip: refuse the matrix
+      if (threadIdx.x == 0) ok[m] = 0;
+      continue;  // n is the same for every thread, so the whole CTA moves on
+    }
     const bool      useS = size + head <= smemCapDoubles;
     double*         mat  = useS ? sm + head : g;
     double*         ev   = mode == 1 ? vecs + numEigs * n : eigvals + static_cast<size_t>(m) * numEigs;

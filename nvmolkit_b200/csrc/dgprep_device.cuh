@@ -9,6 +9,9 @@ namespace b200 {
 #define B200_BFGS_THREADS 256
 #endif
 constexpr int kEigT = B200_BFGS_THREADS;  // threads per CTA of every caller (the embedder's CTA shape)
+constexpr int kEigWarps = kEigT / 32;
+// Doubles of shared memory behind powerEigen's `red`: one double per warp, then the argmax index of each warp as an int.
+constexpr int kEigRed = kEigWarps + (kEigWarps * static_cast<int>(sizeof(int)) + 7) / 8;
 
 __device__ __forceinline__ double warpSumD(double v) {
 #pragma unroll
@@ -26,11 +29,12 @@ __device__ __forceinline__ uint32_t hash32(uint32_t x) {  // counter-based start
   return x;
 }
 
-// mat: n x n symmetric (destroyed by deflation); v, z: n doubles of shared memory; red: 16 doubles.
+// mat: n x n symmetric (destroyed by deflation); v, z: n doubles of shared memory; red: kEigRed doubles.
 // Returns (to all threads) the number of converged eigenpairs. eigvecs: [numEigs][n].
 __device__ inline int powerEigen(double* mat, int n, int numEigs, const double* v0, uint32_t seed, double* v, double* z,
                           double* red, double* eigvals, double* eigvecs) {
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nWarps = kEigT / 32;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nWarps = kEigWarps;
+  int*      redIdx = reinterpret_cast<int*>(red + nWarps);
   int       done = 0;
   for (int e = 0; e < numEigs; ++e) {
     double part = 0.0;
@@ -77,15 +81,15 @@ __device__ inline int powerEigen(double* mat, int n, int numEigs, const double* 
         }
       }
       if (lane == 0) {
-        red[warp]                                    = best;
-        reinterpret_cast<int*>(red + 8)[warp]        = bi;
+        red[warp]    = best;
+        redIdx[warp] = bi;
       }
       __syncthreads();
       best = red[0];
-      bi   = reinterpret_cast<int*>(red + 8)[0];
+      bi   = redIdx[0];
       for (int w = 1; w < nWarps; ++w) {
         const double ob = red[w];
-        const int    oi = reinterpret_cast<int*>(red + 8)[w];
+        const int    oi = redIdx[w];
         if (fabs(ob) > fabs(best) || (fabs(ob) == fabs(best) && oi < bi)) {
           best = ob;
           bi   = oi;

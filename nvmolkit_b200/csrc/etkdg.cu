@@ -84,6 +84,8 @@ __device__ bool anyFail(bool mine);
 // Metric start = RDKit DistGeom::pickRandomDistMat + computeInitialCoords (Code/DistGeom/DistGeomUtils.cpp of the
 // un-vendored RDKit 2025.03, restated: EIGVAL_TOL 1e-3, randNegEig = true, numZeroFail = 1) with the reference's power
 // eigensolver (src/symmetric_eigensolver.cu:62-247, dgprep_device.cuh).
+static_assert(kRed * sizeof(double) >= kEigWarps * (sizeof(double) + sizeof(int)),
+              "powerEigen's argmax needs a double and an int per warp in `red`");
 __device__ bool initialCoords(const b200mol_embed_params& par, const b200mol_dg_system& dg, int mol, int nA, int slot,
                               int attempt, double* pos, double* work, double* mat, double* red) {
   const int tid = threadIdx.x, n = 4 * nA;

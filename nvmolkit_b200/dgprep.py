@@ -11,6 +11,18 @@ from nvmolkit_b200 import _lib
 from nvmolkit_b200._interop import require_cuda, stream_ctx, stream_ptr
 
 
+# The eigen kernel keeps its per-matrix vectors in 220 KB of shared memory even when the matrix itself is in global
+# memory: 2 n doubles for eig_topk, (3 + dim) n + dim for metric_embed (include/b200mol.h).
+_SMEM_DOUBLES = 220 * 1024 // 8
+
+
+def _check_head(ns, per_atom: int, extra: int, what: str) -> None:
+    big = [int(n) for n in ns if per_atom * int(n) + extra > _SMEM_DOUBLES]
+    if big:
+        raise ValueError(f"{what}: matrices of {max(big)} atoms exceed the largest supported size "
+                         f"{(_SMEM_DOUBLES - extra) // per_atom}")
+
+
 def _concat(mats: Sequence[np.ndarray], dev):
     sizes = np.array([m.shape[0] * m.shape[0] for m in mats], dtype=np.int64)
     starts = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
@@ -37,6 +49,7 @@ def eig_topk(mats: Sequence[np.ndarray], num_eigs: int, v0: Optional[Sequence[np
     require_cuda()
     dev = torch.device("cuda", torch.cuda.current_device())
     ns = np.array([m.shape[0] for m in mats], dtype=np.int64)
+    _check_head(ns, 2, 0, "eig_topk")
     with stream_ctx(stream):
         d, st, _ = _concat(mats, dev)
         vstarts = np.concatenate([[0], np.cumsum(ns * num_eigs)]).astype(np.int64)
@@ -58,6 +71,7 @@ def metric_embed(dists: Sequence[np.ndarray], dim: int = 3, v0: Optional[Sequenc
     require_cuda()
     dev = torch.device("cuda", torch.cuda.current_device())
     ns = np.array([m.shape[0] for m in dists], dtype=np.int64)
+    _check_head(ns, 3 + dim, dim, "metric_embed")
     with stream_ctx(stream):
         d, st, _ = _concat(dists, dev)
         astarts = np.concatenate([[0], np.cumsum(ns)]).astype(np.int32)

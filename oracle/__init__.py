@@ -349,6 +349,33 @@ def power_eigen(mat: np.ndarray, num_eigs: int, v0: np.ndarray):
     return vals, vecs, k
 
 
+def power_eigen_trace(mat: np.ndarray, num_eigs: int, v0: np.ndarray):
+    """power_eigen plus, per attempted eigenpair, (iterations, |eig - prev| margin to 1e-3, |eig| margin to 1e-10).
+    Returns (vals, vecs, k, iters, conv_margin, zero_margin); trace entries past the last attempted pair are -1 / inf."""
+    L = lib()
+    m = np.array(mat, dtype=np.float64, order="C", copy=True)
+    n = m.shape[0]
+    v0 = np.ascontiguousarray(v0, dtype=np.float64)
+    vals, vecs = np.zeros(num_eigs), np.zeros((num_eigs, n))
+    iters = np.full(num_eigs, -1, np.int32)
+    conv, zero = np.full(num_eigs, np.inf), np.full(num_eigs, np.inf)
+    L.oracle_power_eigen_trace.restype = C.c_int
+    k = L.oracle_power_eigen_trace(m.ctypes.data_as(C.c_void_p), C.c_int(n), C.c_int(num_eigs), v0.ctypes.data_as(C.c_void_p),
+                                   vals.ctypes.data_as(C.c_void_p), vecs.ctypes.data_as(C.c_void_p),
+                                   iters.ctypes.data_as(C.c_void_p), conv.ctypes.data_as(C.c_void_p),
+                                   zero.ctypes.data_as(C.c_void_p))
+    return vals, vecs, k, iters, conv, zero
+
+
+def metric_matrix(dist: np.ndarray) -> np.ndarray:
+    """RDKit computeInitialCoords' metric matrix of a distance matrix."""
+    L = lib()
+    d = np.ascontiguousarray(dist, dtype=np.float64)
+    T = np.zeros(d.shape)
+    L.oracle_metric_matrix(d.ctypes.data_as(C.c_void_p), C.c_int(d.shape[0]), T.ctypes.data_as(C.c_void_p))
+    return T
+
+
 def metric_embed(dist: np.ndarray, dim: int, v0: np.ndarray):
     """Distance matrix -> coordinates [n, dim] (or None when an eigenvalue is not positive)."""
     L = lib()

@@ -43,8 +43,12 @@ int oracle_triangle_smooth(double* b, int n, double tol) {
 }
 
 /* Top-numEigs eigenpairs of the symmetric n x n matrix `m` (destroyed by deflation). v0[numEigs*n] = start vectors.
- * eigvals[numEigs], eigvecs[numEigs*n] (row e = eigenvector e). Returns the number of eigenpairs that converged. */
-int oracle_power_eigen(double* m, int n, int numEigs, const double* v0, double* eigvals, double* eigvecs) {
+ * eigvals[numEigs], eigvecs[numEigs*n] (row e = eigenvector e). Returns the number of eigenpairs that converged.
+ * The trace arrays (numEigs each, or NULL) describe every eigenpair attempted, the failed last one included:
+ * iters[e] = power iterations run; convMargin[e] = min over iterations of | |eig - prev| - 1e-3 |, zeroMargin[e] = min of
+ * | |eig| - 1e-10 |, i.e. how close each stopping decision came to going the other way. */
+int oracle_power_eigen_trace(double* m, int n, int numEigs, const double* v0, double* eigvals, double* eigvecs, int* iters,
+                             double* convMargin, double* zeroMargin) {
   double* v = (double*)malloc(sizeof(double) * n);
   double* z = (double*)malloc(sizeof(double) * n);
   int     done = 0;
@@ -53,9 +57,10 @@ int oracle_power_eigen(double* m, int n, int numEigs, const double* v0, double* 
     for (int i = 0; i < n; ++i) norm += v0[e * n + i] * v0[e * n + i];
     norm = sqrt(norm);
     for (int i = 0; i < n; ++i) v[i] = v0[e * n + i] / norm;
-    double eig = -1000.0;
-    int    converged = 0;
-    for (int it = 0; it < 1000; ++it) {
+    double eig = -1000.0, cm = INFINITY, zm = INFINITY;
+    int    converged = 0, it = 0;
+    while (it < 1000) {
+      ++it;
       const double prev = eig;
       for (int i = 0; i < n; ++i) {
         double a = 0.0;
@@ -65,13 +70,18 @@ int oracle_power_eigen(double* m, int n, int numEigs, const double* v0, double* 
       eig = z[0];
       for (int i = 1; i < n; ++i)
         if (fabs(z[i]) > fabs(eig)) eig = z[i];
+      zm = fmin(zm, fabs(fabs(eig) - 1.0e-10));
       if (fabs(eig) < 1.0e-10) break;
       for (int i = 0; i < n; ++i) v[i] = z[i] / eig;
+      cm = fmin(cm, fabs(fabs(eig - prev) - 0.001));
       if (fabs(eig - prev) < 0.001) {
         converged = 1;
         break;
       }
     }
+    if (iters) iters[e] = it;
+    if (convMargin) convMargin[e] = cm;
+    if (zeroMargin) zeroMargin[e] = zm;
     if (!converged) break;
     norm = 0.0;
     for (int i = 0; i < n; ++i) norm += v[i] * v[i];
@@ -88,6 +98,10 @@ int oracle_power_eigen(double* m, int n, int numEigs, const double* v0, double* 
   free(v);
   free(z);
   return done;
+}
+
+int oracle_power_eigen(double* m, int n, int numEigs, const double* v0, double* eigvals, double* eigvecs) {
+  return oracle_power_eigen_trace(m, n, numEigs, v0, eigvals, eigvecs, NULL, NULL, NULL);
 }
 
 /* dist[n*n] symmetric distances -> metric matrix T (n*n), RDKit computeInitialCoords. */
