@@ -179,6 +179,39 @@ int b200mol_similarity_threshold(const uint32_t* d_q, size_t nQ, const uint32_t*
                                  int metric, double threshold, int64_t* d_indptr /* [nQ + 1] */, int32_t* d_indices /* [cap] */,
                                  double* d_values /* [cap] */, uint64_t cap, uint64_t* h_nnz, void* stream);
 
+/* Tversky similarity, S[i][j] = c / ((alpha (a - c) + beta (b - c)) + c) with a = |A_i| (group one, the rows), b = |B_j|
+ * and c = |A_i & B_j|; 0 when c = 0 (two empty fingerprints included). Integer popcounts, then each product, sum and the
+ * quotient is one fp64 operation rounded to nearest, in exactly this order, never contracted into an FMA. alpha weights
+ * the bits only in the row fingerprint, as RDKit's TverskySimilarity(fp1, fp2, a, b) does, so the matrix of (one, two,
+ * alpha, beta) is the transpose of that of (two, one, beta, alpha). Dice, 2c / (a + b), is (0.5, 0.5); (1, 1) gives the
+ * bits of b200mol_tanimoto_cross. For dyadic weights (0, 1/4, 1/2, 1, 2, ...) the value is the same for any order of
+ * evaluation; for others, such as (0.3, 0.7), it may differ by a few ulp from an expanded form such as
+ * alpha a + beta b + (1 - alpha - beta) c. Values lie in [0, 1]; a non-empty fingerprint has 1.0 with itself.
+ * 0 <= alpha, beta <= 1000, finite (else B200MOL_ERR_INVALID). Each entry point takes the arguments of its Tanimoto /
+ * cosine twin, with (alpha, beta) after `words`, and has the twin's semantics for this value:
+ *   b200mol_tversky_cross       the (nA, nB) matrix, as b200mol_tanimoto_cross (d_b = NULL: A against itself)
+ *   b200mol_tversky_cross_host  host in / host out in row blocks, as b200mol_similarity_cross_host
+ *   b200mol_tversky_topk        exact top-k, as b200mol_similarity_topk: the first k columns of each row of the matrix by
+ *                               (value descending, column ascending). In a self search the self-match need not come first
+ *                               with alpha != beta: under (1, 0) every superset of the query also scores 1.0, and ties go
+ *                               to the lowest index.
+ *   b200mol_tversky_threshold   the CSR of the entries >= threshold, as b200mol_similarity_threshold; a self search with
+ *                               alpha != beta runs the full pass over the set against itself (the value is not symmetric)
+ * Dice (0.5, 0.5) runs on the Tanimoto machinery: the Dice epilogue of the matrix tiles, the Tanimoto top-k search (its
+ * order is Dice's order) with the values rewritten, and the thresholded graph pass with a Dice threshold table. Other
+ * weights take the cosine design: a float pre-filter on the tile that never drops a pair that could qualify, then an
+ * exact fp64 recount. */
+int b200mol_tversky_cross(const uint32_t* d_a, size_t nA, const uint32_t* d_b, size_t nB, int words, double alpha, double beta,
+                          double* d_out, void* stream);
+int b200mol_tversky_cross_host(const uint32_t* h_a, size_t nA, const uint32_t* h_b, size_t nB, int words, double alpha, double beta,
+                               double* h_out, size_t maxDeviceBytes);
+int b200mol_tversky_topk(const uint32_t* d_q, size_t nQ, const uint32_t* d_lib, size_t nLib, int words, double alpha, double beta,
+                         int k, double* d_values /* [nQ][k] */, int32_t* d_indices /* [nQ][k] */, void* stream);
+int b200mol_tversky_threshold(const uint32_t* d_q, size_t nQ, const uint32_t* d_lib /* NULL = self */, size_t nLib, int words,
+                              double alpha, double beta, double threshold, int64_t* d_indptr /* [nQ + 1] */,
+                              int32_t* d_indices /* [cap] */, double* d_values /* [cap] */, uint64_t cap, uint64_t* h_nnz,
+                              void* stream);
+
 /* MaxMin diversity picking (RDKit MaxMinPicker::LazyBitVectorPick / LazyBitVectorPickWithThreshold) over the pool
  * d_fp[0 .. nPool) ([nPool][words], 16-byte aligned). d(i, j) = 1 - s(i, j), s the fp64 value b200mol_tanimoto_cross /
  * b200mol_cosine_cross store for the pair (metric = B200MOL_METRIC_*), so two empty fingerprints are at distance 1.

@@ -38,6 +38,13 @@ SIGNATURES = {
     "b200mol_similarity_topk": (C.c_int, [_vp, C.c_size_t, _vp, C.c_size_t, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp]),
     "b200mol_similarity_threshold": (C.c_int, [_vp, C.c_size_t, _vp, C.c_size_t, C.c_int, C.c_int, C.c_double, _vp, _vp,
                                                _vp, C.c_uint64, C.POINTER(C.c_uint64), _vp]),
+    "b200mol_tversky_cross": (C.c_int, [_vp, C.c_size_t, _vp, C.c_size_t, C.c_int, C.c_double, C.c_double, _vp, _vp]),
+    "b200mol_tversky_cross_host": (C.c_int, [_vp, C.c_size_t, _vp, C.c_size_t, C.c_int, C.c_double, C.c_double, _vp,
+                                             C.c_size_t]),
+    "b200mol_tversky_topk": (C.c_int, [_vp, C.c_size_t, _vp, C.c_size_t, C.c_int, C.c_double, C.c_double, C.c_int, _vp,
+                                       _vp, _vp]),
+    "b200mol_tversky_threshold": (C.c_int, [_vp, C.c_size_t, _vp, C.c_size_t, C.c_int, C.c_double, C.c_double,
+                                            C.c_double, _vp, _vp, _vp, C.c_uint64, C.POINTER(C.c_uint64), _vp]),
     "b200mol_maxmin_pick": (C.c_int, [_vp, C.c_size_t, C.c_int, C.c_int, _vp, C.c_int, C.c_int, C.c_double, _vp, _vp,
                                       _vp]),
     "b200mol_leader_pick": (C.c_int, [_vp, C.c_size_t, C.c_int, C.c_int, C.c_double, _vp, C.c_int, C.c_int, _vp, _vp,

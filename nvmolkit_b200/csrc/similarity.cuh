@@ -14,6 +14,9 @@ enum SimMode : int {
   kCountCosine         = 3,
   kListCosine          = 4,  // edges only: every pair with sim >= cutoff, possibly with false positives (tensor tile:
                              // a float bound, unordered; the SIMT fallback runs kCountCosine and lists exactly)
+  kMaterialiseDice     = 5,  // fp64 Dice matrix, tversky(c, a, b; 1/2, 1/2)
+  kMaterialiseTversky  = 6,  // fp64 Tversky matrix for SimLaunch::tvAlpha / tvBeta
+  kListTversky         = 7,  // as kListCosine for Tversky (the SIMT fallback counts and lists exactly)
 };
 
 struct SimLaunch {
@@ -35,6 +38,11 @@ struct SimLaunch {
   int2*    edges       = nullptr;  // optional: neighbour pairs (i, j) appended here (symmetric: i < j)
   unsigned long long* edgeCursor = nullptr;  // device counter; entries beyond edgeCap are dropped (cursor still advances)
   unsigned long long  edgeCap    = 0;
+  // kCountTanimoto with atLeast: the table and the pre-filter of Dice, 2c / (|A| + |B|) >= cutoff, instead of Tanimoto's
+  bool   dice    = false;
+  // Tversky modes: the weights of the bits only in X (alpha) and only in Y (beta), 0 <= alpha, beta <= 1000
+  double tvAlpha = 0.0;
+  double tvBeta  = 0.0;
 };
 
 // Launch the tile kernel(s). Row popcounts and the threshold table are computed internally (stream-ordered scratch).
@@ -52,15 +60,53 @@ __device__ __forceinline__ double simFromCounts(int c, int a, int b, bool cosine
   return __ddiv_rn(static_cast<double>(c), static_cast<double>(a + b - c));
 }
 
+// The Tversky similarity of a pair with popcounts a (the group-one fingerprint), b and intersection c, as every Tversky
+// and Dice path stores it: 0 for an empty intersection, else c / ((alpha (a - c) + beta (b - c)) + c) with each product,
+// sum and the quotient one fp64 operation rounded to nearest, in that order (never contracted into an FMA). The
+// denominator is >= c > 0. Dice is (1/2, 1/2): its intermediates are exact, so it is RN(2c / (a + b)); (1, 1) is
+// Tanimoto's RN(c / (a + b - c)) bit for bit.
+__device__ __forceinline__ double tverskyFromCounts(int c, int a, int b, double alpha, double beta) {
+  if (c == 0) return 0.0;
+  return __ddiv_rn(static_cast<double>(c), __dadd_rn(__dadd_rn(__dmul_rn(alpha, static_cast<double>(a - c)),
+                                                                 __dmul_rn(beta, static_cast<double>(b - c))),
+                                                       static_cast<double>(c)));
+}
+
+// A float bound for the tile filters of the Tversky searches: can a pair with count c reach a value >= L, L a float
+// lower bound of the bar (or threshold) at least 1e-5 (relative) below it? Tested as c - L d >= 0 with
+// d = alpha_f (a - c) + (beta_f (b - c) + c) in float (fmaf), alpha_f, beta_f alpha and beta rounded to float.
+// Why no pair whose fp64 value v >= V (V >= L (1 + 1e-5)) is dropped: every term of the denominator is >= 0, so
+// rounding alpha and beta (2^-24 relative each) and the two fmaf (2^-24 each) give d <= D (1 + 2^-24)^3 < D (1 + 2e-7),
+// D the exact real denominator; the fp64 evaluation errs by at most 4 ulp, so v >= V means c >= V D (1 - 5e-16).
+// Then L d <= V D (1 - 1e-5 + 2e-7) < c. The final fmaf rounds once and keeps the sign of c - L d exactly. c and the
+// popcounts (<= 4096) are exact floats. c = 0 (value 0) never beats a bar (its column comes earlier) nor reaches t > 0.
+__device__ __forceinline__ bool tverskyMayReach(int c, int a, int b, float alphaF, float betaF, float L) {
+  const float cf = static_cast<float>(c);
+  const float d  = fmaf(alphaF, static_cast<float>(a - c), fmaf(betaF, static_cast<float>(b - c), cf));
+  return c != 0 && fmaf(-L, d, cf) >= 0.0f;
+}
+
+// Is (alpha, beta) Dice, or Tanimoto? Those two run on the Tanimoto machinery (integer ratio order, threshold table).
+inline bool tverskyIsDice(double alpha, double beta) { return alpha == 0.5 && beta == 0.5; }
+inline bool tverskyIsTanimoto(double alpha, double beta) { return alpha == 1.0 && beta == 1.0; }
+// The weights the Tversky entry points accept: finite, 0 <= alpha, beta <= 1000 (the range the float tile filters are
+// derived for). NaN fails the comparisons.
+inline void requireTverskyWeights(double alpha, double beta) {
+  B200_REQUIRE(alpha >= 0.0 && alpha <= 1000.0 && beta >= 0.0 && beta <= 1000.0,
+               "Tversky weights must be finite with 0 <= alpha, beta <= 1000 (got alpha = %g, beta = %g)", alpha, beta);
+}
+
 // ---- top-k search: what topk.cu uses of the tensor-core tile (tanimoto_tc.cu) ----
 // one u8 (0 / 1) per bit of n fingerprints
 void launchExpandBits(const uint32_t* fp, size_t n, int words, uint8_t* out, cudaStream_t s);
 bool topkTileEligible(int words);  // the tile takes widths that are multiples of 128 bits up to 4096
 // One pass of the expanded queries over an expanded column slab of the library (caller's indices colBase ..): for every
 // pair that could beat its row's bar[row] = {c, |A| + |B|, column, float bits of a lower bound of the value} of the row's
-// current k-th best, the caller's column index goes to cand[row][at], at = count[row]++, while at < cap.
-void launchTopkTile(bool cosine, const uint8_t* expQ, size_t nQ, const int32_t* popQ, const uint8_t* expLib, size_t nCols,
+// current k-th best, the caller's column index goes to cand[row][at], at = count[row]++, while at < cap. Tanimoto filters
+// with the integer ratio (.x, .y), cosine and Tversky (weights alpha, beta) with the float bound (.w).
+enum TopkMetric : int { kTopkTanimoto = 0, kTopkCosine = 1, kTopkTversky = 2 };
+void launchTopkTile(TopkMetric metric, const uint8_t* expQ, size_t nQ, const int32_t* popQ, const uint8_t* expLib, size_t nCols,
                     const int32_t* popCols, int words, const int4* bar, uint32_t* cand, uint32_t* count, uint32_t cap,
-                    uint32_t colBase, cudaStream_t s);
+                    uint32_t colBase, double alpha, double beta, cudaStream_t s);
 
 }  // namespace b200

@@ -49,6 +49,7 @@ struct TileParams {
   int2*           edges;
   unsigned long long* edgeCursor;
   unsigned long long  edgeCap;
+  double              tvAlpha, tvBeta;  // Tversky modes
 };
 
 __global__ void rowPopcountKernel(const uint32_t* __restrict__ fp, size_t n, int words, int32_t* __restrict__ pop) {
@@ -97,6 +98,25 @@ __global__ void threshTableKernel(int maxS, double cutoff, int atLeast, uint16_t
   thresh[s] = static_cast<uint16_t>(found);
 }
 
+// The Dice table of the threshold search: thresh[s] = the smallest c with the fp64 value tverskyFromCounts(c, a, b;
+// 1/2, 1/2) >= cutoff for |A| + |B| = s (that value is RN(2c / s), whatever a and b are), 0xFFFF = never. It grows with
+// c, and c <= min(a, b) <= s / 2: bisection over [1, s / 2] as threshTableKernel does.
+__global__ void diceTableKernel(int maxS, double cutoff, uint16_t* __restrict__ thresh) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s > maxS) return;
+  auto passes = [&](int c) { return tverskyFromCounts(c, c, s - c, 0.5, 0.5) >= cutoff; };
+  int  found = 0xFFFF, lo = 1, hi = s / 2;
+  if (hi >= lo && passes(hi)) {
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (passes(mid)) hi = mid;
+      else lo = mid + 1;
+    }
+    found = lo;
+  }
+  thresh[s] = static_cast<uint16_t>(found);
+}
+
 __device__ __forceinline__ uint4 lds128(uint32_t addr) {
   uint4 v;
   asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
@@ -109,6 +129,8 @@ __global__ void __launch_bounds__(kThreads, 2)
   extern __shared__ __align__(1024) uint8_t smemRaw[];
   __shared__ uint64_t                      fullBar[kStages];
   __shared__ int                           colAcc[kBN];
+  constexpr bool MATERIALISE = MODE == kMaterialiseTanimoto || MODE == kMaterialiseCosine || MODE == kMaterialiseDice ||
+                               MODE == kMaterialiseTversky;
 
   // ---- tile coordinates: groups of kGroupM tile-rows sweep all tile-columns (Y tiles reused out of L2) ----
   const uint32_t perGroup = kGroupM * p.tilesN;
@@ -137,7 +159,7 @@ __global__ void __launch_bounds__(kThreads, 2)
     for (int s = 0; s < kStages; ++s) mbarInit(&fullBar[s], 1);
     fenceBarrierInit();
   }
-  if (MODE >= kCountTanimoto && tid < kBN) colAcc[tid] = 0;
+  if (!MATERIALISE && tid < kBN) colAcc[tid] = 0;
   __syncthreads();
 
   uint8_t* smemGeneric = smemRaw + (smemBase - smemAddr(smemRaw));
@@ -195,7 +217,7 @@ __global__ void __launch_bounds__(kThreads, 2)
 #pragma unroll
   for (int j = 0; j < 8; ++j) pb[j] = (col0 + 16 * j < p.nY) ? __ldg(p.popY + col0 + 16 * j) : 0;
 
-  if constexpr (MODE == kMaterialiseTanimoto || MODE == kMaterialiseCosine) {
+  if constexpr (MATERIALISE) {
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       if (row0 + i >= p.nX) break;
@@ -209,6 +231,10 @@ __global__ void __launch_bounds__(kThreads, 2)
         if (c != 0) {
           if constexpr (MODE == kMaterialiseTanimoto) {
             v = __ddiv_rn(static_cast<double>(c), static_cast<double>(pa[i] + pb[j] - c));
+          } else if constexpr (MODE == kMaterialiseDice) {
+            v = tverskyFromCounts(c, pa[i], pb[j], 0.5, 0.5);
+          } else if constexpr (MODE == kMaterialiseTversky) {
+            v = tverskyFromCounts(c, pa[i], pb[j], p.tvAlpha, p.tvBeta);
           } else {
             v = __ddiv_rn(static_cast<double>(c),
                           __dsqrt_rn(__dmul_rn(static_cast<double>(pa[i]), static_cast<double>(pb[j]))));
@@ -231,6 +257,8 @@ __global__ void __launch_bounds__(kThreads, 2)
         bool      h;
         if constexpr (MODE == kCountTanimoto) {
           h = c >= static_cast<int>(__ldg(p.thresh + pa[i] + pb[j]));
+        } else if constexpr (MODE == kListTversky) {  // (the threshold search's exact list: atLeast)
+          h = tverskyFromCounts(c, pa[i], pb[j], p.tvAlpha, p.tvBeta) >= p.cutoff;
         } else {
           const double sim =
             (c == 0) ? 0.0
@@ -312,8 +340,12 @@ void launchTile(const CUtensorMap& tmX, const CUtensorMap& tmY, const TileParams
 
 bool launchSimilarityTensor(SimMode mode, const SimLaunch& q, cudaStream_t s);
 
-void launchThreshTable(int maxS, double cutoff, bool atLeast, uint16_t* thresh, cudaStream_t s) {
-  threshTableKernel<<<(maxS + 1 + 127) / 128, 128, 0, s>>>(maxS, cutoff, atLeast ? 1 : 0, thresh);
+void launchThreshTable(int maxS, double cutoff, bool atLeast, bool dice, uint16_t* thresh, cudaStream_t s) {
+  if (dice) {  // (a threshold search: atLeast)
+    diceTableKernel<<<(maxS + 1 + 127) / 128, 128, 0, s>>>(maxS, cutoff, thresh);
+  } else {
+    threshTableKernel<<<(maxS + 1 + 127) / 128, 128, 0, s>>>(maxS, cutoff, atLeast ? 1 : 0, thresh);
+  }
   B200_LAUNCHED();
 }
 
@@ -361,6 +393,8 @@ void launchSimilarity(SimMode mode, const SimLaunch& q, cudaStream_t s) {
   tp.edges      = q.edges;
   tp.edgeCursor = q.edgeCursor;
   tp.edgeCap    = q.edgeCap;
+  tp.tvAlpha    = q.tvAlpha;
+  tp.tvBeta     = q.tvBeta;
   if (q.symmetric) B200_REQUIRE(q.x == q.y && q.nX == q.nY, "symmetric mode needs x == y");
 
   CUtensorMap tmX, tmY;
@@ -379,8 +413,7 @@ void launchSimilarity(SimMode mode, const SimLaunch& q, cudaStream_t s) {
   if (mode == kCountTanimoto) {
     const int maxS = 2 * q.words * 32;
     thresh         = Scratch<uint16_t>(maxS + 1, s);
-    threshTableKernel<<<(maxS + 1 + 127) / 128, 128, 0, s>>>(maxS, q.cutoff, q.atLeast ? 1 : 0, thresh.get());
-    B200_LAUNCHED();
+    launchThreshTable(maxS, q.cutoff, q.atLeast, q.dice, thresh.get(), s);
     tp.thresh = thresh.get();
   }
 
@@ -392,6 +425,9 @@ void launchSimilarity(SimMode mode, const SimLaunch& q, cudaStream_t s) {
     case kCountTanimoto: launchTile<kCountTanimoto>(tmX, tmY, tp, smemBytes, s); break;
     case kCountCosine:
     case kListCosine: launchTile<kCountCosine>(tmX, tmY, tp, smemBytes, s); break;  // (exact: lists no false positive)
+    case kMaterialiseDice: launchTile<kMaterialiseDice>(tmX, tmY, tp, smemBytes, s); break;
+    case kMaterialiseTversky: launchTile<kMaterialiseTversky>(tmX, tmY, tp, smemBytes, s); break;
+    case kListTversky: launchTile<kListTversky>(tmX, tmY, tp, smemBytes, s); break;  // (exact, as cosine's)
   }
 }
 
@@ -453,8 +489,9 @@ extern "C" int b200mol_free_async(void* d_ptr, void* stream) {
 }
 
 static int crossImpl(SimMode mode, const uint32_t* d_a, size_t nA, const uint32_t* d_b, size_t nB, int words,
-                     double* d_out, void* stream) {
+                     double* d_out, void* stream, double alpha = 0.0, double beta = 0.0) {
   return guarded([&] {
+    if (mode == kMaterialiseTversky) requireTverskyWeights(alpha, beta);
     B200_REQUIRE(nA == 0 || d_a, "null fingerprint pointer");
     if (!d_b) {
       d_b = d_a;
@@ -468,8 +505,16 @@ static int crossImpl(SimMode mode, const uint32_t* d_a, size_t nA, const uint32_
     q.nY    = nB;
     q.words = words;
     q.out   = d_out;
+    q.tvAlpha = alpha;
+    q.tvBeta  = beta;
     launchSimilarity(mode, q, asStream(stream));
   });
+}
+
+// Tversky / Dice: (1/2, 1/2) is the Dice epilogue of the Tanimoto tiles, (1, 1) Tanimoto itself (the same bits as the
+// general expression in both cases), anything else the general Tversky epilogue
+static SimMode tverskyMaterialiseMode(double alpha, double beta) {
+  return tverskyIsDice(alpha, beta) ? kMaterialiseDice : tverskyIsTanimoto(alpha, beta) ? kMaterialiseTanimoto : kMaterialiseTversky;
 }
 
 extern "C" int b200mol_tanimoto_cross(const uint32_t* d_a, size_t nA, const uint32_t* d_b, size_t nB, int words,
@@ -479,6 +524,10 @@ extern "C" int b200mol_tanimoto_cross(const uint32_t* d_a, size_t nA, const uint
 extern "C" int b200mol_cosine_cross(const uint32_t* d_a, size_t nA, const uint32_t* d_b, size_t nB, int words,
                                     double* d_out, void* stream) {
   return crossImpl(kMaterialiseCosine, d_a, nA, d_b, nB, words, d_out, stream);
+}
+extern "C" int b200mol_tversky_cross(const uint32_t* d_a, size_t nA, const uint32_t* d_b, size_t nB, int words, double alpha,
+                                     double beta, double* d_out, void* stream) {
+  return crossImpl(tverskyMaterialiseMode(alpha, beta), d_a, nA, d_b, nB, words, d_out, stream, alpha, beta);
 }
 
 extern "C" int b200mol_tanimoto_count_ge(const uint32_t* d_x, size_t nX, const uint32_t* d_y, size_t nY, int words,
@@ -505,63 +554,53 @@ extern "C" int b200mol_tanimoto_count_ge(const uint32_t* d_x, size_t nX, const u
 }
 
 // Host-in / host-out: row blocks of A through two device buffers, D2H of block k overlapped with compute of block k+1.
-extern "C" int b200mol_similarity_cross_host(const uint32_t* h_a, size_t nA, const uint32_t* h_b, size_t nB, int words,
-                                             int metric, double* h_out, size_t maxDeviceBytes) {
-  return guarded([&] {
-    B200_REQUIRE(metric == B200MOL_METRIC_TANIMOTO || metric == B200MOL_METRIC_COSINE, "unknown metric %d", metric);
-    if (!h_b) {
-      h_b = h_a;
-      nB  = nA;
+static void crossHost(SimMode mode, double alpha, double beta, const uint32_t* h_a, size_t nA, const uint32_t* h_b, size_t nB,
+                      int words, double* h_out, size_t maxDeviceBytes) {
+  if (!h_b) {
+    h_b = h_a;
+    nB  = nA;
+  }
+  if (nA == 0 || nB == 0) return;
+  B200_REQUIRE(h_a && h_out, "null pointer");
+  if (maxDeviceBytes == 0) maxDeviceBytes = size_t(8) << 30;
+  size_t rowsPer = maxDeviceBytes / 2 / (nB * sizeof(double));
+  rowsPer        = rowsPer / kBM * kBM;
+  if (rowsPer < static_cast<size_t>(kBM)) rowsPer = kBM;
+  if (rowsPer > nA) rowsPer = nA;
+  cudaStream_t st[2];
+  cudaEvent_t  done[2];
+  for (int i = 0; i < 2; ++i) {
+    B200_CUDA(cudaStreamCreateWithFlags(&st[i], cudaStreamNonBlocking));
+    B200_CUDA(cudaEventCreateWithFlags(&done[i], cudaEventDisableTiming));
+  }
+  uint32_t *dA = nullptr, *dB = nullptr;
+  double*   dOut[2] = {nullptr, nullptr};
+  try {
+    B200_CUDA(cudaMalloc(reinterpret_cast<void**>(&dA), nA * words * sizeof(uint32_t)));
+    B200_CUDA(cudaMalloc(reinterpret_cast<void**>(&dB), nB * words * sizeof(uint32_t)));
+    for (int i = 0; i < 2; ++i) B200_CUDA(cudaMalloc(reinterpret_cast<void**>(&dOut[i]), rowsPer * nB * sizeof(double)));
+    B200_CUDA(cudaMemcpyAsync(dA, h_a, nA * words * sizeof(uint32_t), cudaMemcpyHostToDevice, st[0]));
+    B200_CUDA(cudaMemcpyAsync(dB, h_b, nB * words * sizeof(uint32_t), cudaMemcpyHostToDevice, st[0]));
+    B200_CUDA(cudaEventRecord(done[0], st[0]));
+    B200_CUDA(cudaStreamWaitEvent(st[1], done[0], 0));
+    int buf = 0;
+    for (size_t r0 = 0; r0 < nA; r0 += rowsPer, buf ^= 1) {
+      const size_t rows = (nA - r0 < rowsPer) ? nA - r0 : rowsPer;
+      SimLaunch    q;
+      q.x     = dA + r0 * words;
+      q.y     = dB;
+      q.nX    = rows;
+      q.nY    = nB;
+      q.words = words;
+      q.out   = dOut[buf];
+      q.tvAlpha = alpha;
+      q.tvBeta  = beta;
+      launchSimilarity(mode, q, st[buf]);
+      B200_CUDA(cudaMemcpyAsync(h_out + r0 * nB, dOut[buf], rows * nB * sizeof(double), cudaMemcpyDeviceToHost, st[buf]));
     }
-    if (nA == 0 || nB == 0) return;
-    B200_REQUIRE(h_a && h_out, "null pointer");
-    if (maxDeviceBytes == 0) maxDeviceBytes = size_t(8) << 30;
-    size_t rowsPer = maxDeviceBytes / 2 / (nB * sizeof(double));
-    rowsPer        = rowsPer / kBM * kBM;
-    if (rowsPer < static_cast<size_t>(kBM)) rowsPer = kBM;
-    if (rowsPer > nA) rowsPer = nA;
-    cudaStream_t st[2];
-    cudaEvent_t  done[2];
-    for (int i = 0; i < 2; ++i) {
-      B200_CUDA(cudaStreamCreateWithFlags(&st[i], cudaStreamNonBlocking));
-      B200_CUDA(cudaEventCreateWithFlags(&done[i], cudaEventDisableTiming));
-    }
-    uint32_t *dA = nullptr, *dB = nullptr;
-    double*   dOut[2] = {nullptr, nullptr};
-    try {
-      B200_CUDA(cudaMalloc(reinterpret_cast<void**>(&dA), nA * words * sizeof(uint32_t)));
-      B200_CUDA(cudaMalloc(reinterpret_cast<void**>(&dB), nB * words * sizeof(uint32_t)));
-      for (int i = 0; i < 2; ++i) B200_CUDA(cudaMalloc(reinterpret_cast<void**>(&dOut[i]), rowsPer * nB * sizeof(double)));
-      B200_CUDA(cudaMemcpyAsync(dA, h_a, nA * words * sizeof(uint32_t), cudaMemcpyHostToDevice, st[0]));
-      B200_CUDA(cudaMemcpyAsync(dB, h_b, nB * words * sizeof(uint32_t), cudaMemcpyHostToDevice, st[0]));
-      B200_CUDA(cudaEventRecord(done[0], st[0]));
-      B200_CUDA(cudaStreamWaitEvent(st[1], done[0], 0));
-      int buf = 0;
-      for (size_t r0 = 0; r0 < nA; r0 += rowsPer, buf ^= 1) {
-        const size_t rows = (nA - r0 < rowsPer) ? nA - r0 : rowsPer;
-        SimLaunch    q;
-        q.x     = dA + r0 * words;
-        q.y     = dB;
-        q.nX    = rows;
-        q.nY    = nB;
-        q.words = words;
-        q.out   = dOut[buf];
-        launchSimilarity(metric == B200MOL_METRIC_TANIMOTO ? kMaterialiseTanimoto : kMaterialiseCosine, q, st[buf]);
-        B200_CUDA(cudaMemcpyAsync(h_out + r0 * nB, dOut[buf], rows * nB * sizeof(double), cudaMemcpyDeviceToHost, st[buf]));
-      }
-      B200_CUDA(cudaStreamSynchronize(st[0]));
-      B200_CUDA(cudaStreamSynchronize(st[1]));
-    } catch (...) {
-      cudaFree(dA);
-      cudaFree(dB);
-      cudaFree(dOut[0]);
-      cudaFree(dOut[1]);
-      for (int i = 0; i < 2; ++i) {
-        cudaStreamDestroy(st[i]);
-        cudaEventDestroy(done[i]);
-      }
-      throw;
-    }
+    B200_CUDA(cudaStreamSynchronize(st[0]));
+    B200_CUDA(cudaStreamSynchronize(st[1]));
+  } catch (...) {
     cudaFree(dA);
     cudaFree(dB);
     cudaFree(dOut[0]);
@@ -570,5 +609,31 @@ extern "C" int b200mol_similarity_cross_host(const uint32_t* h_a, size_t nA, con
       cudaStreamDestroy(st[i]);
       cudaEventDestroy(done[i]);
     }
+    throw;
+  }
+  cudaFree(dA);
+  cudaFree(dB);
+  cudaFree(dOut[0]);
+  cudaFree(dOut[1]);
+  for (int i = 0; i < 2; ++i) {
+    cudaStreamDestroy(st[i]);
+    cudaEventDestroy(done[i]);
+  }
+}
+
+extern "C" int b200mol_similarity_cross_host(const uint32_t* h_a, size_t nA, const uint32_t* h_b, size_t nB, int words,
+                                             int metric, double* h_out, size_t maxDeviceBytes) {
+  return guarded([&] {
+    B200_REQUIRE(metric == B200MOL_METRIC_TANIMOTO || metric == B200MOL_METRIC_COSINE, "unknown metric %d", metric);
+    crossHost(metric == B200MOL_METRIC_TANIMOTO ? kMaterialiseTanimoto : kMaterialiseCosine, 0.0, 0.0, h_a, nA, h_b, nB, words, h_out,
+              maxDeviceBytes);
+  });
+}
+
+extern "C" int b200mol_tversky_cross_host(const uint32_t* h_a, size_t nA, const uint32_t* h_b, size_t nB, int words, double alpha,
+                                          double beta, double* h_out, size_t maxDeviceBytes) {
+  return guarded([&] {
+    requireTverskyWeights(alpha, beta);
+    crossHost(tverskyMaterialiseMode(alpha, beta), alpha, beta, h_a, nA, h_b, nB, words, h_out, maxDeviceBytes);
   });
 }

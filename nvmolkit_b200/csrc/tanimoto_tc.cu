@@ -98,6 +98,10 @@ struct TcParams {
   uint32_t*   topkCount;  // [n] slots asked for (may pass topkCap: the row is then redone, nothing of it is merged)
   uint32_t    topkCap;
   uint32_t    topkColBase;  // caller's index of the Y operand's first row (the library is searched in column slabs)
+  // Tversky modes: the weights in fp64 (the matrix) and rounded to float (the filters, tverskyMayReach), and the list
+  // mode's float lower bound of the threshold
+  double tvAlpha, tvBeta;
+  float  tvAlphaF, tvBetaF, tvBound;
 };
 
 // The popcount band. A pair with popcounts a, b and intersection c <= min(a, b) can only be a neighbour if
@@ -108,7 +112,10 @@ struct TcParams {
 // row group whose largest popcount is A, no column past the first one this cuts can be a neighbour of any of its rows.
 __host__ __device__ __forceinline__ bool bandCuts(const uint16_t* tmin, int A, int b) { return tmin[A + b] > A; }
 
-enum TcMode : int { kTcCount = 0, kTcTanimoto = 1, kTcCosine = 2, kTcTopkTanimoto = 3, kTcTopkCosine = 4, kTcListCosine = 5 };
+enum TcMode : int {
+  kTcCount = 0, kTcTanimoto = 1, kTcCosine = 2, kTcTopkTanimoto = 3, kTcTopkCosine = 4, kTcListCosine = 5,
+  kTcDice = 6, kTcTversky = 7, kTcTopkTversky = 8, kTcListTversky = 9
+};
 }  // namespace
 int g_tensorCluster = 1;  // count tile in clusters of two CTAs with a multicast column operand (option "similarity_tensor_cluster":
                           // 0 one CTA per tile, 1 the pair, 2 the pair too (kept for callers written for the CTA-pair MMA
@@ -412,6 +419,13 @@ __device__ __forceinline__ int4 ldsFresh(const int4* p) {
   return v;
 }
 
+// An accumulator the compiler may not share between the Tversky filters' two passes over the tile (the test and the
+// listing): kept, the float terms of 128 accumulators would spill
+__device__ __forceinline__ int fresh(int a) {
+  asm volatile("" : "+r"(a));
+  return a;
+}
+
 // The list of one epilogue warp of the count tile - candidates when superposed, else edges (if asked for): (row, column)
 // pairs are parked in kStagePairs shared-memory slots and leave with ONE global atomic per flush, when the slots are
 // full and at the end of the warp's work. The atomic's result (the store address) is waited on once per flush instead
@@ -576,8 +590,9 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
   extern __shared__ __align__(1024) uint8_t smemRaw[];
   static_assert(!CL || MODE == kTcCount, "the two-CTA cluster is wired for the count tile");
   constexpr bool COUNT = MODE == kTcCount;
-  constexpr bool TOPK  = MODE == kTcTopkTanimoto || MODE == kTcTopkCosine;
-  constexpr bool LIST  = MODE == kTcListCosine;  // edges only, through the same per-warp staging as the count mode
+  constexpr bool TOPK  = MODE == kTcTopkTanimoto || MODE == kTcTopkCosine || MODE == kTcTopkTversky;
+  constexpr bool LIST  = MODE == kTcListCosine || MODE == kTcListTversky;  // edges only, through the same per-warp staging
+                                                                         // as the count mode
   constexpr bool ST    = CL == 3;  // row operand stationary
   using Walk           = UnitWalk<CL != 0, ST ? kRunStat : 1>;
   constexpr int  kStg       = ST ? kStagesStat : kStages;
@@ -842,7 +857,11 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
           // 2^-26, far above an ulp, so this integer order is the order of the fp64 values the select kernel compares.
           // Cosine, c / sqrt(|A| |B|), has no integer form: float(c) >= tauLow sqrt|A| sqrt|B| with tauLow a few 1e-5
           // (relative) below the bar, which covers the float roundings; ties and near ties survive.
+          // Tversky depends on c, |A| and |B| apart: tverskyMayReach (similarity.cuh) with the same float bar. For fixed
+          // |A| and |B| the value c / (K + (1 - alpha - beta) c), K = alpha |A| + beta |B|, has derivative K / D^2 >= 0 in c,
+          // so the exact select kernel orders by value alone, as for cosine.
           constexpr bool COS = MODE == kTcTopkCosine;
+          constexpr bool TV  = MODE == kTcTopkTversky;
           const bool in0 = r0 < p.n, in1 = r1 < p.n;
           // per row: margin(c, column) = c f - g term(column) must exceed t. Past the end nothing does.
           int   f0 = 0, g0 = 0, t0 = 0x7fffffff, f1 = 0, g1 = 0, t1 = 0x7fffffff;
@@ -850,17 +869,18 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
           if (in0) {
             const int4 b = __ldg(p.topkBar + r0);
             f0 = b.y, g0 = b.x, t0 = b.x * pa0;
-            rt0 = __int_as_float(b.w) * sqrtf(static_cast<float>(pa0));
+            rt0 = TV ? __int_as_float(b.w) : __int_as_float(b.w) * sqrtf(static_cast<float>(pa0));
           }
           if (in1) {
             const int4 b = __ldg(p.topkBar + r1);
             f1 = b.y, g1 = b.x, t1 = b.x * pa1;
-            rt1 = __int_as_float(b.w) * sqrtf(static_cast<float>(pa1));
+            rt1 = TV ? __int_as_float(b.w) : __int_as_float(b.w) * sqrtf(static_cast<float>(pa1));
           }
           // does accumulator e of a column block (popcount pb, sqrt(pb) as float bits sq) pass? (cosine: the count through
           // the 2^23 trick, exact and no I2F)
           auto pass = [&](int e, int a, int pb, int sq) {
             if constexpr (COS) return fmaf(-(e < 2 ? rt0 : rt1), __int_as_float(sq), __int_as_float(0x4b000000 | a) - 8388608.0f) >= 0.0f;
+            else if constexpr (TV) return tverskyMayReach(fresh(a), e < 2 ? pa0 : pa1, pb, p.tvAlphaF, p.tvBetaF, e < 2 ? rt0 : rt1);
             else return a * (e < 2 ? f0 : f1) - (e < 2 ? g0 : g1) * pb > (e < 2 ? t0 : t1);
           };
           bool any = false;
@@ -899,16 +919,20 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
           // square roots and products can err by, so every pair whose fp64 value is >= t is listed; the assembly re-counts
           // each listed pair and drops the near misses. rowMeta .y = float bits of tLow sqrt|A|, colMeta .y = those of
           // sqrt|B| (3e38 past the end). An empty intersection never reaches t > 0.
+          // Tversky: tverskyMayReach (similarity.cuh) against p.tvBound = t (1 - 1e-5) rounded down; .x the popcounts.
           const float rt0 = __int_as_float(ra0.y), rt1 = __int_as_float(ra1.y);
-          auto pass = [&](int e, int a, int sq) {  // (the count through the 2^23 trick, exact and no I2F)
-            return a != 0 && fmaf(-(e < 2 ? rt0 : rt1), __int_as_float(sq), __int_as_float(0x4b000000 | a) - 8388608.0f) >= 0.0f;
+          auto pass = [&](int e, int a, int4 ci) {  // (cosine: the count through the 2^23 trick, exact and no I2F)
+            if constexpr (MODE == kTcListTversky)
+              return tverskyMayReach(fresh(a), e < 2 ? pa0 : pa1, (e & 1) ? ci.z : ci.x, p.tvAlphaF, p.tvBetaF, p.tvBound);
+            else
+              return a != 0 && fmaf(-(e < 2 ? rt0 : rt1), __int_as_float((e & 1) ? ci.w : ci.y), __int_as_float(0x4b000000 | a) - 8388608.0f) >= 0.0f;
           };
           bool any = false;
 #pragma unroll
           for (int j = 0; j < 32; ++j) {
             const int4 ci = cm[4 * j];
-            any |= pass(0, static_cast<int>(acc[4 * j]), ci.y) | pass(1, static_cast<int>(acc[4 * j + 1]), ci.w) |
-                   pass(2, static_cast<int>(acc[4 * j + 2]), ci.y) | pass(3, static_cast<int>(acc[4 * j + 3]), ci.w);
+            any |= pass(0, static_cast<int>(acc[4 * j]), ci) | pass(1, static_cast<int>(acc[4 * j + 1]), ci) |
+                   pass(2, static_cast<int>(acc[4 * j + 2]), ci) | pass(3, static_cast<int>(acc[4 * j + 3]), ci);
           }
           if (__any_sync(0xffffffffu, any)) {
             // survivors as bits 4 (j % 8) + e of sv[j / 8] in one unrolled pass, listed in a rolled loop over the column
@@ -920,7 +944,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
               uint32_t   nib = 0;
 #pragma unroll
               for (int e = 0; e < 4; ++e)
-                if (pass(e, static_cast<int>(acc[4 * j + e]), (e & 1) ? ci.w : ci.y)) nib |= 1u << e;
+                if (pass(e, static_cast<int>(acc[4 * j + e]), ci)) nib |= 1u << e;
               sv[j >> 3] |= nib << (4 * (j & 7));
               if (nib) blocks |= 1u << j;
             }
@@ -937,7 +961,8 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
             }
           }
         } else {
-          // fp64 Tanimoto / cosine straight from the accumulators: a quad of lanes writes 64 contiguous bytes of a row
+          // fp64 Tanimoto / cosine / Dice / Tversky straight from the accumulators: a quad of lanes writes 64 contiguous
+          // bytes of a row
 #pragma unroll
           for (int j = 0; j < 32; ++j) {
             const uint32_t c = c0 + 8 * j;
@@ -958,6 +983,16 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
                   const double du = __hiloint2double(0x43300000, u) - 4503599627370496.0;
                   const double rc = __ldg(p.recipG + u), q0 = __dmul_rn(dc, rc);
                   v[e]            = __fma_rn(__fma_rn(-q0, du, dc), rc, q0);
+                } else if constexpr (MODE == kTcDice) {
+                  // 2c / (a + b) = 2 RN(c / u), u = a + b: the same correctly rounded quotient (c <= u / 2 <= 4096), then
+                  // an exact doubling; equal to tverskyFromCounts(c, a, b; 1/2, 1/2), whose intermediates are exact
+                  const int    u  = pak + pb;
+                  const double dc = __hiloint2double(0x43300000, cnt) - 4503599627370496.0;
+                  const double du = __hiloint2double(0x43300000, u) - 4503599627370496.0;
+                  const double rc = __ldg(p.recipG + u), q0 = __dmul_rn(dc, rc);
+                  v[e]            = 2.0 * __fma_rn(__fma_rn(-q0, du, dc), rc, q0);
+                } else if constexpr (MODE == kTcTversky) {
+                  v[e] = tverskyFromCounts(cnt, pak, pb, p.tvAlpha, p.tvBeta);
                 } else {
                   v[e] = __ddiv_rn(static_cast<double>(cnt), __dsqrt_rn(__dmul_rn(static_cast<double>(pak), static_cast<double>(pb))));
                 }
@@ -1003,7 +1038,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
 }  // namespace
 
 void launchRowPopcount(const uint32_t* fp, size_t n, int words, int32_t* pop, cudaStream_t s);
-void launchThreshTable(int maxS, double cutoff, bool atLeast, uint16_t* thresh, cudaStream_t s);
+void launchThreshTable(int maxS, double cutoff, bool atLeast, bool dice, uint16_t* thresh, cudaStream_t s);
 
 // A fingerprint set in popcount order: row i of fp is the caller's row perm[i], pop its popcount; ascending, ties in the
 // caller's order (CUB's radix sort is stable), so the same input always gives the same order.
@@ -1191,9 +1226,10 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
   p.edgeCap   = q.edgeCap;
   p.out       = q.out;
   p.outVec    = (q.nY % 2 == 0 && (reinterpret_cast<uintptr_t>(q.out) & 15) == 0) ? 1 : 0;
-  const int recipLen = 2 * bits;
-  Scratch<double> recip(mode == kMaterialiseTanimoto ? static_cast<size_t>(recipLen) + 1 : 0, s);
-  if (mode == kMaterialiseTanimoto) {
+  const int  recipLen = 2 * bits;
+  const bool useRecip = mode == kMaterialiseTanimoto || mode == kMaterialiseDice;
+  Scratch<double> recip(useRecip ? static_cast<size_t>(recipLen) + 1 : 0, s);
+  if (useRecip) {
     recipTableKernel<<<(recipLen + 256) / 256, 256, 0, s>>>(recip.get(), recipLen);
     B200_LAUNCHED();
     p.recipG = recip.get();
@@ -1201,13 +1237,16 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
   {
     // a pair passes iff 1 - c / (|A| + |B| - c) <= cutoff, i.e. c >= alpha (|A| + |B|) - or, for the threshold search's
     // c / (|A| + |B| - c) >= t, with alpha = t / (1 + t); the pre-filter's alpha is rounded DOWN (and its products
-    // too), so it never rejects what the exact fp64 table accepts
-    const double a  = q.atLeast ? q.cutoff / (1.0 + q.cutoff) : q.cutoff < 2.0 ? (1.0 - q.cutoff) / (2.0 - q.cutoff) : 0.0;
+    // too), so it never rejects what the exact fp64 table accepts. Dice's 2c / (|A| + |B|) >= t needs c >= (t / 2) (|A| + |B|).
+    const double a  = q.atLeast ? (q.dice ? q.cutoff / 2.0 : q.cutoff / (1.0 + q.cutoff))
+                                : q.cutoff < 2.0 ? (1.0 - q.cutoff) / (2.0 - q.cutoff) : 0.0;
     float        af = static_cast<float>(a);
     if (static_cast<double>(af) > a) af = nextafterf(af, -1.0f);
     p.alpha = nextafterf(af, -1.0f);  // (one more ulp: fp64 rounding inside the table's predicate)
     if (p.alpha < 0.0f) p.alpha = 0.0f;
   }
+  p.tvAlpha = q.tvAlpha, p.tvBeta = q.tvBeta;
+  p.tvAlphaF = static_cast<float>(q.tvAlpha), p.tvBetaF = static_cast<float>(q.tvBeta);
 
   Scratch<int32_t> popX(q.nX, s), popYown(same ? 0 : q.nY, s);
   launchRowPopcount(q.x, q.nX, q.words, popX.get(), s);
@@ -1259,10 +1298,11 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
   // tile of a CTA pair may lie one tile row past the end)
   const size_t  rowsPad = (static_cast<size_t>(p.tilesM) + 1) * kTM, colsPad = static_cast<size_t>(p.tilesN) * kTN;
   Scratch<int2> rowMeta(rowsPad, s), colMeta(colsPad, s);
-  if (mode == kListCosine) {
+  if (mode == kListCosine || mode == kListTversky) {
     // the list tile's bound: tLow = t (1 - 1e-5), rounded down
     float tLow = static_cast<float>(q.cutoff * (1.0 - 1e-5));
     if (static_cast<double>(tLow) > q.cutoff * (1.0 - 1e-5)) tLow = nextafterf(tLow, 0.0f);
+    p.tvBound = tLow;
     listMetaKernel<<<static_cast<unsigned>((rowsPad + 255) / 256), 256, 0, s>>>(popXs, q.nX, rowsPad, tLow, rowMeta.get());
     B200_LAUNCHED();
     listMetaKernel<<<static_cast<unsigned>((colsPad + 255) / 256), 256, 0, s>>>(popYs, q.nY, colsPad, 1.0f, colMeta.get());
@@ -1293,7 +1333,7 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
   const int         maxS = 2 * bits;
   Scratch<uint16_t> thresh(static_cast<size_t>(maxS + 1), s);
   if (mode == kCountTanimoto) {
-    launchThreshTable(maxS, q.cutoff, q.atLeast, thresh.get(), s);
+    launchThreshTable(maxS, q.cutoff, q.atLeast, q.dice, thresh.get(), s);
     p.threshLen = maxS + 1;
   }
   p.thresh = thresh.get();
@@ -1335,6 +1375,9 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
     optIn(simTensorKernel<kTcTanimoto, 0>);
     optIn(simTensorKernel<kTcCosine, 0>);
     optIn(simTensorKernel<kTcListCosine, 0>);
+    optIn(simTensorKernel<kTcDice, 0>);
+    optIn(simTensorKernel<kTcTversky, 0>);
+    optIn(simTensorKernel<kTcListTversky, 0>);
     configured[currentDeviceSlot()] = true;
   }
   // units a call owns: tiles, or vertical tile pairs (same enumeration as the kernel's UnitWalk)
@@ -1457,6 +1500,15 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
   } else if (mode == kListCosine) {
     PhaseTimer t("threshold_list_tc", s);
     simTensorKernel<kTcListCosine, 0><<<blocks, kThreadsTC, smemBytes, s>>>(tmA, tmB, p);
+  } else if (mode == kListTversky) {
+    PhaseTimer t("threshold_list_tc", s);
+    simTensorKernel<kTcListTversky, 0><<<blocks, kThreadsTC, smemBytes, s>>>(tmA, tmB, p);
+  } else if (mode == kMaterialiseDice) {
+    PhaseTimer t("cross_tc", s);
+    simTensorKernel<kTcDice, 0><<<blocks, kThreadsTC, smemBytes, s>>>(tmA, tmB, p);
+  } else if (mode == kMaterialiseTversky) {
+    PhaseTimer t("cross_tc", s);
+    simTensorKernel<kTcTversky, 0><<<blocks, kThreadsTC, smemBytes, s>>>(tmA, tmB, p);
   } else if (mode == kMaterialiseTanimoto) {
     PhaseTimer t("cross_tc", s);
     simTensorKernel<kTcTanimoto, 0><<<blocks, kThreadsTC, smemBytes, s>>>(tmA, tmB, p);
@@ -1506,9 +1558,10 @@ void launchExpandBits(const uint32_t* fp, size_t n, int words, uint8_t* out, cud
 
 bool topkTileEligible(int words) { return (words * 32) % kTK == 0 && words * 32 <= 4096; }
 
-void launchTopkTile(bool cosine, const uint8_t* expQ, size_t nQ, const int32_t* popQ, const uint8_t* expLib, size_t nCols,
+void launchTopkTile(TopkMetric metric, const uint8_t* expQ, size_t nQ, const int32_t* popQ, const uint8_t* expLib, size_t nCols,
                     const int32_t* popCols, int words, const int4* bar, uint32_t* cand, uint32_t* count, uint32_t cap,
-                    uint32_t colBase, cudaStream_t s) {
+                    uint32_t colBase, double alpha, double beta, cudaStream_t s) {
+  const bool cosine = metric == kTopkCosine;
   const int rowBytes = words * 32;
   TcParams  p{};
   p.n           = static_cast<uint32_t>(nQ);
@@ -1526,6 +1579,8 @@ void launchTopkTile(bool cosine, const uint8_t* expQ, size_t nQ, const int32_t* 
   p.topkCount   = count;
   p.topkCap     = cap;
   p.topkColBase = colBase;
+  p.tvAlphaF    = static_cast<float>(alpha);
+  p.tvBetaF     = static_cast<float>(beta);
   const size_t  rowsPad = static_cast<size_t>(p.tilesM) * kTM, colsPad = static_cast<size_t>(p.tilesN) * kTN;
   Scratch<int2> rowMeta(rowsPad, s), colMeta(colsPad, s);
   topkMetaKernel<<<static_cast<unsigned>((rowsPad + 255) / 256), 256, 0, s>>>(popQ, nQ, rowsPad, 0, rowMeta.get());
@@ -1542,12 +1597,14 @@ void launchTopkTile(bool cosine, const uint8_t* expQ, size_t nQ, const int32_t* 
   if (!configured[currentDeviceSlot()]) {
     B200_CUDA(cudaFuncSetAttribute(simTensorKernel<kTcTopkTanimoto, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smemBytes)));
     B200_CUDA(cudaFuncSetAttribute(simTensorKernel<kTcTopkCosine, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smemBytes)));
+    B200_CUDA(cudaFuncSetAttribute(simTensorKernel<kTcTopkTversky, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smemBytes)));
     configured[currentDeviceSlot()] = true;
   }
   const uint64_t units = countUnits<false>(p, nullptr);
   if (units == 0) return;
   const int grid = static_cast<int>(std::min<uint64_t>(static_cast<uint64_t>(smCount()), units));
   if (cosine) simTensorKernel<kTcTopkCosine, 0><<<grid, kThreadsTC, smemBytes, s>>>(tmA, tmB, p);
+  else if (metric == kTopkTversky) simTensorKernel<kTcTopkTversky, 0><<<grid, kThreadsTC, smemBytes, s>>>(tmA, tmB, p);
   else simTensorKernel<kTcTopkTanimoto, 0><<<grid, kThreadsTC, smemBytes, s>>>(tmA, tmB, p);
   B200_LAUNCHED();
 }

@@ -11,7 +11,10 @@
 //             pairs whose integer threshold-table test passes - the fp64 predicate s >= t, bit for bit.
 //             Cosine: the list mode kListCosine - on the wgmma tile every pair that passes a float bound with a margin
 //             (a superset of the answer, unordered); on the SIMT tile the exact fp64 test.
-//             Both run on SIMT or on the tensor cores as "similarity_tensor_min_pairs" decides.
+//             Dice (b200mol_tversky_threshold at (1/2, 1/2)): Tanimoto's graph pass with the Dice table and pre-filter.
+//             Tversky: the list mode kListTversky, a float bound like cosine's. With alpha != beta the value is not
+//             symmetric, so a self search runs the full (non-symmetric) pass over the set against itself.
+//             All run on SIMT or on the tensor cores as "similarity_tensor_min_pairs" decides.
 //   read      the listed-pair total, the pairs the re-count keeps and the non-empty queries: the one host read of an attempt.
 //             A list longer than its buffer is rerun once into a buffer of the exact size.
 //   assembly  (a) every listed pair is re-counted by popcount and its value computed with simFromCounts (the matrix's
@@ -35,11 +38,13 @@ constexpr int kRecountLanes = 8;  // lanes per listed pair in the re-count (up t
 
 // stat[0] listed pairs (the pass's edge cursor), [1] pairs the re-count keeps, [2] non-empty queries, [3] fill cursor
 
-// (a): one group of kRecountLanes lanes per listed pair (i, j) in the caller's indices; a dropped pair gets i = -1
+// (a): one group of kRecountLanes lanes per listed pair (i, j) in the caller's indices; a dropped pair gets i = -1.
+// TV: the value is tverskyFromCounts(alpha, beta) (Dice too), else Tanimoto / cosine.
+template <bool TV>
 __global__ void __launch_bounds__(256) recountKernel(const uint32_t* __restrict__ x, const uint32_t* __restrict__ y, int words,
                                                      const int32_t* __restrict__ popX, const int32_t* __restrict__ popY, int cosine,
-                                                     double t, int2* list, unsigned long long cap, double* __restrict__ vals,
-                                                     unsigned long long* stat) {
+                                                     double alpha, double beta, double t, int2* list, unsigned long long cap,
+                                                     double* __restrict__ vals, unsigned long long* stat) {
   const unsigned long long n = min(stat[0], cap);
   const int                lane = threadIdx.x & 31, gl = lane % kRecountLanes, chunks = words / 4;
   const unsigned long long step = static_cast<unsigned long long>(gridDim.x) * blockDim.x / kRecountLanes;
@@ -62,7 +67,7 @@ __global__ void __launch_bounds__(256) recountKernel(const uint32_t* __restrict_
     for (int o = kRecountLanes / 2; o; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
     bool keep = false;
     if (have && gl == 0) {
-      const double v = simFromCounts(c, popX[ij.x], popY[ij.y], cosine != 0);
+      const double v = TV ? tverskyFromCounts(c, popX[ij.x], popY[ij.y], alpha, beta) : simFromCounts(c, popX[ij.x], popY[ij.y], cosine != 0);
       keep           = v >= t;
       vals[e]        = v;
       if (!keep) list[e].x = -1;
@@ -155,8 +160,12 @@ unsigned blocksFor(unsigned long long items, int perBlock) {
                                                                                             static_cast<unsigned long long>(smCount()) * 16)));
 }
 
-void thresholdSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t nLib, bool self, int words, bool cosine, double t,
-                     int64_t* indptr, int32_t* indices, double* values, uint64_t cap, uint64_t* hNnz, cudaStream_t s) {
+enum Measure : int { kTanimoto, kCosine, kDice, kTversky };
+
+void thresholdSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t nLib, bool self, int words, Measure measure,
+                     double alpha, double beta, double t, int64_t* indptr, int32_t* indices, double* values, uint64_t cap,
+                     uint64_t* hNnz, cudaStream_t s) {
+  const bool cosine = measure == kCosine, tv = measure == kDice || measure == kTversky;
   Scratch<int32_t> popQ(nQ, s), popLibOwn(self ? 0 : nLib, s), counts(nQ, s);
   launchRowPopcount(q, nQ, words, popQ.get(), s);
   if (!self) launchRowPopcount(lib, nLib, words, popLibOwn.get(), s);
@@ -192,13 +201,22 @@ void thresholdSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t n
       p.edges     = list.get();
       p.edgeCursor = stat.get();
       p.edgeCap   = listCap;
+      p.dice      = measure == kDice;
+      p.tvAlpha   = alpha;
+      p.tvBeta    = beta;
       B200_CUDA(cudaMemsetAsync(counts.get(), 0, nQ * sizeof(int32_t), s));
-      launchSimilarity(cosine ? kListCosine : kCountTanimoto, p, s);
+      launchSimilarity(cosine ? kListCosine : measure == kTversky ? kListTversky : kCountTanimoto, p, s);
     }
     {
       PhaseTimer timer("threshold_recount", s);
-      recountKernel<<<blocksFor(listCap * kRecountLanes, 256), 256, 0, s>>>(q, lib, words, popQ.get(), popLib, cosine ? 1 : 0, t,
-                                                                           list.get(), listCap, vals.get(), stat.get());
+      const unsigned blocks = blocksFor(listCap * kRecountLanes, 256);
+      if (tv) {
+        recountKernel<true><<<blocks, 256, 0, s>>>(q, lib, words, popQ.get(), popLib, 0, alpha, beta, t, list.get(), listCap, vals.get(),
+                                                   stat.get());
+      } else {
+        recountKernel<false><<<blocks, 256, 0, s>>>(q, lib, words, popQ.get(), popLib, cosine ? 1 : 0, 0.0, 0.0, t, list.get(), listCap,
+                                                    vals.get(), stat.get());
+      }
       B200_LAUNCHED();
       if (self) {
         nonEmptyKernel<<<static_cast<unsigned>((nQ + 255) / 256), 256, 0, s>>>(popQ.get(), nQ, stat.get());
@@ -243,29 +261,49 @@ void thresholdSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t n
 
 using namespace b200;
 
+static void thresholdEntry(const uint32_t* d_q, size_t nQ, const uint32_t* d_lib, size_t nLib, int words, Measure measure, double alpha,
+                           double beta, double threshold, int64_t* d_indptr, int32_t* d_indices, double* d_values, uint64_t cap,
+                           uint64_t* h_nnz, void* stream) {
+  B200_REQUIRE(words > 0 && words % 4 == 0 && words <= 128,
+               "fingerprint width must be a multiple of 128 bits and at most 4096 bits (got %d words)", words);
+  B200_REQUIRE(threshold > 0.0 && threshold <= 1.0, "threshold must be in (0, 1] (got %g)", threshold);
+  const bool self = d_lib == nullptr;
+  if (self) nLib = nQ;
+  B200_REQUIRE(nQ < (1ull << 31) && nLib < (1ull << 31), "too many fingerprints");
+  B200_REQUIRE(h_nnz && d_indptr, "null pointer");
+  B200_REQUIRE(nQ == 0 || d_q, "null fingerprint pointer");
+  B200_REQUIRE(cap == 0 || (d_indices && d_values), "null output pointer");
+  B200_REQUIRE((reinterpret_cast<uintptr_t>(d_q) & 15) == 0 && (reinterpret_cast<uintptr_t>(d_lib) & 15) == 0,
+               "fingerprint buffers must be 16-byte aligned");
+  const cudaStream_t s = asStream(stream);
+  *h_nnz               = 0;
+  if (nQ == 0 || nLib == 0) {  // no pair: every row is empty
+    B200_CUDA(cudaMemsetAsync(d_indptr, 0, (nQ + 1) * sizeof(int64_t), s));
+    return;
+  }
+  // an asymmetric measure has no symmetric pass: the set is searched against itself as a library, every pair in full
+  const bool symmetricPass = self && !(measure == kTversky && alpha != beta);
+  thresholdSearch(d_q, nQ, self ? d_q : d_lib, nLib, symmetricPass, words, measure, alpha, beta, threshold, d_indptr, d_indices,
+                  d_values, cap, h_nnz, s);
+}
+
 extern "C" int b200mol_similarity_threshold(const uint32_t* d_q, size_t nQ, const uint32_t* d_lib, size_t nLib, int words, int metric,
                                             double threshold, int64_t* d_indptr, int32_t* d_indices, double* d_values, uint64_t cap,
                                             uint64_t* h_nnz, void* stream) {
   return guarded([&] {
     B200_REQUIRE(metric == B200MOL_METRIC_TANIMOTO || metric == B200MOL_METRIC_COSINE, "unknown metric %d", metric);
-    B200_REQUIRE(words > 0 && words % 4 == 0 && words <= 128,
-                 "fingerprint width must be a multiple of 128 bits and at most 4096 bits (got %d words)", words);
-    B200_REQUIRE(threshold > 0.0 && threshold <= 1.0, "threshold must be in (0, 1] (got %g)", threshold);
-    const bool self = d_lib == nullptr;
-    if (self) nLib = nQ;
-    B200_REQUIRE(nQ < (1ull << 31) && nLib < (1ull << 31), "too many fingerprints");
-    B200_REQUIRE(h_nnz && d_indptr, "null pointer");
-    B200_REQUIRE(nQ == 0 || d_q, "null fingerprint pointer");
-    B200_REQUIRE(cap == 0 || (d_indices && d_values), "null output pointer");
-    B200_REQUIRE((reinterpret_cast<uintptr_t>(d_q) & 15) == 0 && (reinterpret_cast<uintptr_t>(d_lib) & 15) == 0,
-                 "fingerprint buffers must be 16-byte aligned");
-    const cudaStream_t s = asStream(stream);
-    *h_nnz               = 0;
-    if (nQ == 0 || nLib == 0) {  // no pair: every row is empty
-      B200_CUDA(cudaMemsetAsync(d_indptr, 0, (nQ + 1) * sizeof(int64_t), s));
-      return;
-    }
-    thresholdSearch(d_q, nQ, self ? d_q : d_lib, nLib, self, words, metric == B200MOL_METRIC_COSINE, threshold, d_indptr, d_indices,
-                    d_values, cap, h_nnz, s);
+    thresholdEntry(d_q, nQ, d_lib, nLib, words, metric == B200MOL_METRIC_COSINE ? kCosine : kTanimoto, 0.0, 0.0, threshold, d_indptr,
+                   d_indices, d_values, cap, h_nnz, stream);
+  });
+}
+
+// Tversky / Dice: (1/2, 1/2) runs Tanimoto's graph pass with the Dice table, (1, 1) is Tanimoto itself
+extern "C" int b200mol_tversky_threshold(const uint32_t* d_q, size_t nQ, const uint32_t* d_lib, size_t nLib, int words, double alpha,
+                                         double beta, double threshold, int64_t* d_indptr, int32_t* d_indices, double* d_values,
+                                         uint64_t cap, uint64_t* h_nnz, void* stream) {
+  return guarded([&] {
+    requireTverskyWeights(alpha, beta);
+    const Measure m = tverskyIsDice(alpha, beta) ? kDice : tverskyIsTanimoto(alpha, beta) ? kTanimoto : kTversky;
+    thresholdEntry(d_q, nQ, d_lib, nLib, words, m, alpha, beta, threshold, d_indptr, d_indices, d_values, cap, h_nnz, stream);
   });
 }

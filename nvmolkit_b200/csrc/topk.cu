@@ -47,6 +47,9 @@ __device__ unsigned long long g_topkStat[2];  // [0] candidates the tile passes 
 // The contract's order: value descending, column ascending. For Tanimoto this is also the order of the integer ratios
 // (the tile's filter compares those, see tanimoto_tc.cu): equal ratios round to the same fp64 and distinct ratios with
 // denominators <= 8192 differ by far more than an ulp. For cosine the fp64 values themselves are the only order there is.
+// Dice, 2c / (|A| + |B|), is an increasing function of Tanimoto's c / (|A| + |B|) ratio as well, with the same ties: a
+// Dice search is the Tanimoto search, whose values topkDiceValuesKernel then rewrites. General Tversky orders by the fp64
+// value, like cosine (the kernels' TV instantiations).
 __device__ __forceinline__ bool better(double v1, int32_t i1, double v2, int32_t i2) { return v1 > v2 || (v1 == v2 && i1 < i2); }
 
 // val / idx [0, n2) in shared memory, n2 a power of two, best first. Called by the whole CTA.
@@ -86,11 +89,20 @@ struct TopkArgs {
   uint32_t*       count;    // [nQ] candidate slots in use
   uint32_t*       redo;     // [nQ] 1: the row's candidates of this slab did not fit
   uint32_t        cap;
+  double          alpha, beta;  // Tversky weights (the TV instantiations)
 };
+
+// the value of a pair as the search's matrix stores it: Tanimoto / cosine, or (TV) Tversky
+template <bool TV>
+__device__ __forceinline__ double pairValue(const TopkArgs& a, int c, int pa, int pb) {
+  if constexpr (TV) return tverskyFromCounts(c, pa, pb, a.alpha, a.beta);
+  else return simFromCounts(c, pa, pb, a.cosine);
+}
 
 // Grid (parts, queries). Columns [colBeg, colEnd) in `parts` equal ranges; the CTA's k best of its range (fewer if the
 // bar lets fewer through) go to cand[q][part * k ..], padded with kNoCand. listValid: the row's list holds k entries and
 // its last one is a bar to start from. onlyRedo: rows not marked are left alone.
+template <bool TV>
 __global__ void __launch_bounds__(kSelThreads) topkScanKernel(const TopkArgs a, uint32_t colBeg, uint32_t colEnd, int listValid, int onlyRedo) {
   __shared__ double   val[kSelItems];
   __shared__ int32_t  idx[kSelItems];
@@ -133,7 +145,7 @@ __global__ void __launch_bounds__(kSelThreads) topkScanKernel(const TopkArgs a, 
         const uint4 y = __ldg(row + w), x = reinterpret_cast<const uint4*>(sq)[w];
         c += __popc(x.x & y.x) + __popc(x.y & y.y) + __popc(x.z & y.z) + __popc(x.w & y.w);
       }
-      const double v = simFromCounts(c, pa, a.popLib[col], a.cosine);
+      const double v = pairValue<TV>(a, c, pa, a.popLib[col]);
       if (better(v, static_cast<int32_t>(col), barV, barI)) {
         const int at = k + atomicAdd(&nPend, 1);
         val[at] = v, idx[at] = static_cast<int32_t>(col);
@@ -153,6 +165,7 @@ __global__ void __launch_bounds__(kSelThreads) topkScanKernel(const TopkArgs a, 
 // are re-counted exactly, sorted together with the list by the contract's key, and the k best become the list.
 // afterScan = 0, after a tile pass: a row that asked for more slots than there are merges nothing and is marked for the
 // scan. afterScan = 1: the slots hold the scan's results; with onlyRedo, of the marked rows only.
+template <bool TV>
 __global__ void __launch_bounds__(kSelThreads) topkSelectKernel(const TopkArgs a, int listValid, int afterScan, int onlyRedo) {
   __shared__ double  val[kSelItems];
   __shared__ int32_t idx[kSelItems];
@@ -189,7 +202,7 @@ __global__ void __launch_bounds__(kSelThreads) topkSelectKernel(const TopkArgs a
   for (int j = warp; j < n; j += kSelThreads / 32) {
     const uint32_t col = a.cand[static_cast<size_t>(q) * a.cap + j];
     double         v   = -1.0;
-    if (col != kNoCand) v = simFromCounts(countWith(col), pa, a.popLib[col], a.cosine);
+    if (col != kNoCand) v = pairValue<TV>(a, countWith(col), pa, a.popLib[col]);
     if (lane == 0) val[have + j] = v, idx[have + j] = col == kNoCand ? kNoIdx : static_cast<int32_t>(col);
   }
   const int n2 = nextPow2(have + n);
@@ -207,12 +220,34 @@ __global__ void __launch_bounds__(kSelThreads) topkSelectKernel(const TopkArgs a
   }
 }
 
+// Dice values of a finished Tanimoto search: entry (q, i) of the lists re-counted (one warp each) and stored as
+// tverskyFromCounts(c, |A|, |B|; 1/2, 1/2); the indices stay as they are.
+__global__ void __launch_bounds__(256) topkDiceValuesKernel(const uint32_t* __restrict__ q, const uint32_t* __restrict__ lib, int words,
+                                                            const int32_t* __restrict__ popQ, const int32_t* __restrict__ popLib,
+                                                            size_t nQ, int k, const int32_t* __restrict__ indices, double* values) {
+  const int          lane = threadIdx.x & 31;
+  const size_t       n = nQ * static_cast<size_t>(k), step = static_cast<size_t>(gridDim.x) * (blockDim.x / 32);
+  for (size_t e = (static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x) / 32; e < n; e += step) {
+    const size_t    row = e / k;
+    const int32_t   col = indices[e];
+    const uint32_t* x = q + row * words;
+    const uint32_t* y = lib + static_cast<size_t>(col) * words;
+    int             c = 0;
+    for (int w = lane; w < words; w += 32) c += __popc(x[w] & y[w]);
+    for (int o = 16; o; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+    if (lane == 0) values[e] = tverskyFromCounts(c, popQ[row], popLib[col], 0.5, 0.5);
+  }
+}
+
 }  // namespace
 
 unsigned long long readTopkStat(int i) { return readDeviceCounter(g_topkStat, i); }
 
-static void topkSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t nLib, int words, bool cosine, int k, double* values,
-                       int32_t* indices, cudaStream_t s) {
+// metric: Tanimoto, cosine or Tversky (alpha, beta); dice: a Tanimoto search whose values are then rewritten as Dice
+template <bool TV>
+static void topkSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t nLib, int words, TopkMetric metric, bool dice,
+                       double alpha, double beta, int k, double* values, int32_t* indices, cudaStream_t s) {
+  const bool cosine = metric == kTopkCosine;
   Scratch<int32_t> popQ(nQ, s), popLibOwn(lib == q && nLib == nQ ? 0 : nLib, s);
   launchRowPopcount(q, nQ, words, popQ.get(), s);
   if (popLibOwn.get()) launchRowPopcount(lib, nLib, words, popLibOwn.get(), s);
@@ -232,6 +267,14 @@ static void topkSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t
   a.words = words, a.k = k, a.cosine = cosine;
   a.values = values, a.indices = indices, a.bar = bar.get();
   a.cand = cand.get(), a.count = count.get(), a.redo = redo.get(), a.cap = cap;
+  a.alpha = alpha, a.beta = beta;
+  auto diceValues = [&]() {  // (a Dice search: the Tanimoto lists' values rewritten)
+    if (!dice) return;
+    const size_t   warps  = nQ * static_cast<size_t>(k);
+    const unsigned blocks = static_cast<unsigned>(std::min<size_t>((warps + 7) / 8, static_cast<size_t>(smCount()) * 16));
+    topkDiceValuesKernel<<<blocks, 256, 0, s>>>(q, lib, words, a.popQ, a.popLib, nQ, k, indices, values);
+    B200_LAUNCHED();
+  };
 
   // scan of [beg, end) + the select that merges it; parts: enough CTAs to fill the device, as far as the slots allow
   auto scanAndSelect = [&](size_t beg, size_t end, int listValid, int onlyRedo) {
@@ -241,11 +284,11 @@ static void topkSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t
       TopkArgs ar = a;
       ar.q += r0 * words, ar.popQ += r0, ar.values += r0 * k, ar.indices += r0 * k, ar.bar += r0;
       ar.cand += r0 * cap, ar.count += r0, ar.redo += r0;
-      topkScanKernel<<<dim3(parts, static_cast<unsigned>(std::min<size_t>(65535, nQ - r0))), kSelThreads, 0, s>>>(
+      topkScanKernel<TV><<<dim3(parts, static_cast<unsigned>(std::min<size_t>(65535, nQ - r0))), kSelThreads, 0, s>>>(
         ar, static_cast<uint32_t>(beg), static_cast<uint32_t>(end), listValid, onlyRedo);
       B200_LAUNCHED();
     }
-    topkSelectKernel<<<static_cast<unsigned>(nQ), kSelThreads, 0, s>>>(a, listValid, 1, onlyRedo);
+    topkSelectKernel<TV><<<static_cast<unsigned>(nQ), kSelThreads, 0, s>>>(a, listValid, 1, onlyRedo);
     B200_LAUNCHED();
   };
 
@@ -254,6 +297,7 @@ static void topkSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t
                       topkTileEligible(words) && nLib > warm;
   if (!tensor) {
     scanAndSelect(0, nLib, 0, 0);
+    diceValues();
     return;
   }
   scanAndSelect(0, warm, 0, 0);
@@ -264,14 +308,34 @@ static void topkSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t
   for (size_t done = warm; done < nLib;) {
     const size_t cols = std::min({nLib - done, slabMax, g_topkSlabCols > 0 ? slabMax : done});
     launchExpandBits(lib + done * words, cols, words, expLib.get(), s);
-    launchTopkTile(cosine, expQ.get(), nQ, popQ.get(), expLib.get(), cols, a.popLib + done, words, bar.get(), cand.get(), count.get(), cap,
-                   static_cast<uint32_t>(done), s);
-    topkSelectKernel<<<static_cast<unsigned>(nQ), kSelThreads, 0, s>>>(a, 1, 0, 0);
+    launchTopkTile(metric, expQ.get(), nQ, popQ.get(), expLib.get(), cols, a.popLib + done, words, bar.get(), cand.get(), count.get(), cap,
+                   static_cast<uint32_t>(done), alpha, beta, s);
+    topkSelectKernel<TV><<<static_cast<unsigned>(nQ), kSelThreads, 0, s>>>(a, 1, 0, 0);
     B200_LAUNCHED();
     scanAndSelect(done, done + cols, 1, 1);  // the rows whose candidates did not fit (none, as a rule: the CTAs return at once)
     done += cols;
     ++g_topkSlabsLast;
   }
+  diceValues();
+}
+
+// the checks both entry points make before any device work
+static void topkChecks(const uint32_t* d_q, size_t nQ, const uint32_t*& d_lib, size_t& nLib, int words, int k, double* d_values,
+                       int32_t* d_indices) {
+  B200_REQUIRE(nQ == 0 || d_q, "null fingerprint pointer");
+  if (!d_lib) {
+    d_lib = d_q;
+    nLib  = nQ;
+  }
+  B200_REQUIRE(words > 0 && words % 4 == 0 && words <= 128,
+               "fingerprint width must be a multiple of 128 bits and at most 4096 bits (got %d words)", words);
+  B200_REQUIRE(nQ < (1ull << 31) && nLib < (1ull << 31), "too many fingerprints");
+  B200_REQUIRE(k >= 1 && static_cast<size_t>(k) <= nLib && k <= kTopkMax, "k must be in [1, min(library size, %d)] (got k = %d, library %zu)",
+               kTopkMax, k, nLib);
+  if (nQ == 0) return;
+  B200_REQUIRE(d_values && d_indices, "null output pointer");
+  B200_REQUIRE((reinterpret_cast<uintptr_t>(d_q) & 15) == 0 && (reinterpret_cast<uintptr_t>(d_lib) & 15) == 0,
+               "fingerprint buffers must be 16-byte aligned");
 }
 
 }  // namespace b200
@@ -282,20 +346,25 @@ extern "C" int b200mol_similarity_topk(const uint32_t* d_q, size_t nQ, const uin
                                        double* d_values, int32_t* d_indices, void* stream) {
   return guarded([&] {
     B200_REQUIRE(metric == B200MOL_METRIC_TANIMOTO || metric == B200MOL_METRIC_COSINE, "unknown metric %d", metric);
-    B200_REQUIRE(nQ == 0 || d_q, "null fingerprint pointer");
-    if (!d_lib) {
-      d_lib = d_q;
-      nLib  = nQ;
-    }
-    B200_REQUIRE(words > 0 && words % 4 == 0 && words <= 128,
-                 "fingerprint width must be a multiple of 128 bits and at most 4096 bits (got %d words)", words);
-    B200_REQUIRE(nQ < (1ull << 31) && nLib < (1ull << 31), "too many fingerprints");
-    B200_REQUIRE(k >= 1 && static_cast<size_t>(k) <= nLib && k <= kTopkMax, "k must be in [1, min(library size, %d)] (got k = %d, library %zu)",
-                 kTopkMax, k, nLib);
+    topkChecks(d_q, nQ, d_lib, nLib, words, k, d_values, d_indices);
     if (nQ == 0) return;
-    B200_REQUIRE(d_values && d_indices, "null output pointer");
-    B200_REQUIRE((reinterpret_cast<uintptr_t>(d_q) & 15) == 0 && (reinterpret_cast<uintptr_t>(d_lib) & 15) == 0,
-                 "fingerprint buffers must be 16-byte aligned");
-    topkSearch(d_q, nQ, d_lib, nLib, words, metric == B200MOL_METRIC_COSINE, k, d_values, d_indices, asStream(stream));
+    topkSearch<false>(d_q, nQ, d_lib, nLib, words, metric == B200MOL_METRIC_COSINE ? kTopkCosine : kTopkTanimoto, false, 0.0, 0.0, k,
+                      d_values, d_indices, asStream(stream));
+  });
+}
+
+// Tversky / Dice: (1/2, 1/2) and (1, 1) are Tanimoto searches (Dice with its values rewritten; Tversky(1, 1) is Tanimoto's
+// value bit for bit), any other weights the Tversky instantiations.
+extern "C" int b200mol_tversky_topk(const uint32_t* d_q, size_t nQ, const uint32_t* d_lib, size_t nLib, int words, double alpha,
+                                    double beta, int k, double* d_values, int32_t* d_indices, void* stream) {
+  return guarded([&] {
+    requireTverskyWeights(alpha, beta);
+    topkChecks(d_q, nQ, d_lib, nLib, words, k, d_values, d_indices);
+    if (nQ == 0) return;
+    const bool dice = tverskyIsDice(alpha, beta);
+    if (dice || tverskyIsTanimoto(alpha, beta))
+      topkSearch<false>(d_q, nQ, d_lib, nLib, words, kTopkTanimoto, dice, alpha, beta, k, d_values, d_indices, asStream(stream));
+    else
+      topkSearch<true>(d_q, nQ, d_lib, nLib, words, kTopkTversky, false, alpha, beta, k, d_values, d_indices, asStream(stream));
   });
 }

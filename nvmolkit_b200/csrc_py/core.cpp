@@ -123,6 +123,10 @@ PYBIND11_MODULE(_core, m) {
   DEF(b200mol_tanimoto_count_ge);
   DEF(b200mol_similarity_topk);
   DEF(b200mol_similarity_threshold);
+  DEF(b200mol_tversky_cross);
+  DEF(b200mol_tversky_cross_host);
+  DEF(b200mol_tversky_topk);
+  DEF(b200mol_tversky_threshold);
   DEF(b200mol_maxmin_pick);
   DEF(b200mol_leader_pick);
   DEF(b200mol_butina_fused);

@@ -12,7 +12,7 @@ from nvmolkit_b200._interop import fingerprint_matrix, require_cuda, stream_ctx,
 from nvmolkit_b200.types import AsyncGpuResult
 
 
-def _cross(fn_name: str, one, two, stream) -> AsyncGpuResult:
+def _cross(fn_name: str, one, two, stream, weights=()) -> AsyncGpuResult:
     sptr = stream_ptr(stream)  # validates `stream` first, like the reference (TypeError)
     require_cuda()
     a = fingerprint_matrix(one, "fingerprint_group_one")
@@ -21,7 +21,7 @@ def _cross(fn_name: str, one, two, stream) -> AsyncGpuResult:
         raise ValueError(f"fingerprint widths differ: {a.shape[1]} vs {b.shape[1]} words")
     with stream_ctx(stream):
         out = torch.empty((a.shape[0], b.shape[0]), dtype=torch.float64, device=a.device)
-        _lib.call(fn_name, a.data_ptr(), a.shape[0], b.data_ptr(), b.shape[0], a.shape[1], out.data_ptr(), sptr)
+        _lib.call(fn_name, a.data_ptr(), a.shape[0], b.data_ptr(), b.shape[0], a.shape[1], *weights, out.data_ptr(), sptr)
         # keep inputs alive until the stream has consumed them
         a.record_stream(torch.cuda.current_stream())
         b.record_stream(torch.cuda.current_stream())
@@ -48,7 +48,8 @@ def _check_k(k, library_size: int) -> int:
     return k
 
 
-def _topk(metric: str, one, two, k, stream):
+def _topk(metric, one, two, k, stream):
+    """metric: a key of _lib.METRIC, or the (alpha, beta) of a Tversky search"""
     sptr = stream_ptr(stream)  # validates `stream` first, like the matrix calls (TypeError)
     require_cuda()
     a = fingerprint_matrix(one, "fingerprint_group_one")
@@ -59,8 +60,10 @@ def _topk(metric: str, one, two, k, stream):
     with stream_ctx(stream):
         values = torch.empty((a.shape[0], k), dtype=torch.float64, device=a.device)
         indices = torch.empty((a.shape[0], k), dtype=torch.int32, device=a.device)
-        _lib.call("b200mol_similarity_topk", a.data_ptr(), a.shape[0], b.data_ptr(), b.shape[0], a.shape[1],
-                  _lib.METRIC[metric], k, values.data_ptr(), indices.data_ptr(), sptr)
+        fn, measure = (("b200mol_similarity_topk", (_lib.METRIC[metric],)) if isinstance(metric, str)
+                       else ("b200mol_tversky_topk", metric))
+        _lib.call(fn, a.data_ptr(), a.shape[0], b.data_ptr(), b.shape[0], a.shape[1], *measure, k, values.data_ptr(),
+                  indices.data_ptr(), sptr)
         # keep inputs alive until the stream has consumed them
         a.record_stream(torch.cuda.current_stream())
         b.record_stream(torch.cuda.current_stream())
@@ -91,7 +94,8 @@ def _check_threshold(threshold) -> float:
     return t
 
 
-def _threshold(metric: str, one, two, threshold, stream):
+def _threshold(metric, one, two, threshold, stream):
+    """metric: a key of _lib.METRIC, or the (alpha, beta) of a Tversky search"""
     sptr = stream_ptr(stream)  # validates `stream` first, like the matrix calls (TypeError)
     t = _check_threshold(threshold)
     require_cuda()
@@ -108,13 +112,14 @@ def _threshold(metric: str, one, two, threshold, stream):
         indptr = torch.empty(n_q + 1, dtype=torch.int64, device=a.device)
         # a first guess at the result size; a larger result is reported and the call is made once more with room for it
         cap = min(max(1 << 20, 64 * n_q), n_q * n_lib)
+        fn, measure = (("b200mol_similarity_threshold", (_lib.METRIC[metric],)) if isinstance(metric, str)
+                       else ("b200mol_tversky_threshold", metric))
         for _ in range(2):
             indices = torch.empty(cap, dtype=torch.int32, device=a.device)
             values = torch.empty(cap, dtype=torch.float64, device=a.device)
             nnz = C.c_uint64(0)
-            _lib.call("b200mol_similarity_threshold", a.data_ptr(), n_q, None if b is None else b.data_ptr(), n_lib,
-                      a.shape[1], _lib.METRIC[metric], t, indptr.data_ptr(), indices.data_ptr(), values.data_ptr(), cap,
-                      C.byref(nnz), sptr)
+            _lib.call(fn, a.data_ptr(), n_q, None if b is None else b.data_ptr(), n_lib, a.shape[1], *measure, t,
+                      indptr.data_ptr(), indices.data_ptr(), values.data_ptr(), cap, C.byref(nnz), sptr)
             if nnz.value <= cap:
                 break
             cap = int(nnz.value)
@@ -148,7 +153,8 @@ def thresholdCosineSimilarity(fingerprint_group_one, fingerprint_group_two=None,
     return _threshold("cosine", fingerprint_group_one, fingerprint_group_two, threshold, stream)
 
 
-def _cross_host(metric: str, one, two, max_device_bytes: int = 0) -> np.ndarray:
+def _cross_host(metric, one, two, max_device_bytes: int = 0) -> np.ndarray:
+    """metric: a key of _lib.METRIC, or the (alpha, beta) of a Tversky matrix"""
     require_cuda()
 
     def host(x):
@@ -166,8 +172,10 @@ def _cross_host(metric: str, one, two, max_device_bytes: int = 0) -> np.ndarray:
     if a.shape[1] != b.shape[1]:
         raise ValueError(f"fingerprint widths differ: {a.shape[1]} vs {b.shape[1]} words")
     out = np.empty((a.shape[0], b.shape[0]), dtype=np.float64)
-    _lib.call("b200mol_similarity_cross_host", a.ctypes.data, a.shape[0], b.ctypes.data, b.shape[0], a.shape[1],
-              _lib.METRIC[metric], out.ctypes.data, int(max_device_bytes))
+    fn, measure = (("b200mol_similarity_cross_host", (_lib.METRIC[metric],)) if isinstance(metric, str)
+                   else ("b200mol_tversky_cross_host", metric))
+    _lib.call(fn, a.ctypes.data, a.shape[0], b.ctypes.data, b.shape[0], a.shape[1], *measure, out.ctypes.data,
+              int(max_device_bytes))
     return out
 
 
@@ -178,3 +186,82 @@ def crossTanimotoSimilarityMemoryConstrained(fingerprint_group_one, fingerprint_
 
 def crossCosineSimilarityMemoryConstrained(fingerprint_group_one, fingerprint_group_two=None) -> np.ndarray:
     return _cross_host("cosine", fingerprint_group_one, fingerprint_group_two)
+
+
+# ---- Dice and Tversky ----
+# tversky(c, a, b; alpha, beta) = 0 if c == 0, else c / ((alpha (a - c) + beta (b - c)) + c), a = |A| (group one, the row),
+# b = |B|, c = |A & B|: each product, sum and the quotient one fp64 operation rounded to nearest, in that order. Dice,
+# 2c / (a + b), is (1/2, 1/2); (1, 1) is Tanimoto bit for bit. alpha weights the bits only in group one's fingerprint, as
+# in RDKit's TverskySimilarity(fp1, fp2, a, b), so cross(one, two, alpha, beta) is cross(two, one, beta, alpha).T.
+# For dyadic weights (0, 1/4, 1/2, 1, 2, ...) the value does not depend on the order of evaluation; for others, such as
+# (0.3, 0.7), an expanded form like alpha a + beta b + (1 - alpha - beta) c may differ from it by a few ulp, so bit parity
+# with RDKit is not claimed there.
+TVERSKY_MAX_WEIGHT = 1000.0  # the weights' range, 0 <= alpha, beta <= 1000 (the float tile filters are derived for it)
+DICE = (0.5, 0.5)
+
+
+def _check_weights(alpha, beta) -> tuple:
+    out = []
+    for name, w in (("alpha", alpha), ("beta", beta)):
+        if isinstance(w, bool) or not isinstance(w, (int, float, np.integer, np.floating)):
+            raise ValueError(f"Tversky {name} must be a real number, got {type(w).__name__}")
+        w = float(w)
+        if not 0.0 <= w <= TVERSKY_MAX_WEIGHT:  # (NaN fails too; so does inf)
+            raise ValueError(f"Tversky {name} must be finite with 0 <= {name} <= {TVERSKY_MAX_WEIGHT:g} (got {w})")
+        out.append(w)
+    return tuple(out)
+
+
+def crossDiceSimilarity(fingerprint_group_one, fingerprint_group_two=None, stream=None) -> AsyncGpuResult:
+    """(n, m) fp64 Dice similarities 2|A & B| / (|A| + |B|) (0 for an empty intersection); all-to-all within group one
+    when group two is None. Asynchronous. Bit-identical to ``crossTverskySimilarity(..., alpha=0.5, beta=0.5)``."""
+    return _cross("b200mol_tversky_cross", fingerprint_group_one, fingerprint_group_two, stream, DICE)
+
+
+def crossTverskySimilarity(fingerprint_group_one, fingerprint_group_two=None, *, alpha, beta, stream=None) -> AsyncGpuResult:
+    """(n, m) fp64 Tversky similarities c / ((alpha (a - c) + beta (b - c)) + c), a the popcount of the row's fingerprint
+    (group one), b the column's, c their intersection, 0 when c == 0; all-to-all within group one when group two is
+    None. ``0 <= alpha, beta <= 1000``. Tversky(1, 0) = c / a is how much of the query a library fingerprint contains;
+    (0.9, 0.1) is the usual fragment / scaffold setting. Asynchronous. See the module note on RDKit parity."""
+    weights = _check_weights(alpha, beta)  # (before anything touches the device)
+    return _cross("b200mol_tversky_cross", fingerprint_group_one, fingerprint_group_two, stream, weights)
+
+
+def topKDiceSimilarity(fingerprint_group_one, fingerprint_group_two=None, k=10, stream=None):
+    """Dice twin of ``topKTanimotoSimilarity``: rows of ``crossDiceSimilarity``. Dice orders pairs exactly as Tanimoto
+    does, so the indices are those of ``topKTanimotoSimilarity`` on the same inputs."""
+    return _topk(DICE, fingerprint_group_one, fingerprint_group_two, k, stream)
+
+
+def topKTverskySimilarity(fingerprint_group_one, fingerprint_group_two=None, k=10, *, alpha, beta, stream=None):
+    """Tversky twin of ``topKTanimotoSimilarity``: the first k columns of each row of ``crossTverskySimilarity`` by
+    (value descending, column ascending). With an asymmetric measure a self search need not list the self-match first:
+    under (alpha, beta) = (1, 0) every superset of the query also scores 1.0, and ties go to the lowest index."""
+    weights = _check_weights(alpha, beta)  # (before anything touches the device)
+    return _topk(weights, fingerprint_group_one, fingerprint_group_two, k, stream)
+
+
+def thresholdDiceSimilarity(fingerprint_group_one, fingerprint_group_two=None, *, threshold, stream=None):
+    """Dice twin of ``thresholdTanimotoSimilarity``: the entries of ``crossDiceSimilarity`` that are ``>= threshold``,
+    as CSR. Synchronises ``stream``."""
+    return _threshold(DICE, fingerprint_group_one, fingerprint_group_two, threshold, stream)
+
+
+def thresholdTverskySimilarity(fingerprint_group_one, fingerprint_group_two=None, *, alpha, beta, threshold, stream=None):
+    """Tversky twin of ``thresholdTanimotoSimilarity``: the entries of ``crossTverskySimilarity`` that are
+    ``>= threshold``, as CSR; a self search (group two None) gives the same result as passing group one twice.
+    Synchronises ``stream``."""
+    weights = _check_weights(alpha, beta)  # (before anything touches the device)
+    return _threshold(weights, fingerprint_group_one, fingerprint_group_two, threshold, stream)
+
+
+def crossDiceSimilarityMemoryConstrained(fingerprint_group_one, fingerprint_group_two=None) -> np.ndarray:
+    """Host-in / host-out Dice matrix as a NumPy array, computed in row blocks with overlapped D2H."""
+    return _cross_host(DICE, fingerprint_group_one, fingerprint_group_two)
+
+
+def crossTverskySimilarityMemoryConstrained(fingerprint_group_one, fingerprint_group_two=None, *, alpha,
+                                            beta) -> np.ndarray:
+    """Host-in / host-out Tversky matrix as a NumPy array, computed in row blocks with overlapped D2H."""
+    weights = _check_weights(alpha, beta)
+    return _cross_host(weights, fingerprint_group_one, fingerprint_group_two)
