@@ -102,7 +102,8 @@ int b200mol_set_option(const char* key, long long value);
  * "leader_bulk_pairs_last" (window x pick pairs sent through the count pass), "leader_window_pairs_last" and
  * "leader_block_pairs_last" (pairs the resolver compared against earlier picks of the same window / of the same block;
  * these two synchronise the device). Of the last b200mol_conformer_rmsd_mapped: "rmsd_match_chunks_last" (chunks of
- * mappings it ran). */
+ * mappings it ran). Of the last b200mol_morgan that launched: "morgan_global_slab_last" (1: the per-molecule slabs were
+ * in device memory, 0: in shared memory). */
 int b200mol_get_option(const char* key, long long* value);
 /* Per-phase CUDA-event timing inside the library (off by default). Phases: "neighbor_pass" (the N^2 tile kernel
  * alone), "csr_build", "cluster_loop", "bfgs". b200mol_profile_read waits for the phase's stop event. */
@@ -281,7 +282,17 @@ int b200mol_butina_dense(const double* d_dist, size_t n, double cutoff, int32_t*
  *   d_atom_inv[totalAtoms]  u32 atom invariants;  d_bond_inv[totalBonds] u32 bond invariants (bond type)
  *   d_bond_a / d_bond_b [totalBonds]  molecule-local atom indices (u16)
  *   d_out  u32[nMols][fpBits/32], overwritten.
- * Molecules may have up to 1024 atoms and 1024 bonds, and any atom up to 8 bonds (kMaxBondsPerAtom).
+ * Bond endpoints must be smaller than their molecule's atom count and distinct (no self-loops); MolGraphBatch checks
+ * this, the kernel does not. An atom may have up to 16 bonds. Any molecule of up to 1024 atoms and 1024 bonds is accepted
+ * at every radius <= 16. Exactly: with A = max(maxAtomsPerMol, 1), B = max(maxBondsPerMol, 1), w = ceil(B / 32),
+ * R = max(radius, 1) and r(x) = x rounded up to a multiple of 16, a molecule's working set (slab) is
+ *   S = 2 r(4A) + 2 r(4Aw) + r(4RAw) + r(4(A + 1)) + 2 r(4B) + 2 r(A) + r(fpBits / 8)  bytes,
+ * and the call is accepted when S <= 256 MiB. Slabs of S <= 200 KiB live in shared memory; larger ones in a device
+ * scratch buffer of at most 256 MiB per call (get option "morgan_global_slab_last" says which the last call used).
+ * Refusals (B200MOL_ERR_INVALID): fpBits not a positive multiple of 32, radius outside [0, 16], maxAtomsPerMol or
+ * maxBondsPerMol outside [0, 65536), S > 256 MiB (all before any launch); after the kernel, a molecule with more atoms
+ * or bonds than maxAtomsPerMol / maxBondsPerMol (its row is zero) or, at radius >= 1, an atom with more than 16 bonds.
+ * Synchronises `stream`.
  * Replaces launchMorganFingerprintKernelBatch<fpSize> (src/morgan_fingerprint_kernels.h:90-95, .cu:152-432) and its
  * CPU twin for large molecules (src/morgan_fingerprint_cpu.cpp:61-255). */
 int b200mol_morgan(const int32_t* d_atom_starts, const int32_t* d_bond_starts, const uint32_t* d_atom_inv,

@@ -11,29 +11,41 @@
 // Design: the reference sorts all (bitset, invariant, atom) tuples of a round with a tile-wide CUB merge sort and
 // scans earlier rounds linearly in global memory. Only the equivalence classes matter, so this kernel replaces the sort
 // with a rank test — "is there an equal bitset with a smaller (invariant, atom) key, or an equal accepted bitset from
-// an earlier round" — all in shared memory, and handles molecules of any size that fits shared memory (no CPU twin).
+// an earlier round" — inside one per-molecule slab. The slab is in shared memory when it fits 200 KiB; larger
+// molecules (up to 1024 atoms and 1024 bonds at every radius, exactly: a slab of at most 256 MiB, include/b200mol.h) run
+// the same code with each warp's slab in a device scratch buffer (no CPU twin). An atom may have up to 16 bonds.
+#include <algorithm>
+
 #include "common.cuh"
+#include "options.cuh"
 
 namespace b200 {
+
+long long g_morganGlobalSlabLast = 0;  // 1: the last call kept its slabs in global memory ("morgan_global_slab_last")
+
 namespace {
 
-constexpr int kMaxDeg = 16;
+constexpr int       kMaxDeg        = 16;
+constexpr long long kSharedBudget  = 200 * 1024;  // bytes of shared memory the slabs of one CTA may take
+constexpr long long kGlobalSlabCap = 256ll << 20;  // bytes of global scratch for the slabs of one call, and of one slab
 
 __device__ __forceinline__ void hashCombine(uint32_t& seed, uint32_t v) {
   seed ^= v + 0x9e3779b9u + (seed << 6) + (seed >> 2);
 }
 
-struct MorganLayout {  // byte offsets inside one molecule's shared-memory slab
-  int inv, invNext, nbhd, nbhdRound, seen, adjStart, adjBond, adjOther, dead, cand, fp, total;
+template <class Int>  // int on the device; long long on the host, which checks the size before any launch
+struct MorganLayout {  // byte offsets inside one molecule's slab
+  Int inv, invNext, nbhd, nbhdRound, seen, adjStart, adjBond, adjOther, dead, cand, fp, total;
 };
 
-__host__ __device__ inline MorganLayout morganLayout(int maxAtoms, int maxBonds, int radius, int fpWords) {
-  const int    bw = (maxBonds + 31) / 32 > 0 ? (maxBonds + 31) / 32 : 1;
-  MorganLayout L;
-  int          o = 0;
-  auto         take = [&](int bytes) {
-    const int at = o;
-    o += (bytes + 15) & ~15;
+template <class Int>
+__host__ __device__ inline MorganLayout<Int> morganLayout(Int maxAtoms, Int maxBonds, Int radius, Int fpWords) {
+  const Int         bw = (maxBonds + 31) / 32 > 0 ? (maxBonds + 31) / 32 : 1;
+  MorganLayout<Int> L;
+  Int               o = 0;
+  auto              take = [&](Int bytes) {
+    const Int at = o;
+    o += (bytes + 15) & ~static_cast<Int>(15);
     return at;
   };
   L.inv       = take(maxAtoms * 4);
@@ -51,19 +63,15 @@ __host__ __device__ inline MorganLayout morganLayout(int maxAtoms, int maxBonds,
   return L;
 }
 
-__global__ void morganKernel(const int32_t* __restrict__ atomStarts, const int32_t* __restrict__ bondStarts,
-                             const uint32_t* __restrict__ atomInv, const uint32_t* __restrict__ bondInv,
-                             const uint16_t* __restrict__ bondA, const uint16_t* __restrict__ bondB, int nMols,
-                             int maxAtoms, int maxBonds, int radius, int fpBits, uint32_t* __restrict__ out,
-                             int* __restrict__ errFlag) {
-  extern __shared__ __align__(16) uint8_t smem[];
-  const int          lane = threadIdx.x & 31;
-  const int          wib  = threadIdx.x >> 5;
-  const int          mol  = blockIdx.x * (blockDim.x >> 5) + wib;
-  if (mol >= nMols) return;
+// One molecule, by one warp, in the slab at `slab` (shared or global memory).
+__device__ __forceinline__ void morganMol(const int32_t* __restrict__ atomStarts, const int32_t* __restrict__ bondStarts,
+                                          const uint32_t* __restrict__ atomInv, const uint32_t* __restrict__ bondInv,
+                                          const uint16_t* __restrict__ bondA, const uint16_t* __restrict__ bondB,
+                                          int mol, const MorganLayout<int>& L, uint8_t* slab, int maxAtoms,
+                                          int maxBonds, int radius, int fpBits, uint32_t* __restrict__ out,
+                                          int* __restrict__ errFlag) {
+  const int          lane    = threadIdx.x & 31;
   const int          fpWords = fpBits >> 5;
-  const MorganLayout L       = morganLayout(maxAtoms, maxBonds, radius, fpWords);
-  uint8_t*           slab    = smem + static_cast<size_t>(wib) * L.total;
   uint32_t*          inv       = reinterpret_cast<uint32_t*>(slab + L.inv);
   uint32_t*          invNext   = reinterpret_cast<uint32_t*>(slab + L.invNext);
   uint32_t*          nbhd      = reinterpret_cast<uint32_t*>(slab + L.nbhd);
@@ -94,7 +102,7 @@ __global__ void morganKernel(const int32_t* __restrict__ atomStarts, const int32
     for (int w = 0; w < bw; ++w) nbhd[a * bw + w] = 0;
   }
   __syncwarp();
-  // adjacency as CSR in shared memory: degree count, warp scan, fill
+  // adjacency as CSR in the slab: degree count, warp scan, fill
   for (int b = lane; b < nB; b += 32) {
     atomicAdd(&adjStart[bondA[b0 + b] + 1], 1);
     atomicAdd(&adjStart[bondB[b0 + b] + 1], 1);
@@ -223,6 +231,32 @@ __global__ void morganKernel(const int32_t* __restrict__ atomStarts, const int32
   }
   __syncwarp();
   for (int w = lane; w < fpWords; w += 32) outRow[w] = fp[w];
+  __syncwarp();  // every lane has read the slab before the warp's next molecule overwrites it
+}
+
+// kGlobalSlab == false: each warp of a CTA has its slab in dynamic shared memory, and the grid has a warp per molecule.
+// true: warp w of the grid has its slab at gslab + w * L.total in global memory and takes molecules w, w + (warps of the
+// grid), ... (molecules whose slab does not fit the shared-memory budget).
+template <bool kGlobalSlab>
+__global__ void morganKernel(const int32_t* __restrict__ atomStarts, const int32_t* __restrict__ bondStarts,
+                             const uint32_t* __restrict__ atomInv, const uint32_t* __restrict__ bondInv,
+                             const uint16_t* __restrict__ bondA, const uint16_t* __restrict__ bondB, int nMols,
+                             int maxAtoms, int maxBonds, int radius, int fpBits, uint8_t* __restrict__ gslab,
+                             uint32_t* __restrict__ out, int* __restrict__ errFlag) {
+  extern __shared__ __align__(16) uint8_t smem[];
+  const int               wib  = threadIdx.x >> 5;
+  const int               warp = blockIdx.x * (blockDim.x >> 5) + wib;
+  const MorganLayout<int> L    = morganLayout<int>(maxAtoms, maxBonds, radius, fpBits >> 5);
+  if constexpr (!kGlobalSlab) {
+    if (warp < nMols)
+      morganMol(atomStarts, bondStarts, atomInv, bondInv, bondA, bondB, warp, L, smem + static_cast<size_t>(wib) * L.total,
+                maxAtoms, maxBonds, radius, fpBits, out, errFlag);
+  } else {
+    uint8_t* slab = gslab + static_cast<size_t>(warp) * L.total;
+    for (int mol = warp; mol < nMols; mol += gridDim.x * (blockDim.x >> 5))
+      morganMol(atomStarts, bondStarts, atomInv, bondInv, bondA, bondB, mol, L, slab, maxAtoms, maxBonds, radius,
+                fpBits, out, errFlag);
+  }
 }
 
 }  // namespace
@@ -242,29 +276,47 @@ extern "C" int b200mol_morgan(const int32_t* d_atom_starts, const int32_t* d_bon
     B200_REQUIRE(nMols < (1ull << 31), "too many molecules");
     if (nMols == 0) return;
     B200_REQUIRE(d_atom_starts && d_bond_starts && d_out, "null pointer");
-    cudaStream_t       s       = asStream(stream);
-    const int          maxA    = maxAtomsPerMol > 0 ? maxAtomsPerMol : 1;
-    const int          maxB    = maxBondsPerMol > 0 ? maxBondsPerMol : 1;
-    const MorganLayout L       = morganLayout(maxA, maxB, radius, fpBits / 32);
-    const size_t       budget  = 200 * 1024;
-    B200_REQUIRE(static_cast<size_t>(L.total) <= budget,
-                 "molecule too large for the shared-memory Morgan kernel (%d atoms, %d bonds, radius %d need %d bytes)",
-                 maxAtomsPerMol, maxBondsPerMol, radius, L.total);
-    int warps = static_cast<int>(budget / 2 / L.total);  // two CTAs per SM when the slab is small
-    warps     = warps < 1 ? 1 : (warps > 8 ? 8 : warps);
-    const size_t smemBytes = static_cast<size_t>(warps) * L.total;
-    static size_t configured[kMaxDevices] = {};
-    if (smemBytes > configured[currentDeviceSlot()]) {
-      B200_CUDA(cudaFuncSetAttribute(morganKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(budget)));
-      configured[currentDeviceSlot()] = budget;
-    }
+    cudaStream_t                  s    = asStream(stream);
+    const int                     maxA = maxAtomsPerMol > 0 ? maxAtomsPerMol : 1;
+    const int                     maxB = maxBondsPerMol > 0 ? maxBondsPerMol : 1;
+    const MorganLayout<long long> L    = morganLayout<long long>(maxA, maxB, radius, fpBits / 32);
+    B200_REQUIRE(L.total <= kGlobalSlabCap,
+                 "molecule too large for the Morgan kernel (%d atoms, %d bonds, radius %d need %lld bytes of working "
+                 "memory, at most %lld)", maxAtomsPerMol, maxBondsPerMol, radius, L.total, kGlobalSlabCap);
+    const int    slabBytes = static_cast<int>(L.total);
     Scratch<int> err(1, s);
     B200_CUDA(cudaMemsetAsync(err.get(), 0, sizeof(int), s));
-    const unsigned blocks = static_cast<unsigned>((nMols + warps - 1) / warps);
-    morganKernel<<<blocks, warps * 32, smemBytes, s>>>(d_atom_starts, d_bond_starts, d_atom_inv, d_bond_inv, d_bond_a,
-                                                      d_bond_b, static_cast<int>(nMols), maxA, maxB, radius, fpBits,
-                                                      d_out, err.get());
-    B200_LAUNCHED();
+    if (L.total <= kSharedBudget) {
+      int warps = static_cast<int>(kSharedBudget / 2 / slabBytes);  // two CTAs per SM when the slab is small
+      warps     = warps < 1 ? 1 : (warps > 8 ? 8 : warps);
+      const size_t smemBytes = static_cast<size_t>(warps) * slabBytes;
+      static size_t configured[kMaxDevices] = {};
+      if (smemBytes > configured[currentDeviceSlot()]) {
+        B200_CUDA(cudaFuncSetAttribute(morganKernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       static_cast<int>(kSharedBudget)));
+        configured[currentDeviceSlot()] = kSharedBudget;
+      }
+      const unsigned blocks = static_cast<unsigned>((nMols + warps - 1) / warps);
+      morganKernel<false><<<blocks, warps * 32, smemBytes, s>>>(d_atom_starts, d_bond_starts, d_atom_inv, d_bond_inv,
+                                                                 d_bond_a, d_bond_b, static_cast<int>(nMols), maxA, maxB,
+                                                                 radius, fpBits, nullptr, d_out, err.get());
+      B200_LAUNCHED();
+      g_morganGlobalSlabLast = 0;
+    } else {
+      // As many warps as the scratch cap holds slabs (at least one), no more than there are molecules or than can be
+      // resident at once; each loops over its molecules.
+      long long warps = kGlobalSlabCap / L.total;
+      warps           = std::min<long long>(warps, static_cast<long long>(nMols));
+      warps           = std::min<long long>(warps, 32ll * smCount());
+      const int      perCta = static_cast<int>(std::min<long long>(warps, 8));
+      const unsigned blocks = static_cast<unsigned>(warps / perCta);
+      Scratch<uint8_t> slabs(static_cast<size_t>(blocks) * perCta * slabBytes, s);
+      morganKernel<true><<<blocks, perCta * 32, 0, s>>>(d_atom_starts, d_bond_starts, d_atom_inv, d_bond_inv, d_bond_a,
+                                                        d_bond_b, static_cast<int>(nMols), maxA, maxB, radius, fpBits,
+                                                        slabs.get(), d_out, err.get());
+      B200_LAUNCHED();
+      g_morganGlobalSlabLast = 1;
+    }
     int hErr = 0;
     B200_CUDA(cudaMemcpyAsync(&hErr, err.get(), sizeof(int), cudaMemcpyDeviceToHost, s));
     B200_CUDA(cudaStreamSynchronize(s));  // documented sync: input validation result

@@ -84,6 +84,7 @@ constexpr Option kOptions[] = {
     {"leader_block_pairs_last", {readLeaderStat, 1}, kReadOnly},
     {"rmsd_match_chunk", &g_rmsdMatchChunk, kRange, 0, kBelow2To31, "must be in [0, 2^31)"},
     {"rmsd_match_chunks_last", &g_rmsdMatchChunksLast, kReadOnly},
+    {"morgan_global_slab_last", &g_morganGlobalSlabLast, kReadOnly},
     // huge = the stepwise loop only
     {"butina_min_round_commits", &g_butinaMinCommits, kClamp, 0, 1000000000, "must be >= 0"},
     {"bfgs_ctas_per_sm", &g_bfgsCtasPerSm, kRange, 1, 8, "must be in [1, 8]"},

@@ -29,6 +29,8 @@ extern unsigned long long g_leaderBulkPairsLast;
 // conformer RMSD matrices (conformer_rmsd.cu)
 extern long long g_rmsdMatchChunk;
 extern long long g_rmsdMatchChunksLast;
+// Morgan fingerprints (morgan.cu)
+extern long long g_morganGlobalSlabLast;
 // Butina clustering (butina.cu)
 extern int g_butinaMinCommits;
 // minimiser and embedder (bfgs.cu, etkdg.cu)

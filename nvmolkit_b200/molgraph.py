@@ -45,6 +45,19 @@ class MolGraphBatch:
         self.bond_b = np.ascontiguousarray(self.bond_b, dtype=np.uint16)
         if len(self.atom_starts) != len(self.bond_starts) or len(self.atom_starts) < 1:
             raise ValueError("atom_starts and bond_starts must both have nMols+1 entries")
+        # The kernel trusts these: an endpoint past its molecule would index outside the molecule's working memory, and
+        # a self-loop would be counted twice there but once by RDKit.
+        for name, starts, n in (("atom", self.atom_starts, len(self.atom_inv)),
+                                ("bond", self.bond_starts, len(self.bond_inv))):
+            if starts[0] != 0 or (np.diff(starts) < 0).any() or starts[-1] != n:
+                raise ValueError(f"{name}_starts must start at 0, not decrease and end at the number of {name}s ({n})")
+        if len(self.bond_a) != len(self.bond_inv) or len(self.bond_b) != len(self.bond_inv):
+            raise ValueError("bond_a, bond_b and bond_inv must have one entry per bond")
+        n_atoms = np.repeat(np.diff(self.atom_starts), np.diff(self.bond_starts))
+        if (self.bond_a >= n_atoms).any() or (self.bond_b >= n_atoms).any():
+            raise ValueError("a bond endpoint is not an atom of its molecule")
+        if (self.bond_a == self.bond_b).any():
+            raise ValueError("a bond joins an atom to itself")
 
     def __len__(self) -> int:
         return len(self.atom_starts) - 1
