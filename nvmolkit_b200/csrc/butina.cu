@@ -442,13 +442,14 @@ namespace b200 {
 namespace {
 
 // counts (+=) and (i<j) edges of the thresholded similarity graph for this rank's tile-row groups.
-void neighborEdges(const uint32_t* d_fp, size_t n, int words, int metric, double cutoff, uint32_t groupOffset,
+void neighborEdges(const uint32_t* d_fp, size_t n, int words, const Measure& m, double cutoff, uint32_t groupOffset,
                    uint32_t groupStride, int32_t* counts, int2* edges, unsigned long long cap,
                    unsigned long long* dCursor, cudaStream_t s) {
   SimLaunch q;
   q.x = q.y     = d_fp;
   q.nX = q.nY   = n;
   q.words       = words;
+  q.measure     = m;
   q.cutoff      = cutoff;
   q.sign        = 1;
   q.rowCounts   = counts;
@@ -458,7 +459,7 @@ void neighborEdges(const uint32_t* d_fp, size_t n, int words, int metric, double
   q.edges       = edges;
   q.edgeCursor  = dCursor;
   q.edgeCap     = cap;
-  launchSimilarity(metric == B200MOL_METRIC_TANIMOTO ? kCountTanimoto : kCountCosine, q, s);
+  launchSimilarity(kCount, q, s);
 }
 
 void clusterFromEdges(int N, int32_t* counts, const int2* edges, unsigned long long nEdges, int32_t* ids,
@@ -488,7 +489,7 @@ extern "C" int b200mol_neighbor_edges(const uint32_t* d_fp, size_t n, int words,
                                       uint32_t group_offset, uint32_t group_stride, int32_t* d_counts,
                                       int32_t* d_edges, uint64_t edge_cap, uint64_t* h_n_edges, void* stream) {
   return guarded([&] {
-    B200_REQUIRE(metric == B200MOL_METRIC_TANIMOTO || metric == B200MOL_METRIC_COSINE, "unknown metric %d", metric);
+    const Measure m = measureOfMetric(metric);
     B200_REQUIRE(cutoff >= 0.0 && cutoff <= 1.0, "cutoff must be in [0, 1], got %g", cutoff);
     B200_REQUIRE(n < (1ull << 31), "too many fingerprints");
     B200_REQUIRE(group_stride >= 1 && group_offset < group_stride, "bad row-group sharding %u/%u", group_offset, group_stride);
@@ -500,7 +501,7 @@ extern "C" int b200mol_neighbor_edges(const uint32_t* d_fp, size_t n, int words,
     B200_CUDA(cudaMemsetAsync(cursor.get(), 0, sizeof(unsigned long long), s));
     {
       PhaseTimer t("neighbor_pass", s);
-      neighborEdges(d_fp, n, words, metric, cutoff, group_offset, group_stride, d_counts,
+      neighborEdges(d_fp, n, words, m, cutoff, group_offset, group_stride, d_counts,
                     reinterpret_cast<int2*>(d_edges), edge_cap, cursor.get(), s);
     }
     if (h_n_edges) {
@@ -541,7 +542,7 @@ extern "C" int b200mol_butina_fused(const uint32_t* d_fp, size_t n, int words, i
                                     int32_t* d_cluster_ids, int32_t* d_centroids, int32_t* d_n_clusters,
                                     int32_t* h_n_clusters, void* stream) {
   return guarded([&] {
-    B200_REQUIRE(metric == B200MOL_METRIC_TANIMOTO || metric == B200MOL_METRIC_COSINE, "unknown metric %d", metric);
+    measureOfMetric(metric);  // (checked first, as b200mol_neighbor_edges does)
     B200_REQUIRE(cutoff >= 0.0 && cutoff <= 1.0, "cutoff must be in [0, 1], got %g", cutoff);
     B200_REQUIRE(n < (1ull << 31), "too many fingerprints");
     cudaStream_t s = asStream(stream);

@@ -10,7 +10,7 @@
 //
 // Host loop over windows [lo, hi) of the pool, in index order. A device leader buffer holds the fingerprints and
 // popcounts of every pick so far, contiguous (it starts as the first picks). Per window:
-//   bulk     one call of the cross count pass (launchSimilarity, kCountTanimoto / kCountCosine, X = the window, Y = the
+//   bulk     one call of the cross count pass (launchSimilarity, kCount, X = the window, Y = the
 //            leader buffer, cutoff = threshold; SIMT or the wgmma u8 tile as that pass decides) counts, per item, the
 //            picks so far that cover it;
 //   select   the survivors, items with count 0 that are no first pick, compacted in index order (flags, an in-place
@@ -299,9 +299,8 @@ extern "C" int b200mol_leader_pick(const uint32_t* d_fp, size_t nPool, int words
                                    const int32_t* h_first, int nFirst, int pickSize, int32_t* d_picks, int32_t* h_n_picks,
                                    void* stream) {
   return guarded([&] {
-    B200_REQUIRE(metric == B200MOL_METRIC_TANIMOTO || metric == B200MOL_METRIC_COSINE, "unknown metric %d", metric);
-    B200_REQUIRE(words > 0 && words % 4 == 0 && words <= 128,
-                 "fingerprint width must be a multiple of 128 bits and at most 4096 bits (got %d words)", words);
+    const Measure m = measureOfMetric(metric);
+    requireFingerprintWidth(words);
     B200_REQUIRE(nPool >= 1 && nPool < (1ull << 31), "pool size must be in [1, 2^31) (got %zu)", nPool);
     B200_REQUIRE(pickSize >= 1 && static_cast<size_t>(pickSize) <= nPool, "pickSize must be in [1, pool size] (got %d, pool %zu)",
                  pickSize, nPool);
@@ -358,7 +357,7 @@ extern "C" int b200mol_leader_pick(const uint32_t* d_fp, size_t nPool, int words
 
     ResolveArgs ra{};
     ra.fp = reinterpret_cast<const uint4*>(d_fp), ra.pop = pop.get(), ra.chunks = chunks;
-    ra.cosine = metric == B200MOL_METRIC_COSINE, ra.threshold = threshold;
+    ra.cosine = m.kind == kCosine, ra.threshold = threshold;
     ra.surv = surv.get(), ra.count = count.get(), ra.nPicks = count.get() + 1, ra.pickSize = pickSize, ra.picks = d_picks;
     ra.covered = covered.get(), ra.mask = mask.get();
 
@@ -384,8 +383,8 @@ extern "C" int b200mol_leader_pick(const uint32_t* d_fp, size_t nPool, int words
         SimLaunch q;
         q.x = d_fp + lo * words, q.nX = rows;
         q.y = reinterpret_cast<const uint32_t*>(leaders.get()), q.nY = static_cast<size_t>(nPicks);
-        q.words = words, q.cutoff = threshold, q.sign = 1, q.rowCounts = counts.get();
-        launchSimilarity(metric == B200MOL_METRIC_TANIMOTO ? kCountTanimoto : kCountCosine, q, s);
+        q.words = words, q.measure = m, q.cutoff = threshold, q.sign = 1, q.rowCounts = counts.get();
+        launchSimilarity(kCount, q, s);
         g_leaderBulkPairsLast += static_cast<unsigned long long>(rows) * static_cast<unsigned long long>(nPicks);
       }
       const unsigned selGrid = static_cast<unsigned>((rows + 1 + 255) / 256);

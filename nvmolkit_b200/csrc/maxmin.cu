@@ -363,9 +363,8 @@ using namespace b200;
 extern "C" int b200mol_maxmin_pick(const uint32_t* d_fp, size_t nPool, int words, int metric, const int32_t* h_first, int nFirst,
                                    int pickSize, double threshold, int32_t* d_picks, double* d_threshold, void* stream) {
   return guarded([&] {
-    B200_REQUIRE(metric == B200MOL_METRIC_TANIMOTO || metric == B200MOL_METRIC_COSINE, "unknown metric %d", metric);
-    B200_REQUIRE(words > 0 && words % 4 == 0 && words <= 128,
-                 "fingerprint width must be a multiple of 128 bits and at most 4096 bits (got %d words)", words);
+    const Measure m = measureOfMetric(metric);
+    requireFingerprintWidth(words);
     B200_REQUIRE(nPool >= 1 && nPool < (1ull << 31), "pool size must be in [1, 2^31) (got %zu)", nPool);
     B200_REQUIRE(pickSize >= 1 && static_cast<size_t>(pickSize) <= nPool, "pickSize must be in [1, pool size] (got %d, pool %zu)",
                  pickSize, nPool);
@@ -409,7 +408,7 @@ extern "C" int b200mol_maxmin_pick(const uint32_t* d_fp, size_t nPool, int words
       gPop(stateSh ? 0 : static_cast<size_t>(blocks) * slice, s);
     PickArgs a{};
     a.fp = reinterpret_cast<const uint4*>(d_fp), a.pop = pop.get();
-    a.n = n, a.chunks = chunks, a.group = G, a.slice = slice, a.cosine = metric == B200MOL_METRIC_COSINE;
+    a.n = n, a.chunks = chunks, a.group = G, a.slice = slice, a.cosine = m.kind == kCosine;
     a.deferred = g_maxminMode == 1, a.nFirst = nFirst, a.pickSize = pickSize, a.threshold = threshold >= 0.0 ? threshold : -1.0;
     a.picks = d_picks, a.thresholdOut = d_threshold, a.slotV = slotV.get(), a.slotI = slotI.get();
     a.gBound = gBound.get(), a.gApplied = gApplied.get(), a.gPop = gPop.get();

@@ -1,4 +1,5 @@
-// Internal interface of the N x M popcount-similarity tile (used by tanimoto.cu and butina.cu).
+// Internal interface of the fingerprint-similarity stack: the measure of a call, the N x M popcount tiles that serve it
+// (tanimoto.cu: SIMT, tanimoto_tc.cu: wgmma) and the fp64 value of a pair from its integer counts.
 #pragma once
 #include <cstdint>
 
@@ -6,17 +7,46 @@
 
 namespace b200 {
 
-// What the tile kernel does with the 128x128 integer intersection counts.
+// The similarity measure of a call. A measure is only made by measureOfMetric and measureOfWeights below, the library's
+// one place that turns caller input into one.
+enum MeasureKind : int { kTanimoto = 0, kCosine = 1, kDice = 2, kTversky = 3 };
+struct Measure {
+  MeasureKind kind  = kTanimoto;
+  double      alpha = 0.0;  // Tversky's weights of the bits only in X (alpha) and only in Y (beta); Dice's are 1/2, 1/2
+  double      beta  = 0.0;
+};
+// Dice and Tversky: the value is tverskyFromCounts of the weights (kernels instantiated for these two take it so)
+__host__ __device__ constexpr bool isWeighted(MeasureKind k) { return k == kDice || k == kTversky; }
+
+// A B200MOL_METRIC_* code
+inline Measure measureOfMetric(int metric) {
+  B200_REQUIRE(metric == B200MOL_METRIC_TANIMOTO || metric == B200MOL_METRIC_COSINE, "unknown metric %d", metric);
+  return Measure{metric == B200MOL_METRIC_COSINE ? kCosine : kTanimoto};
+}
+
+// Tversky weights: finite, 0 <= alpha, beta <= 1000 (the range the float tile filters are derived for; NaN fails the
+// comparisons). (1/2, 1/2) is Dice, which runs on the Tanimoto machinery (integer ratio order, threshold table), and
+// (1, 1) Tanimoto itself: the same bits as the general expression in both cases.
+inline Measure measureOfWeights(double alpha, double beta) {
+  B200_REQUIRE(alpha >= 0.0 && alpha <= 1000.0 && beta >= 0.0 && beta <= 1000.0,
+               "Tversky weights must be finite with 0 <= alpha, beta <= 1000 (got alpha = %g, beta = %g)", alpha, beta);
+  const MeasureKind kind = alpha == 0.5 && beta == 0.5 ? kDice : alpha == 1.0 && beta == 1.0 ? kTanimoto : kTversky;
+  return Measure{kind, alpha, beta};
+}
+
+inline void requireFingerprintWidth(int words) {
+  B200_REQUIRE(words > 0 && words % 4 == 0 && words <= 128,
+               "fingerprint width must be a multiple of 128 bits and at most 4096 bits (got %d words)", words);
+}
+
+// What a tile does with the integer intersection counts of its pairs, for the call's measure (SimLaunch::measure).
+// Each tile maps (operation, measure kind) to its kernel in one place: launchSimilarity (SIMT), launchTensorImpl (wgmma).
 enum SimMode : int {
-  kMaterialiseTanimoto = 0,  // fp64 similarity matrix
-  kMaterialiseCosine   = 1,
-  kCountTanimoto       = 2,  // thresholded neighbour counts (+ optional edge list)
-  kCountCosine         = 3,
-  kListCosine          = 4,  // edges only: every pair with sim >= cutoff, possibly with false positives (tensor tile:
-                             // a float bound, unordered; the SIMT fallback runs kCountCosine and lists exactly)
-  kMaterialiseDice     = 5,  // fp64 Dice matrix, tversky(c, a, b; 1/2, 1/2)
-  kMaterialiseTversky  = 6,  // fp64 Tversky matrix for SimLaunch::tvAlpha / tvBeta
-  kListTversky         = 7,  // as kListCosine for Tversky (the SIMT fallback counts and lists exactly)
+  kMaterialise = 0,  // fp64 similarity matrix
+  kCount       = 1,  // thresholded neighbour counts (+ optional edge list); Tanimoto and Dice (atLeast only) test with an
+                     // integer threshold table, bit-exact with the fp64 predicate; cosine's runs on SIMT only
+  kList        = 2,  // cosine and Tversky, atLeast: edges only, every pair with sim >= cutoff, possibly with false
+                     // positives (tensor tile: a float bound, unordered; the SIMT tile lists exactly)
 };
 
 struct SimLaunch {
@@ -25,6 +55,7 @@ struct SimLaunch {
   size_t          nX     = 0;
   size_t          nY     = 0;
   int             words  = 0;
+  Measure         measure;
   // materialise
   double* out = nullptr;  // [nX][nY]
   // count
@@ -38,15 +69,10 @@ struct SimLaunch {
   int2*    edges       = nullptr;  // optional: neighbour pairs (i, j) appended here (symmetric: i < j)
   unsigned long long* edgeCursor = nullptr;  // device counter; entries beyond edgeCap are dropped (cursor still advances)
   unsigned long long  edgeCap    = 0;
-  // kCountTanimoto with atLeast: the table and the pre-filter of Dice, 2c / (|A| + |B|) >= cutoff, instead of Tanimoto's
-  bool   dice    = false;
-  // Tversky modes: the weights of the bits only in X (alpha) and only in Y (beta), 0 <= alpha, beta <= 1000
-  double tvAlpha = 0.0;
-  double tvBeta  = 0.0;
 };
 
 // Launch the tile kernel(s). Row popcounts and the threshold table are computed internally (stream-ordered scratch).
-void launchSimilarity(SimMode mode, const SimLaunch& p, cudaStream_t stream);
+void launchSimilarity(SimMode op, const SimLaunch& p, cudaStream_t stream);
 
 // pop[i] = popcount of row i
 void launchRowPopcount(const uint32_t* fp, size_t n, int words, int32_t* pop, cudaStream_t s);
@@ -72,6 +98,15 @@ __device__ __forceinline__ double tverskyFromCounts(int c, int a, int b, double 
                                                        static_cast<double>(c)));
 }
 
+// The value of a pair under m as every path stores it, in a kernel instantiated for the weighted measures (WEIGHTED:
+// Dice and Tversky, from m's weights) or for Tanimoto and cosine (told apart at run time: only those two reach it, so any
+// kind but Tanimoto is cosine, a test against zero).
+template <bool WEIGHTED>
+__device__ __forceinline__ double measureFromCounts(const Measure& m, int c, int a, int b) {
+  if constexpr (WEIGHTED) return tverskyFromCounts(c, a, b, m.alpha, m.beta);
+  else return simFromCounts(c, a, b, m.kind != kTanimoto);
+}
+
 // A float bound for the tile filters of the Tversky searches: can a pair with count c reach a value >= L, L a float
 // lower bound of the bar (or threshold) at least 1e-5 (relative) below it? Tested as c - L d >= 0 with
 // d = alpha_f (a - c) + (beta_f (b - c) + c) in float (fmaf), alpha_f, beta_f alpha and beta rounded to float.
@@ -86,16 +121,6 @@ __device__ __forceinline__ bool tverskyMayReach(int c, int a, int b, float alpha
   return c != 0 && fmaf(-L, d, cf) >= 0.0f;
 }
 
-// Is (alpha, beta) Dice, or Tanimoto? Those two run on the Tanimoto machinery (integer ratio order, threshold table).
-inline bool tverskyIsDice(double alpha, double beta) { return alpha == 0.5 && beta == 0.5; }
-inline bool tverskyIsTanimoto(double alpha, double beta) { return alpha == 1.0 && beta == 1.0; }
-// The weights the Tversky entry points accept: finite, 0 <= alpha, beta <= 1000 (the range the float tile filters are
-// derived for). NaN fails the comparisons.
-inline void requireTverskyWeights(double alpha, double beta) {
-  B200_REQUIRE(alpha >= 0.0 && alpha <= 1000.0 && beta >= 0.0 && beta <= 1000.0,
-               "Tversky weights must be finite with 0 <= alpha, beta <= 1000 (got alpha = %g, beta = %g)", alpha, beta);
-}
-
 // ---- top-k search: what topk.cu uses of the tensor-core tile (tanimoto_tc.cu) ----
 // one u8 (0 / 1) per bit of n fingerprints
 void launchExpandBits(const uint32_t* fp, size_t n, int words, uint8_t* out, cudaStream_t s);
@@ -103,10 +128,9 @@ bool topkTileEligible(int words);  // the tile takes widths that are multiples o
 // One pass of the expanded queries over an expanded column slab of the library (caller's indices colBase ..): for every
 // pair that could beat its row's bar[row] = {c, |A| + |B|, column, float bits of a lower bound of the value} of the row's
 // current k-th best, the caller's column index goes to cand[row][at], at = count[row]++, while at < cap. Tanimoto filters
-// with the integer ratio (.x, .y), cosine and Tversky (weights alpha, beta) with the float bound (.w).
-enum TopkMetric : int { kTopkTanimoto = 0, kTopkCosine = 1, kTopkTversky = 2 };
-void launchTopkTile(TopkMetric metric, const uint8_t* expQ, size_t nQ, const int32_t* popQ, const uint8_t* expLib, size_t nCols,
+// with the integer ratio (.x, .y), cosine and Tversky with the float bound (.w). A Dice search is Tanimoto's (topk.cu).
+void launchTopkTile(const Measure& m, const uint8_t* expQ, size_t nQ, const int32_t* popQ, const uint8_t* expLib, size_t nCols,
                     const int32_t* popCols, int words, const int4* bar, uint32_t* cand, uint32_t* count, uint32_t cap,
-                    uint32_t colBase, double alpha, double beta, cudaStream_t s);
+                    uint32_t colBase, cudaStream_t s);
 
 }  // namespace b200

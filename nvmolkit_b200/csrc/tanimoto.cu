@@ -49,7 +49,7 @@ struct TileParams {
   int2*           edges;
   unsigned long long* edgeCursor;
   unsigned long long  edgeCap;
-  double              tvAlpha, tvBeta;  // Tversky modes
+  double              alpha, beta;  // the measure's weights (Tversky kernels)
 };
 
 __global__ void rowPopcountKernel(const uint32_t* __restrict__ fp, size_t n, int words, int32_t* __restrict__ pop) {
@@ -64,48 +64,25 @@ __global__ void rowPopcountKernel(const uint32_t* __restrict__ fp, size_t n, int
 }
 
 // thresh[s] = smallest intersection c such that a pair with |A|+|B| = s is a neighbour, i.e. the fp64 predicate
-// `1.0 - sim <= cutoff` holds with sim = (c == 0 || u == 0) ? 0 : c/u, u = s - c. 0xFFFF = never.
+// `1.0 - sim <= cutoff` holds, sim the pair's value under m (Tanimoto or Dice; Dice only with atLeast). 0xFFFF = never.
 // The predicate is monotone in c, so the hot loop tests `c >= thresh[s]` with integers and stays bit-identical to the
 // fp64 evaluation a CPU makes.
 // atLeast: the threshold search's predicate `sim >= cutoff` instead (cutoff in (0, 1]: c = 0 never passes).
-__global__ void threshTableKernel(int maxS, double cutoff, int atLeast, uint16_t* __restrict__ thresh) {
+__global__ void threshTableKernel(int maxS, Measure m, double cutoff, int atLeast, uint16_t* __restrict__ thresh) {
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
   if (s > maxS) return;
-  // explicit round-to-nearest intrinsics: never contracted into an FMA, so the result is the two-rounding value a CPU
-  // computes for `1.0 - c/u`
+  // the value of a pair with |A| = c, |B| = s - c: Tanimoto's c / (s - c), Dice's RN(2c / s), whatever the popcounts
+  // are; explicit round-to-nearest intrinsics: never contracted into an FMA, so the result is the two-rounding value a
+  // CPU computes for `1.0 - sim`
   auto passes = [&](int c) {
-    const int    u   = s - c;
-    const double sim = (c == 0 || u == 0) ? 0.0 : __ddiv_rn(static_cast<double>(c), static_cast<double>(u));
+    const double sim = m.kind == kDice ? measureFromCounts<true>(m, c, c, s - c) : simFromCounts(c, c, s - c, false);
     return atLeast ? sim >= cutoff : __dsub_rn(1.0, sim) <= cutoff;
   };
-  // c/(s - c) grows with c and correctly rounded division and subtraction keep the order, so the smallest passing c is
-  // found by bisection over [0, s/2] ([1, s/2] for atLeast) (a linear scan cost 0.2 ms per table: 2048 dependent fp64
-  // divisions per thread)
+  // sim grows with c (c <= min(|A|, |B|) <= s/2) and correctly rounded operations keep the order, so the smallest passing
+  // c is found by bisection over [0, s/2] ([1, s/2] for atLeast) (a linear scan cost 0.2 ms per table: 2048 dependent
+  // fp64 divisions per thread)
   int found = 0xFFFF;
   int lo = atLeast ? 1 : 0, hi = s / 2;
-  if (hi < lo) {
-    thresh[s] = static_cast<uint16_t>(found);
-    return;
-  }
-  if (passes(hi)) {
-    while (lo < hi) {
-      const int mid = (lo + hi) >> 1;
-      if (passes(mid)) hi = mid;
-      else lo = mid + 1;
-    }
-    found = lo;
-  }
-  thresh[s] = static_cast<uint16_t>(found);
-}
-
-// The Dice table of the threshold search: thresh[s] = the smallest c with the fp64 value tverskyFromCounts(c, a, b;
-// 1/2, 1/2) >= cutoff for |A| + |B| = s (that value is RN(2c / s), whatever a and b are), 0xFFFF = never. It grows with
-// c, and c <= min(a, b) <= s / 2: bisection over [1, s / 2] as threshTableKernel does.
-__global__ void diceTableKernel(int maxS, double cutoff, uint16_t* __restrict__ thresh) {
-  const int s = blockIdx.x * blockDim.x + threadIdx.x;
-  if (s > maxS) return;
-  auto passes = [&](int c) { return tverskyFromCounts(c, c, s - c, 0.5, 0.5) >= cutoff; };
-  int  found = 0xFFFF, lo = 1, hi = s / 2;
   if (hi >= lo && passes(hi)) {
     while (lo < hi) {
       const int mid = (lo + hi) >> 1;
@@ -123,14 +100,14 @@ __device__ __forceinline__ uint4 lds128(uint32_t addr) {
   return v;
 }
 
-template <int MODE>
+// OP on the counts under measure kind K (launchSimilarity says which (OP, K) serves which call)
+template <SimMode OP, MeasureKind K>
 __global__ void __launch_bounds__(kThreads, 2)
   simTileKernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmY, const TileParams p) {
   extern __shared__ __align__(1024) uint8_t smemRaw[];
   __shared__ uint64_t                      fullBar[kStages];
   __shared__ int                           colAcc[kBN];
-  constexpr bool MATERIALISE = MODE == kMaterialiseTanimoto || MODE == kMaterialiseCosine || MODE == kMaterialiseDice ||
-                               MODE == kMaterialiseTversky;
+  constexpr bool MATERIALISE = OP == kMaterialise;
 
   // ---- tile coordinates: groups of kGroupM tile-rows sweep all tile-columns (Y tiles reused out of L2) ----
   const uint32_t perGroup = kGroupM * p.tilesN;
@@ -209,6 +186,10 @@ __global__ void __launch_bounds__(kThreads, 2)
   }
 
   // ---- epilogue ----
+  // the value of a pair (Dice's weights as constants: the kernel is compiled for them)
+  auto value = [&](int c, int a, int b) {
+    return measureFromCounts<isWeighted(K)>(K == kDice ? Measure{kDice, 0.5, 0.5} : Measure{K, p.alpha, p.beta}, c, a, b);
+  };
   const size_t row0 = static_cast<size_t>(tm) * kBM + ty * 8;
   const size_t col0 = static_cast<size_t>(tn) * kBN + tx;
   int          pa[8], pb[8];
@@ -228,18 +209,7 @@ __global__ void __launch_bounds__(kThreads, 2)
         if (col >= p.nY) continue;
         const int c = acc[i][j];
         double    v = 0.0;
-        if (c != 0) {
-          if constexpr (MODE == kMaterialiseTanimoto) {
-            v = __ddiv_rn(static_cast<double>(c), static_cast<double>(pa[i] + pb[j] - c));
-          } else if constexpr (MODE == kMaterialiseDice) {
-            v = tverskyFromCounts(c, pa[i], pb[j], 0.5, 0.5);
-          } else if constexpr (MODE == kMaterialiseTversky) {
-            v = tverskyFromCounts(c, pa[i], pb[j], p.tvAlpha, p.tvBeta);
-          } else {
-            v = __ddiv_rn(static_cast<double>(c),
-                          __dsqrt_rn(__dmul_rn(static_cast<double>(pa[i]), static_cast<double>(pb[j]))));
-          }
-        }
+        if (c != 0) v = value(c, pa[i], pb[j]);
         __stcs(orow + col, v);
       }
     }
@@ -255,16 +225,12 @@ __global__ void __launch_bounds__(kThreads, 2)
         if (p.symmetric) ok = ok && (diag ? (gr < gc) : true);
         const int c = acc[i][j];
         bool      h;
-        if constexpr (MODE == kCountTanimoto) {
+        if constexpr (K == kTanimoto) {  // (Dice too: its table)
           h = c >= static_cast<int>(__ldg(p.thresh + pa[i] + pb[j]));
-        } else if constexpr (MODE == kListTversky) {  // (the threshold search's exact list: atLeast)
-          h = tverskyFromCounts(c, pa[i], pb[j], p.tvAlpha, p.tvBeta) >= p.cutoff;
         } else {
-          const double sim =
-            (c == 0) ? 0.0
-                     : __ddiv_rn(static_cast<double>(c),
-                                 __dsqrt_rn(__dmul_rn(static_cast<double>(pa[i]), static_cast<double>(pb[j]))));
-          h = p.atLeast ? sim >= p.cutoff : (__dsub_rn(1.0, sim) <= p.cutoff);
+          const double sim = value(c, pa[i], pb[j]);
+          if constexpr (OP == kList) h = sim >= p.cutoff;  // (the threshold search's exact list: atLeast)
+          else h = p.atLeast ? sim >= p.cutoff : (__dsub_rn(1.0, sim) <= p.cutoff);
         }
         if (ok && h) hits |= 1ull << (i * 8 + j);
       }
@@ -320,11 +286,11 @@ __global__ void __launch_bounds__(kThreads, 2)
   }
 }
 
-template <int MODE>
+template <SimMode OP, MeasureKind K>
 void launchTile(const CUtensorMap& tmX, const CUtensorMap& tmY, const TileParams& tp, size_t smemBytes, cudaStream_t s) {
   static bool attrSet[kMaxDevices] = {};  // per instantiation and device
   if (!attrSet[currentDeviceSlot()]) {
-    B200_CUDA(cudaFuncSetAttribute(simTileKernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
+    B200_CUDA(cudaFuncSetAttribute(simTileKernel<OP, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
     attrSet[currentDeviceSlot()] = true;
   }
   const uint64_t groupsM = (tp.tilesM + kGroupM - 1) / kGroupM;
@@ -332,20 +298,16 @@ void launchTile(const CUtensorMap& tmX, const CUtensorMap& tmY, const TileParams
   const uint64_t myGroups = (groupsM - tp.groupOffset + tp.groupStride - 1) / tp.groupStride;
   const uint64_t blocks   = myGroups * kGroupM * tp.tilesN;
   B200_REQUIRE(blocks < (1ull << 31), "similarity grid too large (%llu tiles)", static_cast<unsigned long long>(blocks));
-  simTileKernel<MODE><<<static_cast<unsigned>(blocks), kThreads, smemBytes, s>>>(tmX, tmY, tp);
+  simTileKernel<OP, K><<<static_cast<unsigned>(blocks), kThreads, smemBytes, s>>>(tmX, tmY, tp);
   B200_LAUNCHED();
 }
 
 }  // namespace
 
-bool launchSimilarityTensor(SimMode mode, const SimLaunch& q, cudaStream_t s);
+bool launchSimilarityTensor(SimMode op, const SimLaunch& q, cudaStream_t s);
 
-void launchThreshTable(int maxS, double cutoff, bool atLeast, bool dice, uint16_t* thresh, cudaStream_t s) {
-  if (dice) {  // (a threshold search: atLeast)
-    diceTableKernel<<<(maxS + 1 + 127) / 128, 128, 0, s>>>(maxS, cutoff, thresh);
-  } else {
-    threshTableKernel<<<(maxS + 1 + 127) / 128, 128, 0, s>>>(maxS, cutoff, atLeast ? 1 : 0, thresh);
-  }
+void launchThreshTable(int maxS, const Measure& m, double cutoff, bool atLeast, uint16_t* thresh, cudaStream_t s) {
+  threshTableKernel<<<(maxS + 1 + 127) / 128, 128, 0, s>>>(maxS, m, cutoff, atLeast ? 1 : 0, thresh);
   B200_LAUNCHED();
 }
 
@@ -356,15 +318,14 @@ void launchRowPopcount(const uint32_t* fp, size_t n, int words, int32_t* pop, cu
   B200_LAUNCHED();
 }
 
-void launchSimilarity(SimMode mode, const SimLaunch& q, cudaStream_t s) {
-  B200_REQUIRE(q.words > 0 && q.words % 4 == 0 && q.words <= 128,
-               "fingerprint width must be a multiple of 128 bits and at most 4096 bits (got %d words)", q.words);
+void launchSimilarity(SimMode op, const SimLaunch& q, cudaStream_t s) {
+  requireFingerprintWidth(q.words);
   if (q.nX == 0 || q.nY == 0) return;
   B200_REQUIRE(q.nX < (1ull << 31) && q.nY < (1ull << 31), "too many fingerprints");
-  if (mode != kCountCosine && g_tensorMinPairs >= 0 &&
+  if (g_tensorMinPairs >= 0 &&
       static_cast<double>(q.nX) * static_cast<double>(q.nY) >= static_cast<double>(g_tensorMinPairs) &&
       (reinterpret_cast<uintptr_t>(q.x) & 15) == 0 && (reinterpret_cast<uintptr_t>(q.y) & 15) == 0) {
-    if (launchSimilarityTensor(mode, q, s)) return;
+    if (launchSimilarityTensor(op, q, s)) return;
   }
   B200_REQUIRE((reinterpret_cast<uintptr_t>(q.x) & 15) == 0 && (reinterpret_cast<uintptr_t>(q.y) & 15) == 0,
                "fingerprint buffers must be 16-byte aligned");
@@ -393,8 +354,8 @@ void launchSimilarity(SimMode mode, const SimLaunch& q, cudaStream_t s) {
   tp.edges      = q.edges;
   tp.edgeCursor = q.edgeCursor;
   tp.edgeCap    = q.edgeCap;
-  tp.tvAlpha    = q.tvAlpha;
-  tp.tvBeta     = q.tvBeta;
+  tp.alpha      = q.measure.alpha;
+  tp.beta       = q.measure.beta;
   if (q.symmetric) B200_REQUIRE(q.x == q.y && q.nX == q.nY, "symmetric mode needs x == y");
 
   CUtensorMap tmX, tmY;
@@ -409,25 +370,26 @@ void launchSimilarity(SimMode mode, const SimLaunch& q, cudaStream_t s) {
   tp.popX = popX.get();
   tp.popY = same ? popX.get() : popYown.get();
 
-  Scratch<uint16_t> thresh;
-  if (mode == kCountTanimoto) {
-    const int maxS = 2 * q.words * 32;
-    thresh         = Scratch<uint16_t>(maxS + 1, s);
-    launchThreshTable(maxS, q.cutoff, q.atLeast, q.dice, thresh.get(), s);
-    tp.thresh = thresh.get();
-  }
-
   const int    stages    = tp.nChunks < kStages ? tp.nChunks : kStages;
   const size_t smemBytes = static_cast<size_t>(stages) * 2 * kBM * tp.innerWords * 4 + 1024;
-  switch (mode) {
-    case kMaterialiseTanimoto: launchTile<kMaterialiseTanimoto>(tmX, tmY, tp, smemBytes, s); break;
-    case kMaterialiseCosine: launchTile<kMaterialiseCosine>(tmX, tmY, tp, smemBytes, s); break;
-    case kCountTanimoto: launchTile<kCountTanimoto>(tmX, tmY, tp, smemBytes, s); break;
-    case kCountCosine:
-    case kListCosine: launchTile<kCountCosine>(tmX, tmY, tp, smemBytes, s); break;  // (exact: lists no false positive)
-    case kMaterialiseDice: launchTile<kMaterialiseDice>(tmX, tmY, tp, smemBytes, s); break;
-    case kMaterialiseTversky: launchTile<kMaterialiseTversky>(tmX, tmY, tp, smemBytes, s); break;
-    case kListTversky: launchTile<kListTversky>(tmX, tmY, tp, smemBytes, s); break;  // (exact, as cosine's)
+  const MeasureKind kind = q.measure.kind;
+  if (op == kMaterialise) {
+    if (kind == kTanimoto) launchTile<kMaterialise, kTanimoto>(tmX, tmY, tp, smemBytes, s);
+    else if (kind == kCosine) launchTile<kMaterialise, kCosine>(tmX, tmY, tp, smemBytes, s);
+    else if (kind == kDice) launchTile<kMaterialise, kDice>(tmX, tmY, tp, smemBytes, s);
+    else launchTile<kMaterialise, kTversky>(tmX, tmY, tp, smemBytes, s);
+  } else if (kind == kCosine) {
+    launchTile<kCount, kCosine>(tmX, tmY, tp, smemBytes, s);  // count and list (exact: lists no false positive)
+  } else if (op == kList && kind == kTversky) {
+    launchTile<kList, kTversky>(tmX, tmY, tp, smemBytes, s);  // (exact, as cosine's)
+  } else {
+    B200_REQUIRE(op == kCount && kind != kTversky, "no similarity tile for operation %d, measure %d", op, kind);
+    // Tanimoto, and Dice with its own table
+    const int         maxS = 2 * q.words * 32;
+    Scratch<uint16_t> thresh(maxS + 1, s);
+    launchThreshTable(maxS, q.measure, q.cutoff, q.atLeast, thresh.get(), s);
+    tp.thresh = thresh.get();
+    launchTile<kCount, kTanimoto>(tmX, tmY, tp, smemBytes, s);
   }
 }
 
@@ -488,52 +450,42 @@ extern "C" int b200mol_free_async(void* d_ptr, void* stream) {
   });
 }
 
-static int crossImpl(SimMode mode, const uint32_t* d_a, size_t nA, const uint32_t* d_b, size_t nB, int words,
-                     double* d_out, void* stream, double alpha = 0.0, double beta = 0.0) {
-  return guarded([&] {
-    if (mode == kMaterialiseTversky) requireTverskyWeights(alpha, beta);
-    B200_REQUIRE(nA == 0 || d_a, "null fingerprint pointer");
-    if (!d_b) {
-      d_b = d_a;
-      nB  = nA;
-    }
-    B200_REQUIRE(nA == 0 || nB == 0 || d_out, "null output pointer");
-    SimLaunch q;
-    q.x     = d_a;
-    q.y     = d_b;
-    q.nX    = nA;
-    q.nY    = nB;
-    q.words = words;
-    q.out   = d_out;
-    q.tvAlpha = alpha;
-    q.tvBeta  = beta;
-    launchSimilarity(mode, q, asStream(stream));
-  });
-}
-
-// Tversky / Dice: (1/2, 1/2) is the Dice epilogue of the Tanimoto tiles, (1, 1) Tanimoto itself (the same bits as the
-// general expression in both cases), anything else the general Tversky epilogue
-static SimMode tverskyMaterialiseMode(double alpha, double beta) {
-  return tverskyIsDice(alpha, beta) ? kMaterialiseDice : tverskyIsTanimoto(alpha, beta) ? kMaterialiseTanimoto : kMaterialiseTversky;
+static void cross(const Measure& m, const uint32_t* d_a, size_t nA, const uint32_t* d_b, size_t nB, int words, double* d_out,
+                  void* stream) {
+  B200_REQUIRE(nA == 0 || d_a, "null fingerprint pointer");
+  if (!d_b) {
+    d_b = d_a;
+    nB  = nA;
+  }
+  B200_REQUIRE(nA == 0 || nB == 0 || d_out, "null output pointer");
+  SimLaunch q;
+  q.x       = d_a;
+  q.y       = d_b;
+  q.nX      = nA;
+  q.nY      = nB;
+  q.words   = words;
+  q.measure = m;
+  q.out     = d_out;
+  launchSimilarity(kMaterialise, q, asStream(stream));
 }
 
 extern "C" int b200mol_tanimoto_cross(const uint32_t* d_a, size_t nA, const uint32_t* d_b, size_t nB, int words,
                                       double* d_out, void* stream) {
-  return crossImpl(kMaterialiseTanimoto, d_a, nA, d_b, nB, words, d_out, stream);
+  return guarded([&] { cross(Measure{kTanimoto}, d_a, nA, d_b, nB, words, d_out, stream); });
 }
 extern "C" int b200mol_cosine_cross(const uint32_t* d_a, size_t nA, const uint32_t* d_b, size_t nB, int words,
                                     double* d_out, void* stream) {
-  return crossImpl(kMaterialiseCosine, d_a, nA, d_b, nB, words, d_out, stream);
+  return guarded([&] { cross(Measure{kCosine}, d_a, nA, d_b, nB, words, d_out, stream); });
 }
 extern "C" int b200mol_tversky_cross(const uint32_t* d_a, size_t nA, const uint32_t* d_b, size_t nB, int words, double alpha,
                                      double beta, double* d_out, void* stream) {
-  return crossImpl(tverskyMaterialiseMode(alpha, beta), d_a, nA, d_b, nB, words, d_out, stream, alpha, beta);
+  return guarded([&] { cross(measureOfWeights(alpha, beta), d_a, nA, d_b, nB, words, d_out, stream); });
 }
 
 extern "C" int b200mol_tanimoto_count_ge(const uint32_t* d_x, size_t nX, const uint32_t* d_y, size_t nY, int words,
                                          int metric, double cutoff, int sign, int32_t* d_counts, void* stream) {
   return guarded([&] {
-    B200_REQUIRE(metric == B200MOL_METRIC_TANIMOTO || metric == B200MOL_METRIC_COSINE, "unknown metric %d", metric);
+    const Measure m = measureOfMetric(metric);
     B200_REQUIRE(sign == 1 || sign == -1, "sign must be +1 or -1");
     B200_REQUIRE(nX == 0 || (d_x && d_counts), "null pointer");
     if (!d_y) {
@@ -546,15 +498,16 @@ extern "C" int b200mol_tanimoto_count_ge(const uint32_t* d_x, size_t nX, const u
     q.nX        = nX;
     q.nY        = nY;
     q.words     = words;
+    q.measure   = m;
     q.cutoff    = cutoff;
     q.sign      = sign;
     q.rowCounts = d_counts;
-    launchSimilarity(metric == B200MOL_METRIC_TANIMOTO ? kCountTanimoto : kCountCosine, q, asStream(stream));
+    launchSimilarity(kCount, q, asStream(stream));
   });
 }
 
 // Host-in / host-out: row blocks of A through two device buffers, D2H of block k overlapped with compute of block k+1.
-static void crossHost(SimMode mode, double alpha, double beta, const uint32_t* h_a, size_t nA, const uint32_t* h_b, size_t nB,
+static void crossHost(const Measure& m, const uint32_t* h_a, size_t nA, const uint32_t* h_b, size_t nB,
                       int words, double* h_out, size_t maxDeviceBytes) {
   if (!h_b) {
     h_b = h_a;
@@ -592,10 +545,9 @@ static void crossHost(SimMode mode, double alpha, double beta, const uint32_t* h
       q.nX    = rows;
       q.nY    = nB;
       q.words = words;
+      q.measure = m;
       q.out   = dOut[buf];
-      q.tvAlpha = alpha;
-      q.tvBeta  = beta;
-      launchSimilarity(mode, q, st[buf]);
+      launchSimilarity(kMaterialise, q, st[buf]);
       B200_CUDA(cudaMemcpyAsync(h_out + r0 * nB, dOut[buf], rows * nB * sizeof(double), cudaMemcpyDeviceToHost, st[buf]));
     }
     B200_CUDA(cudaStreamSynchronize(st[0]));
@@ -623,17 +575,10 @@ static void crossHost(SimMode mode, double alpha, double beta, const uint32_t* h
 
 extern "C" int b200mol_similarity_cross_host(const uint32_t* h_a, size_t nA, const uint32_t* h_b, size_t nB, int words,
                                              int metric, double* h_out, size_t maxDeviceBytes) {
-  return guarded([&] {
-    B200_REQUIRE(metric == B200MOL_METRIC_TANIMOTO || metric == B200MOL_METRIC_COSINE, "unknown metric %d", metric);
-    crossHost(metric == B200MOL_METRIC_TANIMOTO ? kMaterialiseTanimoto : kMaterialiseCosine, 0.0, 0.0, h_a, nA, h_b, nB, words, h_out,
-              maxDeviceBytes);
-  });
+  return guarded([&] { crossHost(measureOfMetric(metric), h_a, nA, h_b, nB, words, h_out, maxDeviceBytes); });
 }
 
 extern "C" int b200mol_tversky_cross_host(const uint32_t* h_a, size_t nA, const uint32_t* h_b, size_t nB, int words, double alpha,
                                           double beta, double* h_out, size_t maxDeviceBytes) {
-  return guarded([&] {
-    requireTverskyWeights(alpha, beta);
-    crossHost(tverskyMaterialiseMode(alpha, beta), alpha, beta, h_a, nA, h_b, nB, words, h_out, maxDeviceBytes);
-  });
+  return guarded([&] { crossHost(measureOfWeights(alpha, beta), h_a, nA, h_b, nB, words, h_out, maxDeviceBytes); });
 }

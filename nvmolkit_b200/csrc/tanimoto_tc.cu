@@ -1035,10 +1035,40 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
   if constexpr (CL) clusterSync();  // no CTA leaves while its peer may still signal its barriers
 }
 
+using TcKernel = void (*)(CUtensorMap, CUtensorMap, TcParams);
+// The tensor tile's kernel for each operation (SimMode) and measure kind (MeasureKind); nullptr: the SIMT tile serves it.
+// Dice runs on the Tanimoto machinery: its matrix from the reciprocal table, its count on Tanimoto's count tile with its
+// own threshold table and pre-filter. The count tile's cluster variants are picked in launchTensorImpl.
+const TcKernel kTensorKernels[3][4] = {
+  // Tanimoto                      cosine                           Dice                          Tversky
+  {simTensorKernel<kTcTanimoto, 0>, simTensorKernel<kTcCosine, 0>, simTensorKernel<kTcDice, 0>, simTensorKernel<kTcTversky, 0>},
+  {simTensorKernel<kTcCount, 0>, nullptr, simTensorKernel<kTcCount, 0>, nullptr},
+  {nullptr, simTensorKernel<kTcListCosine, 0>, nullptr, simTensorKernel<kTcListTversky, 0>},
+};
+// ... and of the top-k search's tile pass (a Dice search is Tanimoto's: topk.cu)
+const TcKernel kTopkKernels[4] = {simTensorKernel<kTcTopkTanimoto, 0>, simTensorKernel<kTcTopkCosine, 0>, nullptr,
+                                  simTensorKernel<kTcTopkTversky, 0>};
+constexpr size_t kSmemBytesTC = static_cast<size_t>(kStages) * kStageBytes + 1024;
+
+// Every kernel above opts in to the shared memory it runs with, once per device.
+void optInTensorKernels() {
+  static bool configured[kMaxDevices] = {};
+  if (configured[currentDeviceSlot()]) return;
+  auto optIn = [](TcKernel kernel) {
+    if (kernel) B200_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kSmemBytesTC)));
+  };
+  for (const auto& row : kTensorKernels)
+    for (TcKernel kernel : row) optIn(kernel);
+  for (TcKernel kernel : kTopkKernels) optIn(kernel);
+  optIn(simTensorKernel<kTcCount, 1>);
+  optIn(simTensorKernel<kTcCount, 3>);
+  configured[currentDeviceSlot()] = true;
+}
+
 }  // namespace
 
 void launchRowPopcount(const uint32_t* fp, size_t n, int words, int32_t* pop, cudaStream_t s);
-void launchThreshTable(int maxS, double cutoff, bool atLeast, bool dice, uint16_t* thresh, cudaStream_t s);
+void launchThreshTable(int maxS, const Measure& m, double cutoff, bool atLeast, uint16_t* thresh, cudaStream_t s);
 
 // A fingerprint set in popcount order: row i of fp is the caller's row perm[i], pop its popcount; ascending, ties in the
 // caller's order (CUB's radix sort is stable), so the same input always gives the same order.
@@ -1093,21 +1123,23 @@ static void resetWalkCounters(cudaStream_t s) {
 }
 unsigned long long readWalkCounter(int i) { return readDeviceCounter(g_walkedDev, i); }
 
-static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, int superS, int superC, bool ordered,
+static bool launchTensorImpl(SimMode op, const SimLaunch& q, cudaStream_t s, int superS, int superC, bool ordered,
                              bool* overflow, unsigned long long* pilotCand = nullptr, double* pilotPairs = nullptr);
 
-// Count / materialise modes on tensor cores. Returns false when the problem shape is not eligible (caller uses the SIMT tile).
-bool launchSimilarityTensor(SimMode mode, const SimLaunch& q, cudaStream_t s) {
+// The operations on tensor cores. Returns false when the operation, measure or problem shape is not eligible (caller uses
+// the SIMT tile).
+bool launchSimilarityTensor(SimMode op, const SimLaunch& q, cudaStream_t s) {
+  if (!kTensorKernels[op][q.measure.kind]) return false;
   // Superposition serves the Butina passes (symmetric and / or with an edge list): they synchronise for their edge
   // total anyway, and the superposed pass needs one host read of its candidate count. The plain thresholded count
   // (b200mol_tanimoto_count_ge) stays asynchronous on the unsuperposed tile.
-  const bool graphPass = mode == kCountTanimoto && (q.symmetric || q.edges != nullptr);
+  const bool graphPass = op == kCount && (q.symmetric || q.edges != nullptr);
   if (!graphPass || g_superpose * g_superposeCols == 1) {
     if (graphPass) {
       g_superposeLast = 1;
       resetWalkCounters(s);
     }
-    return launchTensorImpl(mode, q, s, 1, 1, false, nullptr);
+    return launchTensorImpl(op, q, s, 1, 1, false, nullptr);
   }
   int S = g_superpose, C = g_superposeCols;
   // How far superposition pays depends on the data: the sum of S C random intersections must stay below the threshold
@@ -1142,7 +1174,7 @@ bool launchSimilarityTensor(SimMode mode, const SimLaunch& q, cudaStream_t s) {
     for (int c = C; c >= 1; c >>= 1) {
       unsigned long long got = 0;
       double             left = pilotPairs;
-      if (!launchTensorImpl(mode, pilot, s, S, c, true, nullptr, &got, &left)) return false;
+      if (!launchTensorImpl(op, pilot, s, S, c, true, nullptr, &got, &left)) return false;
       const double passPairs = totalPairs * (left / pilotPairs);
       if (bestT < 0.0) bestT = passPairs * tPair;
       const double tPass = passPairs / (S * c) * tPair;
@@ -1155,7 +1187,7 @@ bool launchSimilarityTensor(SimMode mode, const SimLaunch& q, cudaStream_t s) {
   resetWalkCounters(s);
   while (S * C > 1) {
     bool overflow = false;
-    if (!launchTensorImpl(mode, q, s, S, C, true, &overflow)) return false;
+    if (!launchTensorImpl(op, q, s, S, C, true, &overflow)) return false;
     g_superposeLast = S * C;
     if (!overflow) return true;  // else: the candidate list overflowed (dense graph / loose cutoff), nothing was counted yet
     if (C > 1) C = 1;            // second chance: rows only
@@ -1164,7 +1196,7 @@ bool launchSimilarityTensor(SimMode mode, const SimLaunch& q, cudaStream_t s) {
   // The unsuperposed pass that completes a superposed one stays in popcount order: a sharded call's ranks decide their
   // fallbacks independently, and their row groups must still be groups of ONE order for the union to be every pair once.
   g_superposeLast = 1;
-  return launchTensorImpl(mode, q, s, 1, 1, true, nullptr);
+  return launchTensorImpl(op, q, s, 1, 1, true, nullptr);
 }
 
 // ordered (graph passes of the count mode): run on the fingerprints in popcount order and map the results back. Every
@@ -1188,15 +1220,15 @@ static double bandPairs(const TcParams& p, const uint32_t* band, size_t nX, size
   return total;
 }
 
-static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, int superS, int superC, bool ordered,
+static bool launchTensorImpl(SimMode op, const SimLaunch& q, cudaStream_t s, int superS, int superC, bool ordered,
                              bool* overflow, unsigned long long* pilotCand, double* pilotPairs) {
-  if (mode == kCountCosine) return false;
+  const MeasureKind kind = q.measure.kind;
   const int bits = q.words * 32;
   if (bits % kTK != 0 || bits > 4096) return false;
   const bool same = (q.x == q.y && q.nX == q.nY);
   if (q.symmetric && !same) return false;
 
-  const bool count    = mode == kCountTanimoto;
+  const bool count    = op == kCount;
   const int  rowBytes = bits;  // one byte per bit of the fingerprint
   if (!count) superS = superC = 1;  // only the count mode verifies
   const bool   super  = superS * superC > 1;
@@ -1227,7 +1259,7 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
   p.out       = q.out;
   p.outVec    = (q.nY % 2 == 0 && (reinterpret_cast<uintptr_t>(q.out) & 15) == 0) ? 1 : 0;
   const int  recipLen = 2 * bits;
-  const bool useRecip = mode == kMaterialiseTanimoto || mode == kMaterialiseDice;
+  const bool useRecip = op == kMaterialise && (kind == kTanimoto || kind == kDice);
   Scratch<double> recip(useRecip ? static_cast<size_t>(recipLen) + 1 : 0, s);
   if (useRecip) {
     recipTableKernel<<<(recipLen + 256) / 256, 256, 0, s>>>(recip.get(), recipLen);
@@ -1238,15 +1270,15 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
     // a pair passes iff 1 - c / (|A| + |B| - c) <= cutoff, i.e. c >= alpha (|A| + |B|) - or, for the threshold search's
     // c / (|A| + |B| - c) >= t, with alpha = t / (1 + t); the pre-filter's alpha is rounded DOWN (and its products
     // too), so it never rejects what the exact fp64 table accepts. Dice's 2c / (|A| + |B|) >= t needs c >= (t / 2) (|A| + |B|).
-    const double a  = q.atLeast ? (q.dice ? q.cutoff / 2.0 : q.cutoff / (1.0 + q.cutoff))
+    const double a  = q.atLeast ? (kind == kDice ? q.cutoff / 2.0 : q.cutoff / (1.0 + q.cutoff))
                                 : q.cutoff < 2.0 ? (1.0 - q.cutoff) / (2.0 - q.cutoff) : 0.0;
     float        af = static_cast<float>(a);
     if (static_cast<double>(af) > a) af = nextafterf(af, -1.0f);
     p.alpha = nextafterf(af, -1.0f);  // (one more ulp: fp64 rounding inside the table's predicate)
     if (p.alpha < 0.0f) p.alpha = 0.0f;
   }
-  p.tvAlpha = q.tvAlpha, p.tvBeta = q.tvBeta;
-  p.tvAlphaF = static_cast<float>(q.tvAlpha), p.tvBetaF = static_cast<float>(q.tvBeta);
+  p.tvAlpha = q.measure.alpha, p.tvBeta = q.measure.beta;
+  p.tvAlphaF = static_cast<float>(q.measure.alpha), p.tvBetaF = static_cast<float>(q.measure.beta);
 
   Scratch<int32_t> popX(q.nX, s), popYown(same ? 0 : q.nY, s);
   launchRowPopcount(q.x, q.nX, q.words, popX.get(), s);
@@ -1298,7 +1330,7 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
   // tile of a CTA pair may lie one tile row past the end)
   const size_t  rowsPad = (static_cast<size_t>(p.tilesM) + 1) * kTM, colsPad = static_cast<size_t>(p.tilesN) * kTN;
   Scratch<int2> rowMeta(rowsPad, s), colMeta(colsPad, s);
-  if (mode == kListCosine || mode == kListTversky) {
+  if (op == kList) {
     // the list tile's bound: tLow = t (1 - 1e-5), rounded down
     float tLow = static_cast<float>(q.cutoff * (1.0 - 1e-5));
     if (static_cast<double>(tLow) > q.cutoff * (1.0 - 1e-5)) tLow = nextafterf(tLow, 0.0f);
@@ -1332,8 +1364,8 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
   }
   const int         maxS = 2 * bits;
   Scratch<uint16_t> thresh(static_cast<size_t>(maxS + 1), s);
-  if (mode == kCountTanimoto) {
-    launchThreshTable(maxS, q.cutoff, q.atLeast, q.dice, thresh.get(), s);
+  if (count) {
+    launchThreshTable(maxS, q.measure, q.cutoff, q.atLeast, thresh.get(), s);
     p.threshLen = maxS + 1;
   }
   p.thresh = thresh.get();
@@ -1363,23 +1395,9 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
   makeTensorMap2D(&tmB, expY, nSuperY, rowBytes, cluster ? kTN / 2 : kTN, kTK, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1);
 
   static_assert(kMaxChunksStat * kABytes + kStagesStat * kBBytes == kStages * kStageBytes, "both layouts take the same shared memory");
-  const size_t smemBytes = static_cast<size_t>(kStages) * kStageBytes + 1024;
-  static bool configured[kMaxDevices] = {};
-  auto optIn = [&](auto kernel) {
-    B200_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smemBytes)));
-  };
-  if (!configured[currentDeviceSlot()]) {
-    optIn(simTensorKernel<kTcCount, 0>);
-    optIn(simTensorKernel<kTcCount, 1>);
-    optIn(simTensorKernel<kTcCount, 3>);
-    optIn(simTensorKernel<kTcTanimoto, 0>);
-    optIn(simTensorKernel<kTcCosine, 0>);
-    optIn(simTensorKernel<kTcListCosine, 0>);
-    optIn(simTensorKernel<kTcDice, 0>);
-    optIn(simTensorKernel<kTcTversky, 0>);
-    optIn(simTensorKernel<kTcListTversky, 0>);
-    configured[currentDeviceSlot()] = true;
-  }
+  const size_t smemBytes = kSmemBytesTC;
+  optInTensorKernels();
+  const TcKernel kernel = stationary ? simTensorKernel<kTcCount, 3> : cluster ? simTensorKernel<kTcCount, 1> : kTensorKernels[op][kind];
   // units a call owns: tiles, or vertical tile pairs (same enumeration as the kernel's UnitWalk)
   auto unitsOf = [&](const TcParams& pk) -> uint64_t {
     return stationary ? countUnits<true, kRunStat>(pk, bandH) : cluster ? countUnits<true>(pk, bandH) : countUnits<false>(pk, bandH);
@@ -1403,17 +1421,15 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
       cfg.numAttrs         = 1;
       cfg.gridDim          = dim3(2);
       int maxClusters = 0;
-      if (stationary) B200_CUDA(cudaOccupancyMaxActiveClusters(&maxClusters, simTensorKernel<kTcCount, 3>, &cfg));
-      else B200_CUDA(cudaOccupancyMaxActiveClusters(&maxClusters, simTensorKernel<kTcCount, 1>, &cfg));
+      B200_CUDA(cudaOccupancyMaxActiveClusters(&maxClusters, kernel, &cfg));
       B200_REQUIRE(maxClusters >= 1, "no CTA pair fits the device");
       uint64_t pairs = maxClusters;  // persistent: one resident cluster per schedulable SM pair
       if (pairs > units) pairs = units;
       cfg.gridDim = dim3(static_cast<unsigned>(2 * pairs));
-      if (stationary) B200_CUDA(cudaLaunchKernelEx(&cfg, simTensorKernel<kTcCount, 3>, tmA, tmB, pk));
-      else B200_CUDA(cudaLaunchKernelEx(&cfg, simTensorKernel<kTcCount, 1>, tmA, tmB, pk));
+      B200_CUDA(cudaLaunchKernelEx(&cfg, kernel, tmA, tmB, pk));
     } else {
       const int grid = static_cast<int>(std::min<uint64_t>(static_cast<uint64_t>(smCount()), units));
-      simTensorKernel<kTcCount, 0><<<grid, kThreadsTC, smemBytes, s>>>(tmA, tmB, pk);
+      kernel<<<grid, kThreadsTC, smemBytes, s>>>(tmA, tmB, pk);
     }
     B200_LAUNCHED();
     return true;
@@ -1477,8 +1493,8 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
       qk.groupOffset = p.groupOffset + static_cast<uint32_t>(redo[r]) * p.groupStride;
       qk.groupStride = static_cast<uint32_t>(K) * p.groupStride;
       bool again     = false;
-      if (!launchTensorImpl(mode, qk, s, superS, 1, true, &again)) return false;
-      if (again && !launchTensorImpl(mode, qk, s, 1, 1, true, nullptr)) return false;
+      if (!launchTensorImpl(op, qk, s, superS, 1, true, &again)) return false;
+      if (again && !launchTensorImpl(op, qk, s, 1, 1, true, nullptr)) return false;
     }
     return true;
   }
@@ -1486,7 +1502,7 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
   if (unitsOf(p) == 0) return true;  // nothing owned by this rank (more ranks than row groups)
   int blocks = smCount();
   if (static_cast<uint64_t>(blocks) > unitsOf(p)) blocks = static_cast<int>(unitsOf(p));
-  if (mode == kCountTanimoto) {
+  if (count) {
     {
       PhaseTimer t("neighbor_pass_tc", s);
       launchCount(p);
@@ -1497,26 +1513,11 @@ static bool launchTensorImpl(SimMode mode, const SimLaunch& q, cudaStream_t s, i
                                          q.edgeCursor, q.edgeCap);
       B200_LAUNCHED();
     }
-  } else if (mode == kListCosine) {
-    PhaseTimer t("threshold_list_tc", s);
-    simTensorKernel<kTcListCosine, 0><<<blocks, kThreadsTC, smemBytes, s>>>(tmA, tmB, p);
-  } else if (mode == kListTversky) {
-    PhaseTimer t("threshold_list_tc", s);
-    simTensorKernel<kTcListTversky, 0><<<blocks, kThreadsTC, smemBytes, s>>>(tmA, tmB, p);
-  } else if (mode == kMaterialiseDice) {
-    PhaseTimer t("cross_tc", s);
-    simTensorKernel<kTcDice, 0><<<blocks, kThreadsTC, smemBytes, s>>>(tmA, tmB, p);
-  } else if (mode == kMaterialiseTversky) {
-    PhaseTimer t("cross_tc", s);
-    simTensorKernel<kTcTversky, 0><<<blocks, kThreadsTC, smemBytes, s>>>(tmA, tmB, p);
-  } else if (mode == kMaterialiseTanimoto) {
-    PhaseTimer t("cross_tc", s);
-    simTensorKernel<kTcTanimoto, 0><<<blocks, kThreadsTC, smemBytes, s>>>(tmA, tmB, p);
   } else {
-    PhaseTimer t("cross_tc", s);
-    simTensorKernel<kTcCosine, 0><<<blocks, kThreadsTC, smemBytes, s>>>(tmA, tmB, p);
+    PhaseTimer t(op == kList ? "threshold_list_tc" : "cross_tc", s);
+    kernel<<<blocks, kThreadsTC, smemBytes, s>>>(tmA, tmB, p);
+    B200_LAUNCHED();
   }
-  if (mode != kCountTanimoto) B200_LAUNCHED();
   if (super) {
     // the one host read of a superposed pass: how many candidates (the callers synchronise for their edge total anyway)
     unsigned long long nCand = 0;
@@ -1558,10 +1559,12 @@ void launchExpandBits(const uint32_t* fp, size_t n, int words, uint8_t* out, cud
 
 bool topkTileEligible(int words) { return (words * 32) % kTK == 0 && words * 32 <= 4096; }
 
-void launchTopkTile(TopkMetric metric, const uint8_t* expQ, size_t nQ, const int32_t* popQ, const uint8_t* expLib, size_t nCols,
+void launchTopkTile(const Measure& m, const uint8_t* expQ, size_t nQ, const int32_t* popQ, const uint8_t* expLib, size_t nCols,
                     const int32_t* popCols, int words, const int4* bar, uint32_t* cand, uint32_t* count, uint32_t cap,
-                    uint32_t colBase, double alpha, double beta, cudaStream_t s) {
-  const bool cosine = metric == kTopkCosine;
+                    uint32_t colBase, cudaStream_t s) {
+  const TcKernel kernel = kTopkKernels[m.kind];
+  B200_REQUIRE(kernel, "no top-k tile for measure %d", m.kind);
+  const bool cosine = m.kind == kCosine;
   const int rowBytes = words * 32;
   TcParams  p{};
   p.n           = static_cast<uint32_t>(nQ);
@@ -1579,8 +1582,8 @@ void launchTopkTile(TopkMetric metric, const uint8_t* expQ, size_t nQ, const int
   p.topkCount   = count;
   p.topkCap     = cap;
   p.topkColBase = colBase;
-  p.tvAlphaF    = static_cast<float>(alpha);
-  p.tvBetaF     = static_cast<float>(beta);
+  p.tvAlphaF    = static_cast<float>(m.alpha);
+  p.tvBetaF     = static_cast<float>(m.beta);
   const size_t  rowsPad = static_cast<size_t>(p.tilesM) * kTM, colsPad = static_cast<size_t>(p.tilesN) * kTN;
   Scratch<int2> rowMeta(rowsPad, s), colMeta(colsPad, s);
   topkMetaKernel<<<static_cast<unsigned>((rowsPad + 255) / 256), 256, 0, s>>>(popQ, nQ, rowsPad, 0, rowMeta.get());
@@ -1592,20 +1595,11 @@ void launchTopkTile(TopkMetric metric, const uint8_t* expQ, size_t nQ, const int
   CUtensorMap tmA, tmB;
   makeTensorMap2D(&tmA, expQ, nQ, rowBytes, kTM, kTK, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1);
   makeTensorMap2D(&tmB, expLib, nCols, rowBytes, kTN, kTK, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1);
-  const size_t smemBytes = static_cast<size_t>(kStages) * kStageBytes + 1024;
-  static bool  configured[kMaxDevices] = {};
-  if (!configured[currentDeviceSlot()]) {
-    B200_CUDA(cudaFuncSetAttribute(simTensorKernel<kTcTopkTanimoto, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smemBytes)));
-    B200_CUDA(cudaFuncSetAttribute(simTensorKernel<kTcTopkCosine, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smemBytes)));
-    B200_CUDA(cudaFuncSetAttribute(simTensorKernel<kTcTopkTversky, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smemBytes)));
-    configured[currentDeviceSlot()] = true;
-  }
+  optInTensorKernels();
   const uint64_t units = countUnits<false>(p, nullptr);
   if (units == 0) return;
   const int grid = static_cast<int>(std::min<uint64_t>(static_cast<uint64_t>(smCount()), units));
-  if (cosine) simTensorKernel<kTcTopkCosine, 0><<<grid, kThreadsTC, smemBytes, s>>>(tmA, tmB, p);
-  else if (metric == kTopkTversky) simTensorKernel<kTcTopkTversky, 0><<<grid, kThreadsTC, smemBytes, s>>>(tmA, tmB, p);
-  else simTensorKernel<kTcTopkTanimoto, 0><<<grid, kThreadsTC, smemBytes, s>>>(tmA, tmB, p);
+  kernel<<<grid, kThreadsTC, kSmemBytesTC, s>>>(tmA, tmB, p);
   B200_LAUNCHED();
 }
 

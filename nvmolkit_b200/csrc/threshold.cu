@@ -1,24 +1,25 @@
 // Threshold (range) similarity search on packed fingerprints: b200mol_similarity_threshold.
 //
-// Contract. Row q of the CSR result lists exactly the columns j for which the fp64 value b200mol_tanimoto_cross /
-// b200mol_cosine_cross store for (q, j) is >= t (0 < t <= 1), in ascending column order, with those values. Without a
-// library the queries are searched against themselves, self-matches included.
+// Contract. Row q of the CSR result lists exactly the columns j for which the fp64 value the matrix of the measure
+// (b200mol_tanimoto_cross, b200mol_cosine_cross, b200mol_tversky_cross) stores for (q, j) is >= t (0 < t <= 1), in
+// ascending column order, with those values. Without a library the queries are searched against themselves,
+// self-matches included.
 //
 // The pass lists pairs, the assembly makes them exact and orders them:
-//   pass      Tanimoto: the thresholded graph pass (launchSimilarity, kCountTanimoto with atLeast and an edge list):
+//   pass      Tanimoto: the thresholded graph pass (launchSimilarity, kCount with atLeast and an edge list):
 //             X = queries, Y = library; symmetric (pairs i < j only, half the tiles) for a self search. On the wgmma tile it
 //             runs superposed and in popcount order with the popcount band, as the Butina pass does, and lists exactly the
 //             pairs whose integer threshold-table test passes - the fp64 predicate s >= t, bit for bit.
-//             Cosine: the list mode kListCosine - on the wgmma tile every pair that passes a float bound with a margin
+//             Cosine: the list operation kList - on the wgmma tile every pair that passes a float bound with a margin
 //             (a superset of the answer, unordered); on the SIMT tile the exact fp64 test.
 //             Dice (b200mol_tversky_threshold at (1/2, 1/2)): Tanimoto's graph pass with the Dice table and pre-filter.
-//             Tversky: the list mode kListTversky, a float bound like cosine's. With alpha != beta the value is not
+//             Tversky: kList as well, a float bound like cosine's. With alpha != beta the value is not
 //             symmetric, so a self search runs the full (non-symmetric) pass over the set against itself.
 //             All run on SIMT or on the tensor cores as "similarity_tensor_min_pairs" decides.
 //   read      the listed-pair total, the pairs the re-count keeps and the non-empty queries: the one host read of an attempt.
 //             A list longer than its buffer is rerun once into a buffer of the exact size.
-//   assembly  (a) every listed pair is re-counted by popcount and its value computed with simFromCounts (the matrix's
-//             expression), kept iff value >= t [before the read, so the read already knows the result size];
+//   assembly  (a) every listed pair is re-counted by popcount and its value computed with measureFromCounts (the
+//             matrix's expression), kept iff value >= t [before the read, so the read already knows the result size];
 //             (b) kept pairs become 64-bit keys (row << colBits | column) with the value as payload, mirrored in a self
 //             search, plus the diagonal (s(q, q) = 1 for a non-empty fingerprint; an empty one is at 0 < t);
 //             (c) one CUB radix sort over the key bits in use;
@@ -39,12 +40,11 @@ constexpr int kRecountLanes = 8;  // lanes per listed pair in the re-count (up t
 // stat[0] listed pairs (the pass's edge cursor), [1] pairs the re-count keeps, [2] non-empty queries, [3] fill cursor
 
 // (a): one group of kRecountLanes lanes per listed pair (i, j) in the caller's indices; a dropped pair gets i = -1.
-// TV: the value is tverskyFromCounts(alpha, beta) (Dice too), else Tanimoto / cosine.
-template <bool TV>
+template <bool WEIGHTED>
 __global__ void __launch_bounds__(256) recountKernel(const uint32_t* __restrict__ x, const uint32_t* __restrict__ y, int words,
-                                                     const int32_t* __restrict__ popX, const int32_t* __restrict__ popY, int cosine,
-                                                     double alpha, double beta, double t, int2* list, unsigned long long cap,
-                                                     double* __restrict__ vals, unsigned long long* stat) {
+                                                     const int32_t* __restrict__ popX, const int32_t* __restrict__ popY, Measure m,
+                                                     double t, int2* list, unsigned long long cap, double* __restrict__ vals,
+                                                     unsigned long long* stat) {
   const unsigned long long n = min(stat[0], cap);
   const int                lane = threadIdx.x & 31, gl = lane % kRecountLanes, chunks = words / 4;
   const unsigned long long step = static_cast<unsigned long long>(gridDim.x) * blockDim.x / kRecountLanes;
@@ -67,7 +67,7 @@ __global__ void __launch_bounds__(256) recountKernel(const uint32_t* __restrict_
     for (int o = kRecountLanes / 2; o; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
     bool keep = false;
     if (have && gl == 0) {
-      const double v = TV ? tverskyFromCounts(c, popX[ij.x], popY[ij.y], alpha, beta) : simFromCounts(c, popX[ij.x], popY[ij.y], cosine != 0);
+      const double v = measureFromCounts<WEIGHTED>(m, c, popX[ij.x], popY[ij.y]);
       keep           = v >= t;
       vals[e]        = v;
       if (!keep) list[e].x = -1;
@@ -87,7 +87,7 @@ __global__ void nonEmptyKernel(const int32_t* __restrict__ pop, size_t n, unsign
 // cursor; item e < listed is a listed pair, e >= listed the diagonal entry of query e - listed
 __global__ void __launch_bounds__(256) fillKernel(const int2* __restrict__ list, const double* __restrict__ vals,
                                                   unsigned long long listed, int symmetric, const int32_t* __restrict__ popX,
-                                                  size_t nX, int cosine, int colBits, unsigned long long* __restrict__ keys,
+                                                  size_t nX, MeasureKind kind, int colBits, unsigned long long* __restrict__ keys,
                                                   double* __restrict__ out, unsigned long long* stat) {
   const unsigned long long total = listed + (symmetric ? nX : 0);
   const int                lane  = threadIdx.x & 31;
@@ -110,7 +110,9 @@ __global__ void __launch_bounds__(256) fillKernel(const int2* __restrict__ list,
       const size_t i = static_cast<size_t>(e - listed);
       const int    a = popX[i];
       if (a > 0) {
-        v  = simFromCounts(a, a, a, cosine != 0);  // 1.0, as the matrix's diagonal
+        // 1.0, the matrix's diagonal: every measure's value is exactly 1 at c = |A| = |B| (cosine's c / sqrt(c c) too, so
+        // the test is against Tanimoto alone, as in the recount)
+        v  = simFromCounts(a, a, a, kind != kTanimoto);
         k0 = (static_cast<unsigned long long>(i) << colBits) | static_cast<unsigned long long>(i);
         m  = 1;
       }
@@ -160,12 +162,8 @@ unsigned blocksFor(unsigned long long items, int perBlock) {
                                                                                             static_cast<unsigned long long>(smCount()) * 16)));
 }
 
-enum Measure : int { kTanimoto, kCosine, kDice, kTversky };
-
-void thresholdSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t nLib, bool self, int words, Measure measure,
-                     double alpha, double beta, double t, int64_t* indptr, int32_t* indices, double* values, uint64_t cap,
-                     uint64_t* hNnz, cudaStream_t s) {
-  const bool cosine = measure == kCosine, tv = measure == kDice || measure == kTversky;
+void thresholdSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t nLib, bool self, int words, const Measure& m, double t,
+                     int64_t* indptr, int32_t* indices, double* values, uint64_t cap, uint64_t* hNnz, cudaStream_t s) {
   Scratch<int32_t> popQ(nQ, s), popLibOwn(self ? 0 : nLib, s), counts(nQ, s);
   launchRowPopcount(q, nQ, words, popQ.get(), s);
   if (!self) launchRowPopcount(lib, nLib, words, popLibOwn.get(), s);
@@ -194,6 +192,7 @@ void thresholdSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t n
       p.nX        = nQ;
       p.nY        = nLib;
       p.words     = words;
+      p.measure   = m;
       p.cutoff    = t;
       p.atLeast   = true;
       p.rowCounts = counts.get();
@@ -201,22 +200,15 @@ void thresholdSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t n
       p.edges     = list.get();
       p.edgeCursor = stat.get();
       p.edgeCap   = listCap;
-      p.dice      = measure == kDice;
-      p.tvAlpha   = alpha;
-      p.tvBeta    = beta;
       B200_CUDA(cudaMemsetAsync(counts.get(), 0, nQ * sizeof(int32_t), s));
-      launchSimilarity(cosine ? kListCosine : measure == kTversky ? kListTversky : kCountTanimoto, p, s);
+      // Tanimoto and Dice count with their exact tables; cosine and Tversky list by a float bound
+      launchSimilarity(m.kind == kCosine || m.kind == kTversky ? kList : kCount, p, s);
     }
     {
       PhaseTimer timer("threshold_recount", s);
       const unsigned blocks = blocksFor(listCap * kRecountLanes, 256);
-      if (tv) {
-        recountKernel<true><<<blocks, 256, 0, s>>>(q, lib, words, popQ.get(), popLib, 0, alpha, beta, t, list.get(), listCap, vals.get(),
-                                                   stat.get());
-      } else {
-        recountKernel<false><<<blocks, 256, 0, s>>>(q, lib, words, popQ.get(), popLib, cosine ? 1 : 0, 0.0, 0.0, t, list.get(), listCap,
-                                                    vals.get(), stat.get());
-      }
+      const auto     recount = isWeighted(m.kind) ? recountKernel<true> : recountKernel<false>;
+      recount<<<blocks, 256, 0, s>>>(q, lib, words, popQ.get(), popLib, m, t, list.get(), listCap, vals.get(), stat.get());
       B200_LAUNCHED();
       if (self) {
         nonEmptyKernel<<<static_cast<unsigned>((nQ + 255) / 256), 256, 0, s>>>(popQ.get(), nQ, stat.get());
@@ -241,7 +233,7 @@ void thresholdSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t n
   Scratch<double>             valsIn(nnz, s);
   if (listed + (self ? nQ : 0) > 0) {
     fillKernel<<<blocksFor(listed + (self ? nQ : 0), 256), 256, 0, s>>>(list.get(), vals.get(), listed, self ? 1 : 0, popQ.get(), nQ,
-                                                                        cosine ? 1 : 0, colBits, keysIn.get(), valsIn.get(), stat.get());
+                                                                        m.kind, colBits, keysIn.get(), valsIn.get(), stat.get());
     B200_LAUNCHED();
   }
   if (nnz) {
@@ -261,11 +253,10 @@ void thresholdSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t n
 
 using namespace b200;
 
-static void thresholdEntry(const uint32_t* d_q, size_t nQ, const uint32_t* d_lib, size_t nLib, int words, Measure measure, double alpha,
-                           double beta, double threshold, int64_t* d_indptr, int32_t* d_indices, double* d_values, uint64_t cap,
-                           uint64_t* h_nnz, void* stream) {
-  B200_REQUIRE(words > 0 && words % 4 == 0 && words <= 128,
-               "fingerprint width must be a multiple of 128 bits and at most 4096 bits (got %d words)", words);
+static void thresholdEntry(const uint32_t* d_q, size_t nQ, const uint32_t* d_lib, size_t nLib, int words, const Measure& m,
+                           double threshold, int64_t* d_indptr, int32_t* d_indices, double* d_values, uint64_t cap, uint64_t* h_nnz,
+                           void* stream) {
+  requireFingerprintWidth(words);
   B200_REQUIRE(threshold > 0.0 && threshold <= 1.0, "threshold must be in (0, 1] (got %g)", threshold);
   const bool self = d_lib == nullptr;
   if (self) nLib = nQ;
@@ -282,28 +273,23 @@ static void thresholdEntry(const uint32_t* d_q, size_t nQ, const uint32_t* d_lib
     return;
   }
   // an asymmetric measure has no symmetric pass: the set is searched against itself as a library, every pair in full
-  const bool symmetricPass = self && !(measure == kTversky && alpha != beta);
-  thresholdSearch(d_q, nQ, self ? d_q : d_lib, nLib, symmetricPass, words, measure, alpha, beta, threshold, d_indptr, d_indices,
-                  d_values, cap, h_nnz, s);
+  const bool symmetricPass = self && !(m.kind == kTversky && m.alpha != m.beta);
+  thresholdSearch(d_q, nQ, self ? d_q : d_lib, nLib, symmetricPass, words, m, threshold, d_indptr, d_indices, d_values, cap, h_nnz, s);
 }
 
 extern "C" int b200mol_similarity_threshold(const uint32_t* d_q, size_t nQ, const uint32_t* d_lib, size_t nLib, int words, int metric,
                                             double threshold, int64_t* d_indptr, int32_t* d_indices, double* d_values, uint64_t cap,
                                             uint64_t* h_nnz, void* stream) {
   return guarded([&] {
-    B200_REQUIRE(metric == B200MOL_METRIC_TANIMOTO || metric == B200MOL_METRIC_COSINE, "unknown metric %d", metric);
-    thresholdEntry(d_q, nQ, d_lib, nLib, words, metric == B200MOL_METRIC_COSINE ? kCosine : kTanimoto, 0.0, 0.0, threshold, d_indptr,
-                   d_indices, d_values, cap, h_nnz, stream);
+    thresholdEntry(d_q, nQ, d_lib, nLib, words, measureOfMetric(metric), threshold, d_indptr, d_indices, d_values, cap, h_nnz, stream);
   });
 }
 
-// Tversky / Dice: (1/2, 1/2) runs Tanimoto's graph pass with the Dice table, (1, 1) is Tanimoto itself
 extern "C" int b200mol_tversky_threshold(const uint32_t* d_q, size_t nQ, const uint32_t* d_lib, size_t nLib, int words, double alpha,
                                          double beta, double threshold, int64_t* d_indptr, int32_t* d_indices, double* d_values,
                                          uint64_t cap, uint64_t* h_nnz, void* stream) {
   return guarded([&] {
-    requireTverskyWeights(alpha, beta);
-    const Measure m = tverskyIsDice(alpha, beta) ? kDice : tverskyIsTanimoto(alpha, beta) ? kTanimoto : kTversky;
-    thresholdEntry(d_q, nQ, d_lib, nLib, words, m, alpha, beta, threshold, d_indptr, d_indices, d_values, cap, h_nnz, stream);
+    thresholdEntry(d_q, nQ, d_lib, nLib, words, measureOfWeights(alpha, beta), threshold, d_indptr, d_indices, d_values, cap, h_nnz,
+                   stream);
   });
 }

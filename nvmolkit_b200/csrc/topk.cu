@@ -49,7 +49,7 @@ __device__ unsigned long long g_topkStat[2];  // [0] candidates the tile passes 
 // denominators <= 8192 differ by far more than an ulp. For cosine the fp64 values themselves are the only order there is.
 // Dice, 2c / (|A| + |B|), is an increasing function of Tanimoto's c / (|A| + |B|) ratio as well, with the same ties: a
 // Dice search is the Tanimoto search, whose values topkDiceValuesKernel then rewrites. General Tversky orders by the fp64
-// value, like cosine (the kernels' TV instantiations).
+// value, like cosine (the kernels' WEIGHTED instantiations).
 __device__ __forceinline__ bool better(double v1, int32_t i1, double v2, int32_t i2) { return v1 > v2 || (v1 == v2 && i1 < i2); }
 
 // val / idx [0, n2) in shared memory, n2 a power of two, best first. Called by the whole CTA.
@@ -81,7 +81,7 @@ struct TopkArgs {
   const uint32_t *q, *lib;  // [nQ][words], [nLib][words]
   const int32_t * popQ, *popLib;
   int             words, k;
-  bool            cosine;
+  Measure         measure;  // Tanimoto, cosine or Tversky (a Dice search is Tanimoto's)
   double*         values;   // [nQ][k] the running lists
   int32_t*        indices;  // [nQ][k]
   int4*           bar;      // [nQ] {c, |A| + |B|, column, float bits of a lower bound of the value} of the k-th best
@@ -89,20 +89,12 @@ struct TopkArgs {
   uint32_t*       count;    // [nQ] candidate slots in use
   uint32_t*       redo;     // [nQ] 1: the row's candidates of this slab did not fit
   uint32_t        cap;
-  double          alpha, beta;  // Tversky weights (the TV instantiations)
 };
-
-// the value of a pair as the search's matrix stores it: Tanimoto / cosine, or (TV) Tversky
-template <bool TV>
-__device__ __forceinline__ double pairValue(const TopkArgs& a, int c, int pa, int pb) {
-  if constexpr (TV) return tverskyFromCounts(c, pa, pb, a.alpha, a.beta);
-  else return simFromCounts(c, pa, pb, a.cosine);
-}
 
 // Grid (parts, queries). Columns [colBeg, colEnd) in `parts` equal ranges; the CTA's k best of its range (fewer if the
 // bar lets fewer through) go to cand[q][part * k ..], padded with kNoCand. listValid: the row's list holds k entries and
 // its last one is a bar to start from. onlyRedo: rows not marked are left alone.
-template <bool TV>
+template <bool WEIGHTED>
 __global__ void __launch_bounds__(kSelThreads) topkScanKernel(const TopkArgs a, uint32_t colBeg, uint32_t colEnd, int listValid, int onlyRedo) {
   __shared__ double   val[kSelItems];
   __shared__ int32_t  idx[kSelItems];
@@ -145,7 +137,7 @@ __global__ void __launch_bounds__(kSelThreads) topkScanKernel(const TopkArgs a, 
         const uint4 y = __ldg(row + w), x = reinterpret_cast<const uint4*>(sq)[w];
         c += __popc(x.x & y.x) + __popc(x.y & y.y) + __popc(x.z & y.z) + __popc(x.w & y.w);
       }
-      const double v = pairValue<TV>(a, c, pa, a.popLib[col]);
+      const double v = measureFromCounts<WEIGHTED>(a.measure, c, pa, a.popLib[col]);
       if (better(v, static_cast<int32_t>(col), barV, barI)) {
         const int at = k + atomicAdd(&nPend, 1);
         val[at] = v, idx[at] = static_cast<int32_t>(col);
@@ -165,7 +157,7 @@ __global__ void __launch_bounds__(kSelThreads) topkScanKernel(const TopkArgs a, 
 // are re-counted exactly, sorted together with the list by the contract's key, and the k best become the list.
 // afterScan = 0, after a tile pass: a row that asked for more slots than there are merges nothing and is marked for the
 // scan. afterScan = 1: the slots hold the scan's results; with onlyRedo, of the marked rows only.
-template <bool TV>
+template <bool WEIGHTED>
 __global__ void __launch_bounds__(kSelThreads) topkSelectKernel(const TopkArgs a, int listValid, int afterScan, int onlyRedo) {
   __shared__ double  val[kSelItems];
   __shared__ int32_t idx[kSelItems];
@@ -202,7 +194,7 @@ __global__ void __launch_bounds__(kSelThreads) topkSelectKernel(const TopkArgs a
   for (int j = warp; j < n; j += kSelThreads / 32) {
     const uint32_t col = a.cand[static_cast<size_t>(q) * a.cap + j];
     double         v   = -1.0;
-    if (col != kNoCand) v = pairValue<TV>(a, countWith(col), pa, a.popLib[col]);
+    if (col != kNoCand) v = measureFromCounts<WEIGHTED>(a.measure, countWith(col), pa, a.popLib[col]);
     if (lane == 0) val[have + j] = v, idx[have + j] = col == kNoCand ? kNoIdx : static_cast<int32_t>(col);
   }
   const int n2 = nextPow2(have + n);
@@ -243,11 +235,12 @@ __global__ void __launch_bounds__(256) topkDiceValuesKernel(const uint32_t* __re
 
 unsigned long long readTopkStat(int i) { return readDeviceCounter(g_topkStat, i); }
 
-// metric: Tanimoto, cosine or Tversky (alpha, beta); dice: a Tanimoto search whose values are then rewritten as Dice
-template <bool TV>
-static void topkSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t nLib, int words, TopkMetric metric, bool dice,
-                       double alpha, double beta, int k, double* values, int32_t* indices, cudaStream_t s) {
-  const bool cosine = metric == kTopkCosine;
+static void topkSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t nLib, int words, const Measure& m, int k,
+                       double* values, int32_t* indices, cudaStream_t s) {
+  const bool    dice   = m.kind == kDice;  // a Tanimoto search whose values are then rewritten as Dice
+  const Measure search = dice ? Measure{kTanimoto} : m;
+  const auto    scanKernel   = isWeighted(search.kind) ? topkScanKernel<true> : topkScanKernel<false>;
+  const auto    selectKernel = isWeighted(search.kind) ? topkSelectKernel<true> : topkSelectKernel<false>;
   Scratch<int32_t> popQ(nQ, s), popLibOwn(lib == q && nLib == nQ ? 0 : nLib, s);
   launchRowPopcount(q, nQ, words, popQ.get(), s);
   if (popLibOwn.get()) launchRowPopcount(lib, nLib, words, popLibOwn.get(), s);
@@ -264,10 +257,9 @@ static void topkSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t
 
   TopkArgs a{};
   a.q = q, a.lib = lib, a.popQ = popQ.get(), a.popLib = popLibOwn.get() ? popLibOwn.get() : popQ.get();
-  a.words = words, a.k = k, a.cosine = cosine;
+  a.words = words, a.k = k, a.measure = search;
   a.values = values, a.indices = indices, a.bar = bar.get();
   a.cand = cand.get(), a.count = count.get(), a.redo = redo.get(), a.cap = cap;
-  a.alpha = alpha, a.beta = beta;
   auto diceValues = [&]() {  // (a Dice search: the Tanimoto lists' values rewritten)
     if (!dice) return;
     const size_t   warps  = nQ * static_cast<size_t>(k);
@@ -284,11 +276,11 @@ static void topkSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t
       TopkArgs ar = a;
       ar.q += r0 * words, ar.popQ += r0, ar.values += r0 * k, ar.indices += r0 * k, ar.bar += r0;
       ar.cand += r0 * cap, ar.count += r0, ar.redo += r0;
-      topkScanKernel<TV><<<dim3(parts, static_cast<unsigned>(std::min<size_t>(65535, nQ - r0))), kSelThreads, 0, s>>>(
+      scanKernel<<<dim3(parts, static_cast<unsigned>(std::min<size_t>(65535, nQ - r0))), kSelThreads, 0, s>>>(
         ar, static_cast<uint32_t>(beg), static_cast<uint32_t>(end), listValid, onlyRedo);
       B200_LAUNCHED();
     }
-    topkSelectKernel<TV><<<static_cast<unsigned>(nQ), kSelThreads, 0, s>>>(a, listValid, 1, onlyRedo);
+    selectKernel<<<static_cast<unsigned>(nQ), kSelThreads, 0, s>>>(a, listValid, 1, onlyRedo);
     B200_LAUNCHED();
   };
 
@@ -308,9 +300,9 @@ static void topkSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t
   for (size_t done = warm; done < nLib;) {
     const size_t cols = std::min({nLib - done, slabMax, g_topkSlabCols > 0 ? slabMax : done});
     launchExpandBits(lib + done * words, cols, words, expLib.get(), s);
-    launchTopkTile(metric, expQ.get(), nQ, popQ.get(), expLib.get(), cols, a.popLib + done, words, bar.get(), cand.get(), count.get(), cap,
-                   static_cast<uint32_t>(done), alpha, beta, s);
-    topkSelectKernel<TV><<<static_cast<unsigned>(nQ), kSelThreads, 0, s>>>(a, 1, 0, 0);
+    launchTopkTile(search, expQ.get(), nQ, popQ.get(), expLib.get(), cols, a.popLib + done, words, bar.get(), cand.get(), count.get(), cap,
+                   static_cast<uint32_t>(done), s);
+    selectKernel<<<static_cast<unsigned>(nQ), kSelThreads, 0, s>>>(a, 1, 0, 0);
     B200_LAUNCHED();
     scanAndSelect(done, done + cols, 1, 1);  // the rows whose candidates did not fit (none, as a rule: the CTAs return at once)
     done += cols;
@@ -319,16 +311,15 @@ static void topkSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t
   diceValues();
 }
 
-// the checks both entry points make before any device work
-static void topkChecks(const uint32_t* d_q, size_t nQ, const uint32_t*& d_lib, size_t& nLib, int words, int k, double* d_values,
-                       int32_t* d_indices) {
+// both entry points: the checks before any device work, then the search
+static void topkEntry(const uint32_t* d_q, size_t nQ, const uint32_t* d_lib, size_t nLib, int words, const Measure& m, int k,
+                      double* d_values, int32_t* d_indices, void* stream) {
   B200_REQUIRE(nQ == 0 || d_q, "null fingerprint pointer");
   if (!d_lib) {
     d_lib = d_q;
     nLib  = nQ;
   }
-  B200_REQUIRE(words > 0 && words % 4 == 0 && words <= 128,
-               "fingerprint width must be a multiple of 128 bits and at most 4096 bits (got %d words)", words);
+  requireFingerprintWidth(words);
   B200_REQUIRE(nQ < (1ull << 31) && nLib < (1ull << 31), "too many fingerprints");
   B200_REQUIRE(k >= 1 && static_cast<size_t>(k) <= nLib && k <= kTopkMax, "k must be in [1, min(library size, %d)] (got k = %d, library %zu)",
                kTopkMax, k, nLib);
@@ -336,6 +327,7 @@ static void topkChecks(const uint32_t* d_q, size_t nQ, const uint32_t*& d_lib, s
   B200_REQUIRE(d_values && d_indices, "null output pointer");
   B200_REQUIRE((reinterpret_cast<uintptr_t>(d_q) & 15) == 0 && (reinterpret_cast<uintptr_t>(d_lib) & 15) == 0,
                "fingerprint buffers must be 16-byte aligned");
+  topkSearch(d_q, nQ, d_lib, nLib, words, m, k, d_values, d_indices, asStream(stream));
 }
 
 }  // namespace b200
@@ -344,27 +336,10 @@ using namespace b200;
 
 extern "C" int b200mol_similarity_topk(const uint32_t* d_q, size_t nQ, const uint32_t* d_lib, size_t nLib, int words, int metric, int k,
                                        double* d_values, int32_t* d_indices, void* stream) {
-  return guarded([&] {
-    B200_REQUIRE(metric == B200MOL_METRIC_TANIMOTO || metric == B200MOL_METRIC_COSINE, "unknown metric %d", metric);
-    topkChecks(d_q, nQ, d_lib, nLib, words, k, d_values, d_indices);
-    if (nQ == 0) return;
-    topkSearch<false>(d_q, nQ, d_lib, nLib, words, metric == B200MOL_METRIC_COSINE ? kTopkCosine : kTopkTanimoto, false, 0.0, 0.0, k,
-                      d_values, d_indices, asStream(stream));
-  });
+  return guarded([&] { topkEntry(d_q, nQ, d_lib, nLib, words, measureOfMetric(metric), k, d_values, d_indices, stream); });
 }
 
-// Tversky / Dice: (1/2, 1/2) and (1, 1) are Tanimoto searches (Dice with its values rewritten; Tversky(1, 1) is Tanimoto's
-// value bit for bit), any other weights the Tversky instantiations.
 extern "C" int b200mol_tversky_topk(const uint32_t* d_q, size_t nQ, const uint32_t* d_lib, size_t nLib, int words, double alpha,
                                     double beta, int k, double* d_values, int32_t* d_indices, void* stream) {
-  return guarded([&] {
-    requireTverskyWeights(alpha, beta);
-    topkChecks(d_q, nQ, d_lib, nLib, words, k, d_values, d_indices);
-    if (nQ == 0) return;
-    const bool dice = tverskyIsDice(alpha, beta);
-    if (dice || tverskyIsTanimoto(alpha, beta))
-      topkSearch<false>(d_q, nQ, d_lib, nLib, words, kTopkTanimoto, dice, alpha, beta, k, d_values, d_indices, asStream(stream));
-    else
-      topkSearch<true>(d_q, nQ, d_lib, nLib, words, kTopkTversky, false, alpha, beta, k, d_values, d_indices, asStream(stream));
-  });
+  return guarded([&] { topkEntry(d_q, nQ, d_lib, nLib, words, measureOfWeights(alpha, beta), k, d_values, d_indices, stream); });
 }

@@ -12,29 +12,62 @@ from nvmolkit_b200._interop import fingerprint_matrix, require_cuda, stream_ctx,
 from nvmolkit_b200.types import AsyncGpuResult
 
 
-def _cross(fn_name: str, one, two, stream, weights=()) -> AsyncGpuResult:
-    sptr = stream_ptr(stream)  # validates `stream` first, like the reference (TypeError)
+def _entry(operation: str, measure):
+    """The C entry point of an operation ("cross", "topk", "threshold" or "cross_host") for a measure (a key of
+    _lib.METRIC, or the (alpha, beta) of Tversky), and the measure's arguments to it."""
+    if not isinstance(measure, str):
+        return f"b200mol_tversky_{operation}", measure
+    if operation == "cross":  # (one entry point per metric)
+        return f"b200mol_{measure}_cross", ()
+    return f"b200mol_similarity_{operation}", (_lib.METRIC[measure],)
+
+
+def _check_width(a, b) -> None:
+    if b is not None and a.shape[1] != b.shape[1]:
+        raise ValueError(f"fingerprint widths differ: {a.shape[1]} vs {b.shape[1]} words")
+
+
+def _fingerprints(one, two):
+    """CUDA, both fingerprint matrices and their widths; b is None for a search of group one against itself."""
     require_cuda()
     a = fingerprint_matrix(one, "fingerprint_group_one")
-    b = a if two is None else fingerprint_matrix(two, "fingerprint_group_two")
-    if a.shape[1] != b.shape[1]:
-        raise ValueError(f"fingerprint widths differ: {a.shape[1]} vs {b.shape[1]} words")
+    b = None if two is None else fingerprint_matrix(two, "fingerprint_group_two")
+    _check_width(a, b)
+    return a, b
+
+
+def _operands(one, two, stream):
+    """The stream pointer and both fingerprint matrices (b = a when group two is None), the stream checked first, like
+    the reference (TypeError)."""
+    sptr = stream_ptr(stream)
+    a, b = _fingerprints(one, two)
+    return sptr, a, a if b is None else b
+
+
+def _keep_alive(*tensors) -> None:
+    """keep inputs alive until the stream has consumed them"""
+    for x in tensors:
+        if x is not None:
+            x.record_stream(torch.cuda.current_stream())
+
+
+def _cross(measure, one, two, stream) -> AsyncGpuResult:
+    sptr, a, b = _operands(one, two, stream)
+    fn, args = _entry("cross", measure)
     with stream_ctx(stream):
         out = torch.empty((a.shape[0], b.shape[0]), dtype=torch.float64, device=a.device)
-        _lib.call(fn_name, a.data_ptr(), a.shape[0], b.data_ptr(), b.shape[0], a.shape[1], *weights, out.data_ptr(), sptr)
-        # keep inputs alive until the stream has consumed them
-        a.record_stream(torch.cuda.current_stream())
-        b.record_stream(torch.cuda.current_stream())
+        _lib.call(fn, a.data_ptr(), a.shape[0], b.data_ptr(), b.shape[0], a.shape[1], *args, out.data_ptr(), sptr)
+        _keep_alive(a, b)
     return AsyncGpuResult(out)
 
 
 def crossTanimotoSimilarity(fingerprint_group_one, fingerprint_group_two=None, stream=None) -> AsyncGpuResult:
     """(n, m) fp64 Tanimoto similarities; all-to-all within group one when group two is None. Asynchronous."""
-    return _cross("b200mol_tanimoto_cross", fingerprint_group_one, fingerprint_group_two, stream)
+    return _cross("tanimoto", fingerprint_group_one, fingerprint_group_two, stream)
 
 
 def crossCosineSimilarity(fingerprint_group_one, fingerprint_group_two=None, stream=None) -> AsyncGpuResult:
-    return _cross("b200mol_cosine_cross", fingerprint_group_one, fingerprint_group_two, stream)
+    return _cross("cosine", fingerprint_group_one, fingerprint_group_two, stream)
 
 
 TOPK_MAX = 256  # B200MOL_TOPK_MAX (include/b200mol.h): the largest k the search kernels are compiled for
@@ -48,25 +81,16 @@ def _check_k(k, library_size: int) -> int:
     return k
 
 
-def _topk(metric, one, two, k, stream):
-    """metric: a key of _lib.METRIC, or the (alpha, beta) of a Tversky search"""
-    sptr = stream_ptr(stream)  # validates `stream` first, like the matrix calls (TypeError)
-    require_cuda()
-    a = fingerprint_matrix(one, "fingerprint_group_one")
-    b = a if two is None else fingerprint_matrix(two, "fingerprint_group_two")
-    if a.shape[1] != b.shape[1]:
-        raise ValueError(f"fingerprint widths differ: {a.shape[1]} vs {b.shape[1]} words")
+def _topk(measure, one, two, k, stream):
+    sptr, a, b = _operands(one, two, stream)
     k = _check_k(k, b.shape[0])
+    fn, args = _entry("topk", measure)
     with stream_ctx(stream):
         values = torch.empty((a.shape[0], k), dtype=torch.float64, device=a.device)
         indices = torch.empty((a.shape[0], k), dtype=torch.int32, device=a.device)
-        fn, measure = (("b200mol_similarity_topk", (_lib.METRIC[metric],)) if isinstance(metric, str)
-                       else ("b200mol_tversky_topk", metric))
-        _lib.call(fn, a.data_ptr(), a.shape[0], b.data_ptr(), b.shape[0], a.shape[1], *measure, k, values.data_ptr(),
+        _lib.call(fn, a.data_ptr(), a.shape[0], b.data_ptr(), b.shape[0], a.shape[1], *args, k, values.data_ptr(),
                   indices.data_ptr(), sptr)
-        # keep inputs alive until the stream has consumed them
-        a.record_stream(torch.cuda.current_stream())
-        b.record_stream(torch.cuda.current_stream())
+        _keep_alive(a, b)
     return AsyncGpuResult(values), AsyncGpuResult(indices)
 
 
@@ -94,15 +118,10 @@ def _check_threshold(threshold) -> float:
     return t
 
 
-def _threshold(metric, one, two, threshold, stream):
-    """metric: a key of _lib.METRIC, or the (alpha, beta) of a Tversky search"""
+def _threshold(measure, one, two, threshold, stream):
     sptr = stream_ptr(stream)  # validates `stream` first, like the matrix calls (TypeError)
     t = _check_threshold(threshold)
-    require_cuda()
-    a = fingerprint_matrix(one, "fingerprint_group_one")
-    b = None if two is None else fingerprint_matrix(two, "fingerprint_group_two")
-    if b is not None and a.shape[1] != b.shape[1]:
-        raise ValueError(f"fingerprint widths differ: {a.shape[1]} vs {b.shape[1]} words")
+    a, b = _fingerprints(one, two)
     n_q, n_lib = a.shape[0], (a.shape[0] if b is None else b.shape[0])
     with stream_ctx(stream):
         if n_q == 0 or n_lib == 0:  # no pair (and an empty tensor's address may be 0, the C-ABI's "no library")
@@ -112,21 +131,17 @@ def _threshold(metric, one, two, threshold, stream):
         indptr = torch.empty(n_q + 1, dtype=torch.int64, device=a.device)
         # a first guess at the result size; a larger result is reported and the call is made once more with room for it
         cap = min(max(1 << 20, 64 * n_q), n_q * n_lib)
-        fn, measure = (("b200mol_similarity_threshold", (_lib.METRIC[metric],)) if isinstance(metric, str)
-                       else ("b200mol_tversky_threshold", metric))
+        fn, args = _entry("threshold", measure)
         for _ in range(2):
             indices = torch.empty(cap, dtype=torch.int32, device=a.device)
             values = torch.empty(cap, dtype=torch.float64, device=a.device)
             nnz = C.c_uint64(0)
-            _lib.call(fn, a.data_ptr(), n_q, None if b is None else b.data_ptr(), n_lib, a.shape[1], *measure, t,
+            _lib.call(fn, a.data_ptr(), n_q, None if b is None else b.data_ptr(), n_lib, a.shape[1], *args, t,
                       indptr.data_ptr(), indices.data_ptr(), values.data_ptr(), cap, C.byref(nnz), sptr)
             if nnz.value <= cap:
                 break
             cap = int(nnz.value)
-        # keep inputs alive until the stream has consumed them
-        a.record_stream(torch.cuda.current_stream())
-        if b is not None:
-            b.record_stream(torch.cuda.current_stream())
+        _keep_alive(a, b)
     n = int(nnz.value)
     return AsyncGpuResult(indptr), AsyncGpuResult(indices[:n]), AsyncGpuResult(values[:n])
 
@@ -153,8 +168,7 @@ def thresholdCosineSimilarity(fingerprint_group_one, fingerprint_group_two=None,
     return _threshold("cosine", fingerprint_group_one, fingerprint_group_two, threshold, stream)
 
 
-def _cross_host(metric, one, two, max_device_bytes: int = 0) -> np.ndarray:
-    """metric: a key of _lib.METRIC, or the (alpha, beta) of a Tversky matrix"""
+def _cross_host(measure, one, two, max_device_bytes: int = 0) -> np.ndarray:
     require_cuda()
 
     def host(x):
@@ -169,12 +183,10 @@ def _cross_host(metric, one, two, max_device_bytes: int = 0) -> np.ndarray:
 
     a = host(one)
     b = a if two is None else host(two)
-    if a.shape[1] != b.shape[1]:
-        raise ValueError(f"fingerprint widths differ: {a.shape[1]} vs {b.shape[1]} words")
+    _check_width(a, b)
     out = np.empty((a.shape[0], b.shape[0]), dtype=np.float64)
-    fn, measure = (("b200mol_similarity_cross_host", (_lib.METRIC[metric],)) if isinstance(metric, str)
-                   else ("b200mol_tversky_cross_host", metric))
-    _lib.call(fn, a.ctypes.data, a.shape[0], b.ctypes.data, b.shape[0], a.shape[1], *measure, out.ctypes.data,
+    fn, args = _entry("cross_host", measure)
+    _lib.call(fn, a.ctypes.data, a.shape[0], b.ctypes.data, b.shape[0], a.shape[1], *args, out.ctypes.data,
               int(max_device_bytes))
     return out
 
@@ -215,7 +227,7 @@ def _check_weights(alpha, beta) -> tuple:
 def crossDiceSimilarity(fingerprint_group_one, fingerprint_group_two=None, stream=None) -> AsyncGpuResult:
     """(n, m) fp64 Dice similarities 2|A & B| / (|A| + |B|) (0 for an empty intersection); all-to-all within group one
     when group two is None. Asynchronous. Bit-identical to ``crossTverskySimilarity(..., alpha=0.5, beta=0.5)``."""
-    return _cross("b200mol_tversky_cross", fingerprint_group_one, fingerprint_group_two, stream, DICE)
+    return _cross(DICE, fingerprint_group_one, fingerprint_group_two, stream)
 
 
 def crossTverskySimilarity(fingerprint_group_one, fingerprint_group_two=None, *, alpha, beta, stream=None) -> AsyncGpuResult:
@@ -224,7 +236,7 @@ def crossTverskySimilarity(fingerprint_group_one, fingerprint_group_two=None, *,
     None. ``0 <= alpha, beta <= 1000``. Tversky(1, 0) = c / a is how much of the query a library fingerprint contains;
     (0.9, 0.1) is the usual fragment / scaffold setting. Asynchronous. See the module note on RDKit parity."""
     weights = _check_weights(alpha, beta)  # (before anything touches the device)
-    return _cross("b200mol_tversky_cross", fingerprint_group_one, fingerprint_group_two, stream, weights)
+    return _cross(weights, fingerprint_group_one, fingerprint_group_two, stream)
 
 
 def topKDiceSimilarity(fingerprint_group_one, fingerprint_group_two=None, k=10, stream=None):
