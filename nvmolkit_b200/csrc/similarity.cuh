@@ -40,7 +40,7 @@ inline void requireFingerprintWidth(int words) {
 }
 
 // What a tile does with the integer intersection counts of its pairs, for the call's measure (SimLaunch::measure).
-// Each tile maps (operation, measure kind) to its kernel in one place: launchSimilarity (SIMT), launchTensorImpl (wgmma).
+// Each tile maps (operation, measure kind) to its kernel in one place: launchSimilarity (SIMT), kTensorKernels (wgmma).
 enum SimMode : int {
   kMaterialise = 0,  // fp64 similarity matrix
   kCount       = 1,  // thresholded neighbour counts (+ optional edge list); Tanimoto and Dice (atLeast only) test with an

@@ -30,6 +30,7 @@
 // Replaces crossSimilarityKernelTensorOp (src/similarity_kernels.cu:104-240) + the Triton count kernel
 // (nvmolkit/_fusedButina.py:99-179) for the fused Butina pass.
 #include <cub/device/device_radix_sort.cuh>
+#include <tuple>
 #include <vector>
 
 #include "options.cuh"
@@ -1038,7 +1039,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1)
 using TcKernel = void (*)(CUtensorMap, CUtensorMap, TcParams);
 // The tensor tile's kernel for each operation (SimMode) and measure kind (MeasureKind); nullptr: the SIMT tile serves it.
 // Dice runs on the Tanimoto machinery: its matrix from the reciprocal table, its count on Tanimoto's count tile with its
-// own threshold table and pre-filter. The count tile's cluster variants are picked in launchTensorImpl.
+// own threshold table and pre-filter. The count tile's cluster variants are picked in CountSets::pass.
 const TcKernel kTensorKernels[3][4] = {
   // Tanimoto                      cosine                           Dice                          Tversky
   {simTensorKernel<kTcTanimoto, 0>, simTensorKernel<kTcCosine, 0>, simTensorKernel<kTcDice, 0>, simTensorKernel<kTcTversky, 0>},
@@ -1123,85 +1124,6 @@ static void resetWalkCounters(cudaStream_t s) {
 }
 unsigned long long readWalkCounter(int i) { return readDeviceCounter(g_walkedDev, i); }
 
-static bool launchTensorImpl(SimMode op, const SimLaunch& q, cudaStream_t s, int superS, int superC, bool ordered,
-                             bool* overflow, unsigned long long* pilotCand = nullptr, double* pilotPairs = nullptr);
-
-// The operations on tensor cores. Returns false when the operation, measure or problem shape is not eligible (caller uses
-// the SIMT tile).
-bool launchSimilarityTensor(SimMode op, const SimLaunch& q, cudaStream_t s) {
-  if (!kTensorKernels[op][q.measure.kind]) return false;
-  // Superposition serves the Butina passes (symmetric and / or with an edge list): they synchronise for their edge
-  // total anyway, and the superposed pass needs one host read of its candidate count. The plain thresholded count
-  // (b200mol_tanimoto_count_ge) stays asynchronous on the unsuperposed tile.
-  const bool graphPass = op == kCount && (q.symmetric || q.edges != nullptr);
-  if (!graphPass || g_superpose * g_superposeCols == 1) {
-    if (graphPass) {
-      g_superposeLast = 1;
-      resetWalkCounters(s);
-    }
-    return launchTensorImpl(op, q, s, 1, 1, false, nullptr);
-  }
-  int S = g_superpose, C = g_superposeCols;
-  // How far superposition pays depends on the data: the sum of S C random intersections must stay below the threshold
-  // ONE true neighbour pair reaches, or every accumulator is a candidate. A pilot over a prefix sample of the
-  // fingerprints (at most 1/64 of the pairs; candidates listed but nothing counted; launchTensorImpl orders the sample by
-  // popcount as it does the whole set, while a prefix of the whole set's order would hold only its lowest popcounts) measures the candidate rate of each
-  // column factor, widest first; the model
-  //   time(S, C) = pairs / (S C) * tPair + candidates * S C * tVerify
-  // picks the cheapest. A narrower factor can only win while the wider one spends more time verifying than multiplying, so the search stops as soon as it does not.
-  // With the popcount band, `pairs` are the pairs the band leaves: the pilot counts them in its sample, at each column
-  // factor, and the candidate rate is per such pair. The whole set's band is only known after its own sort, so the pass
-  // is costed at the sample's share of banded pairs; every term of the model scales with that share alike, so the
-  // choice does not depend on it.
-  if (g_superposeAuto && q.nX >= 8 * static_cast<size_t>(kGroupRows) && C > 1) {
-    const double nX = static_cast<double>(q.nX), nY = static_cast<double>(q.nY);
-    SimLaunch pilot   = q;
-    pilot.groupOffset = 0;
-    pilot.groupStride = 1;
-    pilot.nX          = std::min<size_t>(32768, std::max<size_t>(2 * kGroupRows, q.nX / 8));
-    pilot.nY          = q.symmetric ? pilot.nX : std::min<size_t>(q.nY, std::max<size_t>(pilot.nX, q.nY / 8));
-    const double sX = static_cast<double>(pilot.nX), sY = static_cast<double>(pilot.nY);
-    const double pilotPairs = q.symmetric ? sX * (sX - 1) / 2.0 : sX * sY;
-    const double totalPairs = (q.symmetric ? nX * (nX - 1) / 2.0 : nX * nY) / (q.groupStride < 1 ? 1 : q.groupStride);
-    // seconds per unsuperposed pair / per verified pair; only their ratio (about 1 : 30) steers the choice. tPair is the
-    // measured pass: 101.8 ms for the 4.67e11 pairs the popcount band leaves of the 1M bench at S C = 16 (H100 SXM, 400 W
-    // limit; 108-110 ms for all 5.0e11 pairs without the band). On the bench data (sample in popcount order) the pilot
-    // then costs 4 x 4 at 0.17 s and runs it; tools/pilot_model.py prints these figures for any fingerprint set without
-    // a GPU.
-    constexpr double tPair = 3.5e-12, tVerify = 0.1e-9;
-    double bestT = -1.0;  // unsuperposed, costed at the widest factor's banded share
-    int    bestS = 1, bestC = 1;
-    for (int c = C; c >= 1; c >>= 1) {
-      unsigned long long got = 0;
-      double             left = pilotPairs;
-      if (!launchTensorImpl(op, pilot, s, S, c, true, nullptr, &got, &left)) return false;
-      const double passPairs = totalPairs * (left / pilotPairs);
-      if (bestT < 0.0) bestT = passPairs * tPair;
-      const double tPass = passPairs / (S * c) * tPair;
-      const double tVer  = left > 0.0 ? static_cast<double>(got) * passPairs / left * S * c * tVerify : 0.0;
-      if (tPass + tVer < bestT) bestT = tPass + tVer, bestS = S, bestC = c;
-      if (tVer <= tPass) break;
-    }
-    S = bestS, C = bestC;
-  }
-  resetWalkCounters(s);
-  while (S * C > 1) {
-    bool overflow = false;
-    if (!launchTensorImpl(op, q, s, S, C, true, &overflow)) return false;
-    g_superposeLast = S * C;
-    if (!overflow) return true;  // else: the candidate list overflowed (dense graph / loose cutoff), nothing was counted yet
-    if (C > 1) C = 1;            // second chance: rows only
-    else S = 1;
-  }
-  // The unsuperposed pass that completes a superposed one stays in popcount order: a sharded call's ranks decide their
-  // fallbacks independently, and their row groups must still be groups of ONE order for the union to be every pair once.
-  g_superposeLast = 1;
-  return launchTensorImpl(op, q, s, 1, 1, true, nullptr);
-}
-
-// ordered (graph passes of the count mode): run on the fingerprints in popcount order and map the results back. Every
-// pass of a graph pass with superposition on is ordered, also an unsuperposed fallback (of the whole call, of a rank or
-// of a pipeline chunk): it must cover the same row groups as the superposed pass it replaces or completes.
 // Pairs i < j (symmetric) or (i, j) of a pass over all row groups that the popcount band leaves (band = nullptr: all).
 static double bandPairs(const TcParams& p, const uint32_t* band, size_t nX, size_t nY) {
   double total = 0.0;
@@ -1220,57 +1142,44 @@ static double bandPairs(const TcParams& p, const uint32_t* band, size_t nX, size
   return total;
 }
 
-static bool launchTensorImpl(SimMode op, const SimLaunch& q, cudaStream_t s, int superS, int superC, bool ordered,
-                             bool* overflow, unsigned long long* pilotCand, double* pilotPairs) {
-  const MeasureKind kind = q.measure.kind;
-  const int bits = q.words * 32;
-  if (bits % kTK != 0 || bits > 4096) return false;
-  const bool same = (q.x == q.y && q.nX == q.nY);
-  if (q.symmetric && !same) return false;
+// The geometry of a tile pass over n x nY fingerprints, S (C) of them summed into one row of the X (Y) operand, over
+// every row group
+static TcParams tileGeometry(size_t n, size_t nY, int words, int S, int C) {
+  const size_t nSuper = (n + S - 1) / S, nSuperY = (nY + C - 1) / C;
+  TcParams     p{};
+  p.n           = static_cast<uint32_t>(nSuper);
+  p.nY          = static_cast<uint32_t>(nSuperY);
+  p.kChunks     = words * 32 / kTK;
+  p.tilesM      = static_cast<uint32_t>((nSuper + kTM - 1) / kTM);
+  p.tilesN      = static_cast<uint32_t>((nSuperY + kTN - 1) / kTN);
+  p.superS      = S;
+  p.superC      = C;
+  p.rowSpan     = static_cast<uint32_t>(kTM * S);
+  p.colSpan     = static_cast<uint32_t>(kTN * C);
+  p.groupTiles  = static_cast<uint32_t>(kGroupRows / (kTM * S));
+  p.groupStride = 1;
+  return p;
+}
 
-  const bool count    = op == kCount;
-  const int  rowBytes = bits;  // one byte per bit of the fingerprint
-  if (!count) superS = superC = 1;  // only the count mode verifies
-  const bool   super  = superS * superC > 1;
-  ordered             = count && (ordered || super);  // (a superposed pass is always ordered)
-  const size_t nSuper = (q.nX + superS - 1) / superS;   // rows of the X operand
-  const size_t nSuperY = (q.nY + superC - 1) / superC;  // rows of the Y operand (tile columns)
-
-  TcParams p{};
-  p.n         = static_cast<uint32_t>(nSuper);
-  p.nY        = static_cast<uint32_t>(nSuperY);
-  p.kChunks   = rowBytes / kTK;
-  p.tilesM    = static_cast<uint32_t>((nSuper + kTM - 1) / kTM);
-  p.superS    = superS;
-  p.superC    = superC;
-  p.rowSpan   = static_cast<uint32_t>(kTM * superS);
-  p.colSpan   = static_cast<uint32_t>(kTN * superC);
-  p.groupTiles = static_cast<uint32_t>(kGroupRows / (kTM * superS));
-  p.tilesN    = static_cast<uint32_t>((nSuperY + kTN - 1) / kTN);
-  p.symmetric = q.symmetric ? 1 : 0;
+// ... and what the call asks of the pass: its row groups, outputs, measure and pre-filter
+static TcParams passParams(const SimLaunch& q, int S, int C) {
+  TcParams p    = tileGeometry(q.nX, q.nY, q.words, S, C);
+  p.symmetric   = q.symmetric ? 1 : 0;
   p.groupOffset = q.groupOffset;
   p.groupStride = q.groupStride < 1 ? 1 : q.groupStride;
-  p.sign      = q.sign;
-  p.counts    = q.rowCounts;
-  p.countsY   = q.symmetric ? q.rowCounts : nullptr;
-  p.edges     = q.edges;
-  p.edgeCursor = q.edgeCursor;
-  p.edgeCap   = q.edgeCap;
-  p.out       = q.out;
-  p.outVec    = (q.nY % 2 == 0 && (reinterpret_cast<uintptr_t>(q.out) & 15) == 0) ? 1 : 0;
-  const int  recipLen = 2 * bits;
-  const bool useRecip = op == kMaterialise && (kind == kTanimoto || kind == kDice);
-  Scratch<double> recip(useRecip ? static_cast<size_t>(recipLen) + 1 : 0, s);
-  if (useRecip) {
-    recipTableKernel<<<(recipLen + 256) / 256, 256, 0, s>>>(recip.get(), recipLen);
-    B200_LAUNCHED();
-    p.recipG = recip.get();
-  }
+  p.sign        = q.sign;
+  p.counts      = q.rowCounts;
+  p.countsY     = q.symmetric ? q.rowCounts : nullptr;
+  p.edges       = q.edges;
+  p.edgeCursor  = q.edgeCursor;
+  p.edgeCap     = q.edgeCap;
+  p.out         = q.out;
+  p.outVec      = (q.nY % 2 == 0 && (reinterpret_cast<uintptr_t>(q.out) & 15) == 0) ? 1 : 0;
   {
     // a pair passes iff 1 - c / (|A| + |B| - c) <= cutoff, i.e. c >= alpha (|A| + |B|) - or, for the threshold search's
     // c / (|A| + |B| - c) >= t, with alpha = t / (1 + t); the pre-filter's alpha is rounded DOWN (and its products
     // too), so it never rejects what the exact fp64 table accepts. Dice's 2c / (|A| + |B|) >= t needs c >= (t / 2) (|A| + |B|).
-    const double a  = q.atLeast ? (kind == kDice ? q.cutoff / 2.0 : q.cutoff / (1.0 + q.cutoff))
+    const double a  = q.atLeast ? (q.measure.kind == kDice ? q.cutoff / 2.0 : q.cutoff / (1.0 + q.cutoff))
                                 : q.cutoff < 2.0 ? (1.0 - q.cutoff) / (2.0 - q.cutoff) : 0.0;
     float        af = static_cast<float>(a);
     if (static_cast<double>(af) > a) af = nextafterf(af, -1.0f);
@@ -1279,27 +1188,164 @@ static bool launchTensorImpl(SimMode op, const SimLaunch& q, cudaStream_t s, int
   }
   p.tvAlpha = q.measure.alpha, p.tvBeta = q.measure.beta;
   p.tvAlphaF = static_cast<float>(q.measure.alpha), p.tvBetaF = static_cast<float>(q.measure.beta);
+  return p;
+}
 
+// One persistent launch over `units` units (tiles, or vertical tile pairs for the clusters of two CTAs that share the
+// column operand): at most one CTA (pair) per SM (pair)
+static void launchPersistent(TcKernel kernel, bool cluster, const CUtensorMap& tmA, const CUtensorMap& tmB, const TcParams& p,
+                             uint64_t units, cudaStream_t s) {
+  optInTensorKernels();
+  if (cluster) {
+    cudaLaunchConfig_t  cfg{};
+    cudaLaunchAttribute attr[1];
+    attr[0].id               = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = 2;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.blockDim             = dim3(kThreadsTC);
+    cfg.dynamicSmemBytes     = kSmemBytesTC;
+    cfg.stream               = s;
+    cfg.attrs                = attr;
+    cfg.numAttrs             = 1;
+    cfg.gridDim              = dim3(2);
+    int maxClusters          = 0;
+    B200_CUDA(cudaOccupancyMaxActiveClusters(&maxClusters, kernel, &cfg));
+    B200_REQUIRE(maxClusters >= 1, "no CTA pair fits the device");
+    uint64_t pairs = maxClusters;  // persistent: one resident cluster per schedulable SM pair
+    if (pairs > units) pairs = units;
+    cfg.gridDim = dim3(static_cast<unsigned>(2 * pairs));
+    B200_CUDA(cudaLaunchKernelEx(&cfg, kernel, tmA, tmB, p));
+  } else {
+    const int grid = static_cast<int>(std::min<uint64_t>(static_cast<uint64_t>(smCount()), units));
+    kernel<<<grid, kThreadsTC, kSmemBytesTC, s>>>(tmA, tmB, p);
+  }
+  B200_LAUNCHED();
+}
+
+// The 0/1 expansion of both operands (one byte per bit, 2 KB per 2048-bit row); a row of a superposed operand is the sum
+// of S (C) consecutive expansions. X and Y share one buffer when they are the same set, summed alike.
+struct Operands {
+  Scratch<uint8_t> x, yOwn;
+  const uint8_t*   y = nullptr;
+};
+static Operands expandOperands(const uint32_t* fx, size_t nX, int S, const uint32_t* fy, size_t nY, int C, int words, bool same,
+                               cudaStream_t s) {
+  auto expand = [&](const uint32_t* src, size_t rows, int k, Scratch<uint8_t>& dst) {
+    const size_t superRows = (rows + k - 1) / k, nw = superRows * static_cast<size_t>(words);
+    dst                    = Scratch<uint8_t>(superRows * static_cast<size_t>(words) * 32, s);
+    const auto grid        = static_cast<unsigned>((nw + 255) / 256);
+    if (k > 1) expandBitsSuperKernel<<<grid, 256, 0, s>>>(src, rows, words, k, superRows, reinterpret_cast<uint4*>(dst.get()));
+    else expandBitsKernel<<<grid, 256, 0, s>>>(src, nw, reinterpret_cast<uint4*>(dst.get()));
+    B200_LAUNCHED();
+  };
+  const bool ownY = !same || S != C;
+  Operands   o;
+  expand(fx, nX, S, o.x);
+  if (ownY) expand(fy, nY, C, o.yOwn);
+  o.y = ownY ? o.yOwn.get() : o.x.get();
+  return o;
+}
+
+// Materialise and list: one unsuperposed pass in the caller's order.
+static void launchTileOp(SimMode op, const SimLaunch& q, cudaStream_t s) {
+  const MeasureKind kind = q.measure.kind;
+  const bool        same = q.x == q.y && q.nX == q.nY;
+  TcParams          p    = passParams(q, 1, 1);
+  const int         recipLen = 2 * q.words * 32;
+  const bool        useRecip = op == kMaterialise && (kind == kTanimoto || kind == kDice);
+  Scratch<double>   recip(useRecip ? static_cast<size_t>(recipLen) + 1 : 0, s);
+  if (useRecip) {
+    recipTableKernel<<<(recipLen + 256) / 256, 256, 0, s>>>(recip.get(), recipLen);
+    B200_LAUNCHED();
+    p.recipG = recip.get();
+  }
   Scratch<int32_t> popX(q.nX, s), popYown(same ? 0 : q.nY, s);
   launchRowPopcount(q.x, q.nX, q.words, popX.get(), s);
   if (!same) launchRowPopcount(q.y, q.nY, q.words, popYown.get(), s);
-  // A superposed pass runs on the fingerprints ordered by popcount (a stable sort: ties keep the caller's order, so every
-  // rank of a sharded pass builds the same order). The S (C) fingerprints summed into one operand row then have nearly
-  // the same popcount, and the pre-filter, which must assume the group's smallest, sits at the members' own threshold
-  // instead of about a standard deviation below it. Row groups, pipeline chunks and rank ownership all live in this
-  // order; the verification maps each pair back (permX / permY). An unsuperposed pass in this order counts and lists
-  // edges in it, and mapBackKernel moves its results to the caller's indices.
-  PopOrder       ordX, ordYown;
-  const uint32_t *fx = q.x, *fy = q.y;
-  const int32_t * popXs = popX.get(), *popYs = same ? popX.get() : popYown.get(), *permX = nullptr, *permY = nullptr;
-  if (ordered) {
-    ordX = popcountOrder(q.x, popX.get(), q.nX, q.words, s);
-    if (!same) ordYown = popcountOrder(q.y, popYown.get(), q.nY, q.words, s);
-    const PopOrder& ordY = same ? ordX : ordYown;
-    fx = ordX.fp.get(), fy = ordY.fp.get();
-    popXs = ordX.pop.get(), popYs = ordY.pop.get();
-    permX = ordX.perm.get(), permY = ordY.perm.get();
+  const int32_t* popY = same ? popX.get() : popYown.get();
+  const Operands e    = expandOperands(q.x, q.nX, 1, q.y, q.nY, 1, q.words, same, s);
+  // the epilogue's per-row metadata of both operands, padded to whole tiles for the producer's bulk copies
+  const size_t  rowsPad = (static_cast<size_t>(p.tilesM) + 1) * kTM, colsPad = static_cast<size_t>(p.tilesN) * kTN;
+  Scratch<int2> rowMeta(rowsPad, s), colMeta(colsPad, s);
+  if (op == kList) {
+    // the list tile's bound: tLow = t (1 - 1e-5), rounded down
+    float tLow = static_cast<float>(q.cutoff * (1.0 - 1e-5));
+    if (static_cast<double>(tLow) > q.cutoff * (1.0 - 1e-5)) tLow = nextafterf(tLow, 0.0f);
+    p.tvBound = tLow;
+    listMetaKernel<<<static_cast<unsigned>((rowsPad + 255) / 256), 256, 0, s>>>(popX.get(), q.nX, rowsPad, tLow, rowMeta.get());
+    B200_LAUNCHED();
+    listMetaKernel<<<static_cast<unsigned>((colsPad + 255) / 256), 256, 0, s>>>(popY, q.nY, colsPad, 1.0f, colMeta.get());
+    B200_LAUNCHED();
+  } else {
+    tileMetaKernel<<<static_cast<unsigned>((rowsPad + 255) / 256), 256, 0, s>>>(popX.get(), q.nX, 1, q.nX, rowsPad, p.alpha, 1,
+                                                                               rowMeta.get());
+    B200_LAUNCHED();
+    tileMetaKernel<<<static_cast<unsigned>((colsPad + 255) / 256), 256, 0, s>>>(popY, q.nY, 1, q.nY, colsPad, p.alpha, -1,
+                                                                               colMeta.get());
+    B200_LAUNCHED();
   }
+  p.rowMeta = rowMeta.get();
+  p.colMeta = colMeta.get();
+  CUtensorMap tmA, tmB;
+  makeTensorMap2D(&tmA, e.x.get(), q.nX, q.words * 32, kTM, kTK, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1);
+  makeTensorMap2D(&tmB, e.y, q.nY, q.words * 32, kTN, kTK, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1);
+  const uint64_t units = countUnits<false>(p, nullptr);
+  if (units == 0) return;  // nothing owned by this rank (more ranks than row groups)
+  PhaseTimer t(op == kList ? "threshold_list_tc" : "cross_tc", s);
+  launchPersistent(kTensorKernels[op][kind], false, tmA, tmB, p, units, s);
+}
+
+// ---- the count operation: the thresholded count and the graph passes (Butina's neighbour pass, the threshold search,
+// Leader's bulk pass) ----
+
+// Row groups a pass covers: offset, offset + stride, ... (multi-GPU ranks, pipeline chunks)
+struct RowGroups {
+  uint32_t offset, stride;
+  RowGroups chunk(int k, int K) const { return {offset + static_cast<uint32_t>(k) * stride, static_cast<uint32_t>(K) * stride}; }
+};
+
+// What one count pass did. Nothing is counted by a pass whose list overflowed: its row groups must be run again.
+struct PassResult {
+  unsigned long long listed      = 0;      // candidates the superposed pass listed
+  bool               overflowed  = false;  // ... more than its list holds
+  double             bandedPairs = 0.0;    // pilot passes: the pairs the pass covered, within its band if it walked one
+};
+
+// The fingerprints a count call's passes run on and what every pass shares, set up once per call: the caller's order,
+// or (ordered) both sets in popcount order with permX / permY mapping a row back to the caller's index.
+struct CountSets {
+  SimLaunch       q;  // the call, or the pilot's sample of it
+  cudaStream_t    s;
+  const uint32_t *x, *y;
+  const int32_t * popX, *popY, *permX, *permY;
+  const uint16_t* thresh;  // [2 bits + 1]
+  bool            same;    // X and Y are one set
+  bool            ordered;
+
+  // One pass at S x C over `groups`: superposed (a pipeline of chunks from 4 K row groups up, see below) or not. A pilot
+  // pass lists candidates and counts nothing (unless unsuperposed), and adds nothing to the call's diagnostics.
+  PassResult pass(RowGroups groups, int S, int C, bool pilot) const;
+
+  // Passes over `groups` from S x C down, rows only (S x 1) and then unsuperposed, until one completes; returns the S C
+  // of the pass that completed. A pass that overflowed counted nothing, so the next one starts afresh on the same groups.
+  int ladder(RowGroups groups, int S, int C) const {
+    while (S * C > 1) {
+      if (!pass(groups, S, C, false).overflowed) return S * C;
+      if (C > 1) C = 1;  // second chance: rows only
+      else S = 1;
+    }
+    pass(groups, 1, 1, false);
+    return 1;
+  }
+};
+
+PassResult CountSets::pass(RowGroups groups, int S, int C, bool pilot) const {
+  const bool super = S * C > 1;
+  TcParams   p     = passParams(q, S, C);
+  p.groupOffset = groups.offset, p.groupStride = groups.stride;
+  // An unsuperposed pass in popcount order counts and lists edges in that order; mapBackKernel moves its results to the
+  // caller's indices.
   const bool                  mapBack = ordered && !super;
   Scratch<int32_t>            countsOrd(mapBack ? q.nX : 0, s);
   Scratch<unsigned long long> edgeStart(mapBack && q.edges ? 1 : 0, s);
@@ -1309,44 +1355,15 @@ static bool launchTensorImpl(SimMode op, const SimLaunch& q, cudaStream_t s, int
     p.countsY = q.symmetric ? countsOrd.get() : nullptr;
     if (q.edges) B200_CUDA(cudaMemcpyAsync(edgeStart.get(), q.edgeCursor, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, s));
   }
-
-  // 0/1 expansion of the fingerprints (2 KB per 2048-bit row); a superposed operand is the sum of superS (superC)
-  // consecutive expansions. X and Y share one buffer when they are the same set, summed alike.
-  const bool       ownY = !same || superS != superC;
-  Scratch<uint8_t> expX(nSuper * static_cast<size_t>(rowBytes), s);
-  Scratch<uint8_t> expYown(ownY ? nSuperY * static_cast<size_t>(rowBytes) : 0, s);
-  auto expand = [&](const uint32_t* src, size_t rows, int S, size_t superRows, uint8_t* dst) {
-    const size_t nw = superRows * static_cast<size_t>(q.words);
-    const auto   grid = static_cast<unsigned>((nw + 255) / 256);
-    if (S > 1) expandBitsSuperKernel<<<grid, 256, 0, s>>>(src, rows, q.words, S, superRows, reinterpret_cast<uint4*>(dst));
-    else expandBitsKernel<<<grid, 256, 0, s>>>(src, nw, reinterpret_cast<uint4*>(dst));
-    B200_LAUNCHED();
-  };
-  expand(fx, q.nX, superS, nSuper, expX.get());
-  if (ownY) expand(fy, q.nY, superC, nSuperY, expYown.get());
-  const uint8_t* expY = ownY ? expYown.get() : expX.get();
-
+  const Operands e = expandOperands(x, q.nX, S, y, q.nY, C, q.words, same, s);
   // the epilogue's per-row metadata of both operands, padded to whole tiles for the producer's bulk copies (the lower
   // tile of a CTA pair may lie one tile row past the end)
   const size_t  rowsPad = (static_cast<size_t>(p.tilesM) + 1) * kTM, colsPad = static_cast<size_t>(p.tilesN) * kTN;
   Scratch<int2> rowMeta(rowsPad, s), colMeta(colsPad, s);
-  if (op == kList) {
-    // the list tile's bound: tLow = t (1 - 1e-5), rounded down
-    float tLow = static_cast<float>(q.cutoff * (1.0 - 1e-5));
-    if (static_cast<double>(tLow) > q.cutoff * (1.0 - 1e-5)) tLow = nextafterf(tLow, 0.0f);
-    p.tvBound = tLow;
-    listMetaKernel<<<static_cast<unsigned>((rowsPad + 255) / 256), 256, 0, s>>>(popXs, q.nX, rowsPad, tLow, rowMeta.get());
-    B200_LAUNCHED();
-    listMetaKernel<<<static_cast<unsigned>((colsPad + 255) / 256), 256, 0, s>>>(popYs, q.nY, colsPad, 1.0f, colMeta.get());
-    B200_LAUNCHED();
-  } else {
-    tileMetaKernel<<<static_cast<unsigned>((rowsPad + 255) / 256), 256, 0, s>>>(popXs, q.nX, superS, nSuper, rowsPad, p.alpha, 1,
-                                                                               rowMeta.get());
-    B200_LAUNCHED();
-    tileMetaKernel<<<static_cast<unsigned>((colsPad + 255) / 256), 256, 0, s>>>(popYs, q.nY, superC, nSuperY, colsPad, p.alpha, -1,
-                                                                               colMeta.get());
-    B200_LAUNCHED();
-  }
+  tileMetaKernel<<<static_cast<unsigned>((rowsPad + 255) / 256), 256, 0, s>>>(popX, q.nX, S, p.n, rowsPad, p.alpha, 1, rowMeta.get());
+  B200_LAUNCHED();
+  tileMetaKernel<<<static_cast<unsigned>((colsPad + 255) / 256), 256, 0, s>>>(popY, q.nY, C, p.nY, colsPad, p.alpha, -1, colMeta.get());
+  B200_LAUNCHED();
   p.rowMeta = rowMeta.get();
   p.colMeta = colMeta.get();
   // candidates of a superposed pass: (super row, super column) pairs the exact kernel re-examines. Sized for the
@@ -1355,101 +1372,65 @@ static bool launchTensorImpl(SimMode op, const SimLaunch& q, cudaStream_t s, int
   Scratch<int2>               cand;
   Scratch<unsigned long long> candCursor;
   if (super) {
-    const unsigned long long all = static_cast<unsigned long long>(nSuper) * nSuperY;
+    const unsigned long long all = static_cast<unsigned long long>(p.n) * p.nY;
     candCap                      = std::min<unsigned long long>(all, std::max<unsigned long long>(1ull << 22, 64ull * q.nX));
     cand                         = Scratch<int2>(candCap, s);
     candCursor                   = Scratch<unsigned long long>(kMaxPipeline, s);
     B200_CUDA(cudaMemsetAsync(candCursor.get(), 0, kMaxPipeline * sizeof(unsigned long long), s));
     p.cand = cand.get(), p.candCursor = candCursor.get(), p.candCap = candCap;
   }
-  const int         maxS = 2 * bits;
-  Scratch<uint16_t> thresh(static_cast<size_t>(maxS + 1), s);
-  if (count) {
-    launchThreshTable(maxS, q.measure, q.cutoff, q.atLeast, thresh.get(), s);
-    p.threshLen = maxS + 1;
-  }
-  p.thresh = thresh.get();
-  // The popcount band of an ordered pass (superposed passes, their unsuperposed fallbacks, the pilot), with a host copy
-  // for the unit count that sizes the grid: one read of a few hundred bytes per pass.
-  const uint32_t        groups = static_cast<uint32_t>((q.nX + kGroupRows - 1) / kGroupRows);
-  const bool            banded = ordered && g_popcountBand;
-  Scratch<uint32_t>     band(banded ? groups : 0, s);
-  std::vector<uint32_t> bandHost(banded ? groups : 0);
+  const int maxS = 2 * q.words * 32;
+  p.thresh       = thresh;
+  p.threshLen    = maxS + 1;
+  // The popcount band of an ordered pass, with a host copy for the unit count that sizes the grid: one read of a few
+  // hundred bytes per pass.
+  const uint32_t        nGroups = static_cast<uint32_t>((q.nX + kGroupRows - 1) / kGroupRows);
+  const bool            banded  = ordered && g_popcountBand;
+  Scratch<uint32_t>     band(banded ? nGroups : 0, s);
+  std::vector<uint32_t> bandHost(banded ? nGroups : 0);
   if (banded) {
-    popcountBandKernel<<<1, kBandThreads, (maxS + 1) * sizeof(uint16_t), s>>>(popXs, q.nX, popYs, q.nY, thresh.get(), maxS + 1,
-                                                                              p.colSpan, p.tilesN, groups, band.get());
+    popcountBandKernel<<<1, kBandThreads, (maxS + 1) * sizeof(uint16_t), s>>>(popX, q.nX, popY, q.nY, thresh, maxS + 1, p.colSpan,
+                                                                              p.tilesN, nGroups, band.get());
     B200_LAUNCHED();
-    B200_CUDA(cudaMemcpyAsync(bandHost.data(), band.get(), groups * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    B200_CUDA(cudaMemcpyAsync(bandHost.data(), band.get(), nGroups * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
     B200_CUDA(cudaStreamSynchronize(s));
     p.bandEnd = band.get();
   }
   const uint32_t* bandH = banded ? bandHost.data() : nullptr;
-  if (count) p.walked = deviceCounters(g_walkedDev);
+  p.walked              = deviceCounters(g_walkedDev);
 
   CUtensorMap tmA, tmB;
-  makeTensorMap2D(&tmA, expX.get(), nSuper, rowBytes, kTM, kTK, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1);
+  makeTensorMap2D(&tmA, e.x.get(), p.n, q.words * 32, kTM, kTK, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1);
   // CTA pairs sharing the column operand (TMA multicast); 3 = the same with the row operand stationary, for fingerprints
   // whose 128-row tile fits its shared-memory region (else the plain pair runs)
-  const bool cluster    = count && g_tensorCluster != 0;
+  const bool cluster    = g_tensorCluster != 0;
   const bool stationary = cluster && g_tensorCluster == 3 && p.kChunks <= kMaxChunksStat;
-  makeTensorMap2D(&tmB, expY, nSuperY, rowBytes, cluster ? kTN / 2 : kTN, kTK, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1);
-
+  makeTensorMap2D(&tmB, e.y, p.nY, q.words * 32, cluster ? kTN / 2 : kTN, kTK, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1);
   static_assert(kMaxChunksStat * kABytes + kStagesStat * kBBytes == kStages * kStageBytes, "both layouts take the same shared memory");
-  const size_t smemBytes = kSmemBytesTC;
-  optInTensorKernels();
-  const TcKernel kernel = stationary ? simTensorKernel<kTcCount, 3> : cluster ? simTensorKernel<kTcCount, 1> : kTensorKernels[op][kind];
-  // units a call owns: tiles, or vertical tile pairs (same enumeration as the kernel's UnitWalk)
+  const TcKernel kernel = stationary ? simTensorKernel<kTcCount, 3> : cluster ? simTensorKernel<kTcCount, 1> : simTensorKernel<kTcCount, 0>;
+  // units a pass over pk's row groups owns: tiles, or vertical tile pairs (same enumeration as the kernel's UnitWalk)
   auto unitsOf = [&](const TcParams& pk) -> uint64_t {
     return stationary ? countUnits<true, kRunStat>(pk, bandH) : cluster ? countUnits<true>(pk, bandH) : countUnits<false>(pk, bandH);
   };
-  // the count kernel over the row groups `pk` selects (false: none of them is owned by this call)
-  auto launchCount = [&](const TcParams& pk) -> bool {
+  auto launchCount = [&](const TcParams& pk) {
     const uint64_t units = unitsOf(pk);
-    if (!pilotCand) g_unitsPlanned += units;
-    if (units == 0) return false;
-    if (cluster) {
-      cudaLaunchConfig_t cfg{};
-      cudaLaunchAttribute attr[1];
-      attr[0].id               = cudaLaunchAttributeClusterDimension;
-      attr[0].val.clusterDim.x = 2;
-      attr[0].val.clusterDim.y = 1;
-      attr[0].val.clusterDim.z = 1;
-      cfg.blockDim         = dim3(kThreadsTC);
-      cfg.dynamicSmemBytes = smemBytes;
-      cfg.stream           = s;
-      cfg.attrs            = attr;
-      cfg.numAttrs         = 1;
-      cfg.gridDim          = dim3(2);
-      int maxClusters = 0;
-      B200_CUDA(cudaOccupancyMaxActiveClusters(&maxClusters, kernel, &cfg));
-      B200_REQUIRE(maxClusters >= 1, "no CTA pair fits the device");
-      uint64_t pairs = maxClusters;  // persistent: one resident cluster per schedulable SM pair
-      if (pairs > units) pairs = units;
-      cfg.gridDim = dim3(static_cast<unsigned>(2 * pairs));
-      B200_CUDA(cudaLaunchKernelEx(&cfg, kernel, tmA, tmB, pk));
-    } else {
-      const int grid = static_cast<int>(std::min<uint64_t>(static_cast<uint64_t>(smCount()), units));
-      kernel<<<grid, kThreadsTC, smemBytes, s>>>(tmA, tmB, pk);
-    }
-    B200_LAUNCHED();
-    return true;
+    if (!pilot) g_unitsPlanned += units;
+    if (units) launchPersistent(kernel, cluster, tmA, tmB, pk, units, s);
   };
   auto launchVerify = [&](const int2* list, unsigned long long nCand, cudaStream_t on) {
     PhaseTimer         t("verify_candidates", on);
-    const unsigned int blocks2 = static_cast<unsigned int>(std::min<unsigned long long>((nCand + 63) / 64, static_cast<unsigned long long>(smCount()) * 16));
-    verifyCandidatesKernel<<<blocks2, 256, 0, on>>>(fx, fy, q.words, list, nCand, superS, superC, static_cast<uint32_t>(q.nX),
-                                                    static_cast<uint32_t>(q.nY), q.symmetric ? 1 : 0, popXs, popYs, permX, permY,
-                                                    thresh.get(), q.sign, q.rowCounts, q.symmetric ? q.rowCounts : nullptr, q.edges,
-                                                    q.edgeCursor, q.edgeCap);
+    const unsigned int blocks = static_cast<unsigned int>(std::min<unsigned long long>((nCand + 63) / 64, static_cast<unsigned long long>(smCount()) * 16));
+    verifyCandidatesKernel<<<blocks, 256, 0, on>>>(x, y, q.words, list, nCand, S, C, static_cast<uint32_t>(q.nX), static_cast<uint32_t>(q.nY),
+                                                   q.symmetric ? 1 : 0, popX, popY, permX, permY, thresh, q.sign, q.rowCounts,
+                                                   q.symmetric ? q.rowCounts : nullptr, q.edges, q.edgeCursor, q.edgeCap);
     B200_LAUNCHED();
   };
 
-  // Superposed pass in a PIPELINE of K chunks of the row groups (chunk k = groups k, k + K, ... of this call's): the exact
-  // verification of chunk k runs on a second stream while the tensor pass of chunk k + 1 has the SMs - a pass CTA leaves
-  // room for one verify block per SM - so only the last chunk's verification is exposed.
-  // A chunk whose candidate list overflowed is redone on its own with fewer pairs per accumulator after the others.
-  const uint64_t ownedGroups = ((q.nX + kGroupRows - 1) / kGroupRows + p.groupStride - 1) / p.groupStride;
-  const int      K = (super && !pilotCand && g_pipelineChunks > 1 && ownedGroups >= 4ull * g_pipelineChunks) ? g_pipelineChunks : 1;
+  // Superposed pass in a PIPELINE of K chunks of the row groups (chunk k = groups k, k + K, ... of this pass's): the
+  // exact verification of chunk k runs on a second stream while the tensor pass of chunk k + 1 has the SMs - a pass CTA
+  // leaves room for one verify block per SM - so only the last chunk's verification is exposed.
+  const uint64_t ownedGroups = (nGroups + groups.stride - 1) / groups.stride;
+  const int      K = (super && !pilot && g_pipelineChunks > 1 && ownedGroups >= 4ull * g_pipelineChunks) ? g_pipelineChunks : 1;
   if (K > 1) {
     static cudaStream_t side[kMaxDevices] = {};
     cudaStream_t&       s2 = side[currentDeviceSlot()];
@@ -1459,9 +1440,9 @@ static bool launchTensorImpl(SimMode op, const SimLaunch& q, cudaStream_t s, int
     {
       PhaseTimer t("neighbor_pass_tc", s);  // the K tensor passes, back to back on the caller's stream
       for (int k = 0; k < K; ++k) {
-        TcParams pk    = p;
-        pk.groupOffset = p.groupOffset + static_cast<uint32_t>(k) * p.groupStride;
-        pk.groupStride = static_cast<uint32_t>(K) * p.groupStride;
+        TcParams        pk = p;
+        const RowGroups g  = groups.chunk(k, K);
+        pk.groupOffset = g.offset, pk.groupStride = g.stride;
         pk.cand        = cand.get() + static_cast<size_t>(k) * capK;
         pk.candCursor  = candCursor.get() + k;
         pk.candCap     = capK;
@@ -1488,53 +1469,138 @@ static bool launchTensorImpl(SimMode op, const SimLaunch& q, cudaStream_t s, int
     B200_CUDA(cudaStreamWaitEvent(s, done, 0));  // the caller's stream continues after the last verification
     cudaEventDestroy(done);
     g_candidatesLast = listed;
-    for (int r = 0; r < nRedo; ++r) {
-      SimLaunch qk   = q;
-      qk.groupOffset = p.groupOffset + static_cast<uint32_t>(redo[r]) * p.groupStride;
-      qk.groupStride = static_cast<uint32_t>(K) * p.groupStride;
-      bool again     = false;
-      if (!launchTensorImpl(op, qk, s, superS, 1, true, &again)) return false;
-      if (again && !launchTensorImpl(op, qk, s, 1, 1, true, nullptr)) return false;
-    }
-    return true;
+    // A chunk whose list overflowed is redone on its own after the others, from rows only (S x 1) with the whole list:
+    // its share of the list was a K-th of it, so even at S x C the chunk may fit, but the pipeline has moved on and the
+    // rows-only pass needs the fewest candidates of the superposed ones.
+    for (int r = 0; r < nRedo; ++r) ladder(groups.chunk(redo[r], K), S, 1);
+    return {listed, false, 0.0};
   }
 
-  if (unitsOf(p) == 0) return true;  // nothing owned by this rank (more ranks than row groups)
-  int blocks = smCount();
-  if (static_cast<uint64_t>(blocks) > unitsOf(p)) blocks = static_cast<int>(unitsOf(p));
-  if (count) {
-    {
-      PhaseTimer t("neighbor_pass_tc", s);
-      launchCount(p);
-    }
-    if (mapBack) {
-      const unsigned grid = static_cast<unsigned>(std::min<size_t>((q.nX + 255) / 256, static_cast<size_t>(smCount()) * 8));
-      mapBackKernel<<<grid, 256, 0, s>>>(countsOrd.get(), permX, q.nX, q.rowCounts, permY, p.symmetric, q.edges, edgeStart.get(),
-                                         q.edgeCursor, q.edgeCap);
-      B200_LAUNCHED();
-    }
-  } else {
-    PhaseTimer t(op == kList ? "threshold_list_tc" : "cross_tc", s);
-    kernel<<<blocks, kThreadsTC, smemBytes, s>>>(tmA, tmB, p);
+  const uint64_t units = unitsOf(p);
+  if (units == 0) return {0, false, pilot ? bandPairs(p, nullptr, q.nX, q.nY) : 0.0};  // nothing owned or left by the band
+  {
+    PhaseTimer t("neighbor_pass_tc", s);
+    launchCount(p);
+  }
+  if (mapBack) {
+    const unsigned grid = static_cast<unsigned>(std::min<size_t>((q.nX + 255) / 256, static_cast<size_t>(smCount()) * 8));
+    mapBackKernel<<<grid, 256, 0, s>>>(countsOrd.get(), permX, q.nX, q.rowCounts, permY, p.symmetric, q.edges, edgeStart.get(),
+                                       q.edgeCursor, q.edgeCap);
     B200_LAUNCHED();
   }
-  if (super) {
-    // the one host read of a superposed pass: how many candidates (the callers synchronise for their edge total anyway)
-    unsigned long long nCand = 0;
-    B200_CUDA(cudaMemcpyAsync(&nCand, candCursor.get(), sizeof(nCand), cudaMemcpyDeviceToHost, s));
-    B200_CUDA(cudaStreamSynchronize(s));
-    if (pilotCand) {  // dry run over one row group: the candidate count is the result, over the pairs the band leaves
-      *pilotCand = nCand;
-      if (pilotPairs) *pilotPairs = bandPairs(p, bandH, q.nX, q.nY);
-      return true;
-    }
-    g_candidatesLast = nCand;
-    if (nCand > candCap) {
-      if (overflow) *overflow = true;  // nothing has been counted yet: the caller reruns without superposition
-      return true;
-    }
-    if (nCand) launchVerify(cand.get(), nCand, s);
+  if (!super) return {0, false, pilot ? bandPairs(p, nullptr, q.nX, q.nY) : 0.0};
+  // the one host read of a superposed pass: how many candidates (the callers synchronise for their edge total anyway)
+  unsigned long long nCand = 0;
+  B200_CUDA(cudaMemcpyAsync(&nCand, candCursor.get(), sizeof(nCand), cudaMemcpyDeviceToHost, s));
+  B200_CUDA(cudaStreamSynchronize(s));
+  if (pilot) return {nCand, false, bandPairs(p, bandH, q.nX, q.nY)};
+  g_candidatesLast = nCand;
+  if (nCand > candCap) return {nCand, true, 0.0};  // nothing has been counted yet
+  if (nCand) launchVerify(cand.get(), nCand, s);
+  return {nCand, false, 0.0};
+}
+
+// How far superposition pays depends on the data: the sum of S C random intersections must stay below the threshold
+// ONE true neighbour pair reaches, or every accumulator is a candidate. A pilot over a prefix sample of the fingerprints
+// (at most 1/64 of the pairs; candidates listed but nothing counted; the sample is put in popcount order of its own, as
+// a prefix of the whole set's order would hold only its lowest popcounts) measures the candidate rate of each column
+// factor, widest first; the model
+//   time(S, C) = pairs / (S C) * tPair + candidates * S C * tVerify
+// picks the cheapest. A narrower factor can only win while the wider one spends more time verifying than multiplying,
+// so the search stops as soon as it does not.
+// With the popcount band, `pairs` are the pairs the band leaves: the pilot counts them in its sample, at each column
+// factor, and the candidate rate is per such pair. The whole set's band is only known after its own sort, so the pass
+// is costed at the sample's share of banded pairs; every term of the model scales with that share alike, so the
+// choice does not depend on it.
+// popX, popY: the call's popcounts in the caller's order. Returns the cheapest (S, C) of (S, C), (S, C / 2), ... and 1 x 1.
+static std::pair<int, int> pilotFactors(const SimLaunch& q, const int32_t* popX, const int32_t* popY, const uint16_t* thresh,
+                                        cudaStream_t s, int S, int C) {
+  const double nX = static_cast<double>(q.nX), nY = static_cast<double>(q.nY);
+  SimLaunch    pilot = q;
+  pilot.groupOffset  = 0;
+  pilot.groupStride  = 1;
+  pilot.nX           = std::min<size_t>(32768, std::max<size_t>(2 * kGroupRows, q.nX / 8));
+  pilot.nY           = q.symmetric ? pilot.nX : std::min<size_t>(q.nY, std::max<size_t>(pilot.nX, q.nY / 8));
+  const bool     same = pilot.x == pilot.y && pilot.nX == pilot.nY;
+  const PopOrder ordX = popcountOrder(q.x, popX, pilot.nX, q.words, s);
+  const PopOrder ordYown = same ? PopOrder{} : popcountOrder(q.y, popY, pilot.nY, q.words, s);
+  const PopOrder& ordY   = same ? ordX : ordYown;
+  const CountSets sample{pilot,           s, ordX.fp.get(), ordY.fp.get(), ordX.pop.get(), ordY.pop.get(), ordX.perm.get(),
+                         ordY.perm.get(), thresh, same, true};
+  const double sX = static_cast<double>(pilot.nX), sY = static_cast<double>(pilot.nY);
+  const double pilotPairs = q.symmetric ? sX * (sX - 1) / 2.0 : sX * sY;
+  const double totalPairs = (q.symmetric ? nX * (nX - 1) / 2.0 : nX * nY) / (q.groupStride < 1 ? 1 : q.groupStride);
+  // seconds per unsuperposed pair / per verified pair; only their ratio (about 1 : 30) steers the choice. tPair is the
+  // measured pass: 101.8 ms for the 4.67e11 pairs the popcount band leaves of the 1M bench at S C = 16 (H100 SXM, 400 W
+  // limit; 108-110 ms for all 5.0e11 pairs without the band). On the bench data (sample in popcount order) the pilot
+  // then costs 4 x 4 at 0.17 s and runs it; tools/pilot_model.py prints these figures for any fingerprint set without
+  // a GPU.
+  constexpr double tPair = 3.5e-12, tVerify = 0.1e-9;
+  double bestT = -1.0;  // unsuperposed, costed at the widest factor's banded share
+  int    bestS = 1, bestC = 1;
+  for (int c = C; c >= 1; c >>= 1) {
+    const PassResult r         = sample.pass({0, 1}, S, c, true);
+    const double     left      = r.bandedPairs;
+    const double     passPairs = totalPairs * (left / pilotPairs);
+    if (bestT < 0.0) bestT = passPairs * tPair;
+    const double tPass = passPairs / (S * c) * tPair;
+    const double tVer  = left > 0.0 ? static_cast<double>(r.listed) * passPairs / left * S * c * tVerify : 0.0;
+    if (tPass + tVer < bestT) bestT = tPass + tVer, bestS = S, bestC = c;
+    if (tVer <= tPass) break;
   }
+  return {bestS, bestC};
+}
+
+static void launchCountOp(const SimLaunch& q, cudaStream_t s) {
+  const bool       same = q.x == q.y && q.nX == q.nY;
+  Scratch<int32_t> popX(q.nX, s), popYown(same ? 0 : q.nY, s);
+  launchRowPopcount(q.x, q.nX, q.words, popX.get(), s);
+  if (!same) launchRowPopcount(q.y, q.nY, q.words, popYown.get(), s);
+  const int32_t*    popY = same ? popX.get() : popYown.get();
+  const int         maxS = 2 * q.words * 32;
+  Scratch<uint16_t> thresh(static_cast<size_t>(maxS + 1), s);
+  launchThreshTable(maxS, q.measure, q.cutoff, q.atLeast, thresh.get(), s);
+  const RowGroups groups{q.groupOffset, q.groupStride < 1 ? 1 : q.groupStride};
+  // Superposition serves the graph passes (symmetric and / or with an edge list): they synchronise for their edge
+  // total anyway, and the superposed pass needs one host read of its candidate count. The plain thresholded count
+  // (b200mol_tanimoto_count_ge) stays asynchronous on the unsuperposed tile.
+  const bool graphPass = q.symmetric || q.edges != nullptr;
+  if (!graphPass || g_superpose * g_superposeCols == 1) {
+    if (graphPass) {
+      g_superposeLast = 1;
+      resetWalkCounters(s);
+    }
+    const CountSets call{q, s, q.x, q.y, popX.get(), popY, nullptr, nullptr, thresh.get(), same, false};
+    call.pass(groups, 1, 1, false);
+    return;
+  }
+  int S = g_superpose, C = g_superposeCols;
+  if (g_superposeAuto && q.nX >= 8 * static_cast<size_t>(kGroupRows) && C > 1) std::tie(S, C) = pilotFactors(q, popX.get(), popY, thresh.get(), s, S, C);
+  // A superposed pass runs on the fingerprints ordered by popcount (a stable sort: ties keep the caller's order, so every
+  // rank of a sharded pass builds the same order). The S (C) fingerprints summed into one operand row then have nearly
+  // the same popcount, and the pre-filter, which must assume the group's smallest, sits at the members' own threshold
+  // instead of about a standard deviation below it. Row groups, pipeline chunks and rank ownership all live in this
+  // order; the verification maps each pair back (permX / permY). Every pass of the call runs in it, also an unsuperposed
+  // fallback (of the whole call, of a rank or of a pipeline chunk): it must cover the same row groups as the superposed
+  // pass it replaces or completes, and a sharded call's ranks decide their fallbacks independently, so their row groups
+  // must still be groups of ONE order for the union to be every pair once.
+  const PopOrder  ordX    = popcountOrder(q.x, popX.get(), q.nX, q.words, s);
+  const PopOrder  ordYown = same ? PopOrder{} : popcountOrder(q.y, popY, q.nY, q.words, s);
+  const PopOrder& ordY    = same ? ordX : ordYown;
+  const CountSets call{q, s, ordX.fp.get(), ordY.fp.get(), ordX.pop.get(), ordY.pop.get(), ordX.perm.get(), ordY.perm.get(),
+                       thresh.get(), same, true};
+  resetWalkCounters(s);
+  g_superposeLast = call.ladder(groups, S, C);
+}
+
+// The operations on tensor cores. Returns false when the operation, measure or problem shape is not eligible (caller uses
+// the SIMT tile); decided before any device work.
+bool launchSimilarityTensor(SimMode op, const SimLaunch& q, cudaStream_t s) {
+  const int bits = q.words * 32;
+  if (!kTensorKernels[op][q.measure.kind] || bits % kTK != 0 || bits > 4096) return false;
+  if (q.symmetric && !(q.x == q.y && q.nX == q.nY)) return false;
+  if (op == kCount) launchCountOp(q, s);
+  else launchTileOp(op, q, s);
   return true;
 }
 
@@ -1565,25 +1631,14 @@ void launchTopkTile(const Measure& m, const uint8_t* expQ, size_t nQ, const int3
   const TcKernel kernel = kTopkKernels[m.kind];
   B200_REQUIRE(kernel, "no top-k tile for measure %d", m.kind);
   const bool cosine = m.kind == kCosine;
-  const int rowBytes = words * 32;
-  TcParams  p{};
-  p.n           = static_cast<uint32_t>(nQ);
-  p.nY          = static_cast<uint32_t>(nCols);
-  p.kChunks     = rowBytes / kTK;
-  p.tilesM      = static_cast<uint32_t>((nQ + kTM - 1) / kTM);
-  p.tilesN      = static_cast<uint32_t>((nCols + kTN - 1) / kTN);
-  p.groupStride = 1;
-  p.superS = p.superC = 1;
-  p.rowSpan     = kTM;
-  p.colSpan     = kTN;
-  p.groupTiles  = kGroupRows / kTM;
-  p.topkBar     = bar;
-  p.topkCand    = cand;
-  p.topkCount   = count;
-  p.topkCap     = cap;
-  p.topkColBase = colBase;
-  p.tvAlphaF    = static_cast<float>(m.alpha);
-  p.tvBetaF     = static_cast<float>(m.beta);
+  TcParams   p      = tileGeometry(nQ, nCols, words, 1, 1);
+  p.topkBar         = bar;
+  p.topkCand        = cand;
+  p.topkCount       = count;
+  p.topkCap         = cap;
+  p.topkColBase     = colBase;
+  p.tvAlphaF        = static_cast<float>(m.alpha);
+  p.tvBetaF         = static_cast<float>(m.beta);
   const size_t  rowsPad = static_cast<size_t>(p.tilesM) * kTM, colsPad = static_cast<size_t>(p.tilesN) * kTN;
   Scratch<int2> rowMeta(rowsPad, s), colMeta(colsPad, s);
   topkMetaKernel<<<static_cast<unsigned>((rowsPad + 255) / 256), 256, 0, s>>>(popQ, nQ, rowsPad, 0, rowMeta.get());
@@ -1593,14 +1648,11 @@ void launchTopkTile(const Measure& m, const uint8_t* expQ, size_t nQ, const int3
   p.rowMeta = rowMeta.get();
   p.colMeta = colMeta.get();
   CUtensorMap tmA, tmB;
-  makeTensorMap2D(&tmA, expQ, nQ, rowBytes, kTM, kTK, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1);
-  makeTensorMap2D(&tmB, expLib, nCols, rowBytes, kTN, kTK, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1);
-  optInTensorKernels();
+  makeTensorMap2D(&tmA, expQ, nQ, words * 32, kTM, kTK, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1);
+  makeTensorMap2D(&tmB, expLib, nCols, words * 32, kTN, kTK, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1);
   const uint64_t units = countUnits<false>(p, nullptr);
   if (units == 0) return;
-  const int grid = static_cast<int>(std::min<uint64_t>(static_cast<uint64_t>(smCount()), units));
-  kernel<<<grid, kThreadsTC, kSmemBytesTC, s>>>(tmA, tmB, p);
-  B200_LAUNCHED();
+  launchPersistent(kernel, false, tmA, tmB, p, units, s);
 }
 
 }  // namespace b200

@@ -7,7 +7,7 @@ sum of a group's S x C counts when superposed):
 
     256 acc - T(|B|) >= T(|A|),   T(m) = floor(RD(256 alpha m)),
 
-with alpha = (1 - cutoff) / (2 - cutoff) rounded down to float32 and then one ulp further (launchTensorImpl), RD a
+with alpha = (1 - cutoff) / (2 - cutoff) rounded down to float32 and then one ulp further (passParams), RD a
 float32 product rounded down, and |A|, |B| the smallest popcounts of the group (tileMetaKernel). It must never reject a
 neighbour: the margin 256 thresh[|A| + |B|] - T(|A|) - T(|B|) must be >= 0 for every pair that can exist.
 
@@ -35,7 +35,7 @@ SEVEN_TENTHS = [(7, 10, 7), (8, 9, 7), (10, 7, 7), (14, 20, 14), (70, 100, 70)] 
 
 # ------------------------------------------------------------------ CPU model of the predicate and the pre-filter
 def prefilter_alpha(cutoff: float) -> np.float32:
-    """The float32 alpha launchTensorImpl hands the tile: (1 - cutoff) / (2 - cutoff) in fp64, rounded down to float32,
+    """The float32 alpha passParams hands the tile: (1 - cutoff) / (2 - cutoff) in fp64, rounded down to float32,
     one ulp further down, clamped at 0."""
     a = (1.0 - cutoff) / (2.0 - cutoff) if cutoff < 2.0 else 0.0
     af = np.float32(a)

@@ -44,7 +44,7 @@ def cost_constants() -> tuple[float, float]:
 
 
 def prefilter_alpha(cutoff: float) -> np.float32:
-    """The float32 alpha launchTensorImpl hands the tile: (1 - cutoff) / (2 - cutoff) rounded down, one ulp further."""
+    """The float32 alpha passParams hands the tile: (1 - cutoff) / (2 - cutoff) rounded down, one ulp further."""
     a = (1.0 - cutoff) / (2.0 - cutoff) if cutoff < 2.0 else 0.0
     af = np.float32(a)
     if float(af) > a:
