@@ -213,6 +213,30 @@ int b200mol_tversky_threshold(const uint32_t* d_q, size_t nQ, const uint32_t* d_
                               int32_t* d_indices /* [cap] */, double* d_values /* [cap] */, uint64_t cap, uint64_t* h_nnz,
                               void* stream);
 
+/* Tanimoto, Dice and Tversky on count vectors (RDKit's SparseIntVect / GetCountFingerprint similarity). A row is bins
+ * int32 counts (d_a [nA][bins], row-major, 1 <= bins <= 4096), each in 0 .. 65535. With a = the sum of the row (group
+ * one), b = the sum of the column's row and c = the sum over bins of min(row, column), the value of a pair is that of
+ * b200mol_tversky_cross: 0 when c = 0, else c / ((alpha (a - c) + beta (b - c)) + c) one rounded fp64 operation at a
+ * time. The count bound keeps every sum and a + b - c exact integers below 2^31, so Tanimoto (1, 1) is RDKit's
+ * andSum / (v1Sum + v2Sum - andSum) and Dice (0.5, 0.5) its 2 andSum / (v1Sum + v2Sum), bit for bit; for non-dyadic
+ * weights the note on b200mol_tversky_cross applies. Each entry point takes the arguments of its b200mol_tversky_* twin
+ * with `bins` in place of `words`, and has its contract: the fp64 matrix, the exact top-k ((value descending, column
+ * ascending), 1 <= k <= min(nLib, B200MOL_TOPK_MAX)), or the exact CSR of the entries >= threshold (0 < threshold <= 1,
+ * the cap / h_nnz protocol of b200mol_similarity_threshold); d_b / d_lib = NULL: group one against itself, self-matches
+ * included. Argument errors are refused before any device work; a count outside 0 .. 65535 is refused
+ * (B200MOL_ERR_INVALID) after a device check whose flag is read once, so every call SYNCHRONISES `stream`, and nothing
+ * is written to the outputs when it fails. Scratch is stream-ordered: each row's non-zeros as 4-byte (bin, count) pairs
+ * and 12 bytes per row; top-k adds the candidate slots of b200mol_similarity_topk (12 bytes each), threshold 16 bytes per
+ * listed pair and the CSR assembly of b200mol_similarity_threshold. Cosine is not defined on counts. */
+int b200mol_count_cross(const int32_t* d_a, size_t nA, const int32_t* d_b, size_t nB, int bins, double alpha, double beta,
+                        double* d_out, void* stream);
+int b200mol_count_topk(const int32_t* d_q, size_t nQ, const int32_t* d_lib, size_t nLib, int bins, double alpha, double beta,
+                       int k, double* d_values /* [nQ][k] */, int32_t* d_indices /* [nQ][k] */, void* stream);
+int b200mol_count_threshold(const int32_t* d_q, size_t nQ, const int32_t* d_lib /* NULL = self */, size_t nLib, int bins,
+                            double alpha, double beta, double threshold, int64_t* d_indptr /* [nQ + 1] */,
+                            int32_t* d_indices /* [cap] */, double* d_values /* [cap] */, uint64_t cap, uint64_t* h_nnz,
+                            void* stream);
+
 /* MaxMin diversity picking (RDKit MaxMinPicker::LazyBitVectorPick / LazyBitVectorPickWithThreshold) over the pool
  * d_fp[0 .. nPool) ([nPool][words], 16-byte aligned). d(i, j) = 1 - s(i, j), s the fp64 value b200mol_tanimoto_cross /
  * b200mol_cosine_cross store for the pair (metric = B200MOL_METRIC_*), so two empty fingerprints are at distance 1.
@@ -298,6 +322,14 @@ int b200mol_butina_dense(const double* d_dist, size_t n, double cutoff, int32_t*
 int b200mol_morgan(const int32_t* d_atom_starts, const int32_t* d_bond_starts, const uint32_t* d_atom_inv,
                    const uint32_t* d_bond_inv, const uint16_t* d_bond_a, const uint16_t* d_bond_b, size_t nMols,
                    int maxAtomsPerMol, int maxBondsPerMol, int radius, int fpBits, uint32_t* d_out, void* stream);
+/* Morgan count fingerprints: the arguments, checks, launch shapes and sync of b200mol_morgan, writing
+ * d_out int32[nMols][fpBits] (overwritten): d_out[i][j] is the number of accepted environments of molecule i whose code
+ * is congruent to j mod fpBits (every atom at radius 0; an environment whose bond set an earlier or equal one already
+ * had does not count). A bin is non-zero exactly where b200mol_morgan sets the bit. RDKit's GetCountFingerprintAsNumPy
+ * for GetMorganGenerator(radius, fpSize) with the options b200mol_morgan fixes. */
+int b200mol_morgan_counts(const int32_t* d_atom_starts, const int32_t* d_bond_starts, const uint32_t* d_atom_inv,
+                          const uint32_t* d_bond_inv, const uint16_t* d_bond_a, const uint16_t* d_bond_b, size_t nMols,
+                          int maxAtomsPerMol, int maxBondsPerMol, int radius, int fpBits, int32_t* d_out, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Batched force fields + BFGS (the conformer hot path).

@@ -45,6 +45,11 @@ SIGNATURES = {
                                        _vp, _vp]),
     "b200mol_tversky_threshold": (C.c_int, [_vp, C.c_size_t, _vp, C.c_size_t, C.c_int, C.c_double, C.c_double,
                                             C.c_double, _vp, _vp, _vp, C.c_uint64, C.POINTER(C.c_uint64), _vp]),
+    "b200mol_count_cross": (C.c_int, [_vp, C.c_size_t, _vp, C.c_size_t, C.c_int, C.c_double, C.c_double, _vp, _vp]),
+    "b200mol_count_topk": (C.c_int, [_vp, C.c_size_t, _vp, C.c_size_t, C.c_int, C.c_double, C.c_double, C.c_int, _vp,
+                                     _vp, _vp]),
+    "b200mol_count_threshold": (C.c_int, [_vp, C.c_size_t, _vp, C.c_size_t, C.c_int, C.c_double, C.c_double,
+                                          C.c_double, _vp, _vp, _vp, C.c_uint64, C.POINTER(C.c_uint64), _vp]),
     "b200mol_maxmin_pick": (C.c_int, [_vp, C.c_size_t, C.c_int, C.c_int, _vp, C.c_int, C.c_int, C.c_double, _vp, _vp,
                                       _vp]),
     "b200mol_leader_pick": (C.c_int, [_vp, C.c_size_t, C.c_int, C.c_int, C.c_double, _vp, C.c_int, C.c_int, _vp, _vp,
@@ -90,6 +95,8 @@ SIGNATURES = {
                                      _vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _vp, _vp, _vp, _vp]),
     "b200mol_morgan": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, _vp,
                                  _vp]),
+    "b200mol_morgan_counts": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int,
+                                        _vp, _vp]),
 }
 
 _lib = None

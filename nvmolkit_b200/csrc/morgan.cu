@@ -15,6 +15,7 @@
 // molecules (up to 1024 atoms and 1024 bonds at every radius, exactly: a slab of at most 256 MiB, include/b200mol.h) run
 // the same code with each warp's slab in a device scratch buffer (no CPU twin). An atom may have up to 16 bonds.
 #include <algorithm>
+#include <type_traits>
 
 #include "common.cuh"
 #include "options.cuh"
@@ -63,12 +64,19 @@ __host__ __device__ inline MorganLayout<Int> morganLayout(Int maxAtoms, Int maxB
   return L;
 }
 
+// What a molecule's accepted environments are written as: bits (kCounts false), u32[fpBits / 32] per molecule, set in the
+// slab's fp words and copied out at the end; or counts (true), int32[fpBits] per molecule, added straight into the
+// output row, which one warp owns. The slab layout is the same for both.
+template <bool kCounts>
+using MorganOut = std::conditional_t<kCounts, int32_t, uint32_t>;
+
 // One molecule, by one warp, in the slab at `slab` (shared or global memory).
+template <bool kCounts>
 __device__ __forceinline__ void morganMol(const int32_t* __restrict__ atomStarts, const int32_t* __restrict__ bondStarts,
                                           const uint32_t* __restrict__ atomInv, const uint32_t* __restrict__ bondInv,
                                           const uint16_t* __restrict__ bondA, const uint16_t* __restrict__ bondB,
                                           int mol, const MorganLayout<int>& L, uint8_t* slab, int maxAtoms,
-                                          int maxBonds, int radius, int fpBits, uint32_t* __restrict__ out,
+                                          int maxBonds, int radius, int fpBits, MorganOut<kCounts>* __restrict__ out,
                                           int* __restrict__ errFlag) {
   const int          lane    = threadIdx.x & 31;
   const int          fpWords = fpBits >> 5;
@@ -86,15 +94,26 @@ __device__ __forceinline__ void morganMol(const int32_t* __restrict__ atomStarts
 
   const int a0 = atomStarts[mol], nA = atomStarts[mol + 1] - a0;
   const int b0 = bondStarts[mol], nB = bondStarts[mol + 1] - b0;
-  uint32_t* outRow = out + static_cast<size_t>(mol) * fpWords;
+  const int           rowLen = kCounts ? fpBits : fpWords;
+  MorganOut<kCounts>* outRow = out + static_cast<size_t>(mol) * rowLen;
   if (nA > maxAtoms || nB > maxBonds) {
     if (lane == 0) atomicExch(errFlag, 1);
-    for (int w = lane; w < fpWords; w += 32) outRow[w] = 0;
+    for (int w = lane; w < rowLen; w += 32) outRow[w] = 0;
     return;
   }
+  // one environment accepted with code `code`
+  auto emit = [&](uint32_t code) {
+    const uint32_t bin = code % fpBits;
+    if constexpr (kCounts) atomicAdd(&outRow[bin], 1);
+    else atomicOr(&fp[bin >> 5], 1u << (bin & 31));
+  };
   const int bw = (maxBonds + 31) / 32 > 0 ? (maxBonds + 31) / 32 : 1;
 
-  for (int w = lane; w < fpWords; w += 32) fp[w] = 0;
+  if constexpr (kCounts) {
+    for (int w = lane; w < fpBits; w += 32) outRow[w] = 0;
+  } else {
+    for (int w = lane; w < fpWords; w += 32) fp[w] = 0;
+  }
   for (int a = lane; a <= nA; a += 32) adjStart[a] = 0;
   for (int a = lane; a < nA; a += 32) {
     inv[a]  = atomInv[a0 + a];
@@ -136,7 +155,7 @@ __device__ __forceinline__ void morganMol(const int32_t* __restrict__ atomStarts
     adjOther[s] = static_cast<uint16_t>(u);
   }
   // round 0
-  for (int a = lane; a < nA; a += 32) atomicOr(&fp[(inv[a] % fpBits) >> 5], 1u << ((inv[a] % fpBits) & 31));
+  for (int a = lane; a < nA; a += 32) emit(inv[a]);
   __syncwarp();
 
   int nSeen = 0;
@@ -215,8 +234,7 @@ __device__ __forceinline__ void morganMol(const int32_t* __restrict__ atomStarts
       if (accept) {
         const int slot = nSeen + newCount + __popc(m & ((1u << lane) - 1));
         for (int w = 0; w < bw; ++w) seen[slot * bw + w] = nbhdRound[a * bw + w];
-        const uint32_t bit = invNext[a] % fpBits;
-        atomicOr(&fp[bit >> 5], 1u << (bit & 31));
+        emit(invNext[a]);
       }
       newCount += __popc(m);
     }
@@ -230,31 +248,32 @@ __device__ __forceinline__ void morganMol(const int32_t* __restrict__ atomStarts
     nbhdRound   = t;
   }
   __syncwarp();
-  for (int w = lane; w < fpWords; w += 32) outRow[w] = fp[w];
+  if constexpr (!kCounts)
+    for (int w = lane; w < fpWords; w += 32) outRow[w] = fp[w];
   __syncwarp();  // every lane has read the slab before the warp's next molecule overwrites it
 }
 
 // kGlobalSlab == false: each warp of a CTA has its slab in dynamic shared memory, and the grid has a warp per molecule.
 // true: warp w of the grid has its slab at gslab + w * L.total in global memory and takes molecules w, w + (warps of the
 // grid), ... (molecules whose slab does not fit the shared-memory budget).
-template <bool kGlobalSlab>
+template <bool kGlobalSlab, bool kCounts>
 __global__ void morganKernel(const int32_t* __restrict__ atomStarts, const int32_t* __restrict__ bondStarts,
                              const uint32_t* __restrict__ atomInv, const uint32_t* __restrict__ bondInv,
                              const uint16_t* __restrict__ bondA, const uint16_t* __restrict__ bondB, int nMols,
                              int maxAtoms, int maxBonds, int radius, int fpBits, uint8_t* __restrict__ gslab,
-                             uint32_t* __restrict__ out, int* __restrict__ errFlag) {
+                             MorganOut<kCounts>* __restrict__ out, int* __restrict__ errFlag) {
   extern __shared__ __align__(16) uint8_t smem[];
   const int               wib  = threadIdx.x >> 5;
   const int               warp = blockIdx.x * (blockDim.x >> 5) + wib;
   const MorganLayout<int> L    = morganLayout<int>(maxAtoms, maxBonds, radius, fpBits >> 5);
   if constexpr (!kGlobalSlab) {
     if (warp < nMols)
-      morganMol(atomStarts, bondStarts, atomInv, bondInv, bondA, bondB, warp, L, smem + static_cast<size_t>(wib) * L.total,
+      morganMol<kCounts>(atomStarts, bondStarts, atomInv, bondInv, bondA, bondB, warp, L, smem + static_cast<size_t>(wib) * L.total,
                 maxAtoms, maxBonds, radius, fpBits, out, errFlag);
   } else {
     uint8_t* slab = gslab + static_cast<size_t>(warp) * L.total;
     for (int mol = warp; mol < nMols; mol += gridDim.x * (blockDim.x >> 5))
-      morganMol(atomStarts, bondStarts, atomInv, bondInv, bondA, bondB, mol, L, slab, maxAtoms, maxBonds, radius,
+      morganMol<kCounts>(atomStarts, bondStarts, atomInv, bondInv, bondA, bondB, mol, L, slab, maxAtoms, maxBonds, radius,
                 fpBits, out, errFlag);
   }
 }
@@ -264,10 +283,12 @@ __global__ void morganKernel(const int32_t* __restrict__ atomStarts, const int32
 
 using namespace b200;
 
-extern "C" int b200mol_morgan(const int32_t* d_atom_starts, const int32_t* d_bond_starts, const uint32_t* d_atom_inv,
-                              const uint32_t* d_bond_inv, const uint16_t* d_bond_a, const uint16_t* d_bond_b,
-                              size_t nMols, int maxAtomsPerMol, int maxBondsPerMol, int radius, int fpBits,
-                              uint32_t* d_out, void* stream) {
+// b200mol_morgan (bits) and b200mol_morgan_counts: the same checks, launch shapes and documented sync
+template <bool kCounts>
+static int morganEntry(const int32_t* d_atom_starts, const int32_t* d_bond_starts, const uint32_t* d_atom_inv,
+                       const uint32_t* d_bond_inv, const uint16_t* d_bond_a, const uint16_t* d_bond_b, size_t nMols,
+                       int maxAtomsPerMol, int maxBondsPerMol, int radius, int fpBits, MorganOut<kCounts>* d_out,
+                       void* stream) {
   return guarded([&] {
     B200_REQUIRE(fpBits > 0 && fpBits % 32 == 0, "fpBits must be a positive multiple of 32, got %d", fpBits);
     B200_REQUIRE(radius >= 0 && radius <= 16, "radius out of range: %d", radius);
@@ -292,12 +313,12 @@ extern "C" int b200mol_morgan(const int32_t* d_atom_starts, const int32_t* d_bon
       const size_t smemBytes = static_cast<size_t>(warps) * slabBytes;
       static size_t configured[kMaxDevices] = {};
       if (smemBytes > configured[currentDeviceSlot()]) {
-        B200_CUDA(cudaFuncSetAttribute(morganKernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        B200_CUDA(cudaFuncSetAttribute(morganKernel<false, kCounts>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        static_cast<int>(kSharedBudget)));
         configured[currentDeviceSlot()] = kSharedBudget;
       }
       const unsigned blocks = static_cast<unsigned>((nMols + warps - 1) / warps);
-      morganKernel<false><<<blocks, warps * 32, smemBytes, s>>>(d_atom_starts, d_bond_starts, d_atom_inv, d_bond_inv,
+      morganKernel<false, kCounts><<<blocks, warps * 32, smemBytes, s>>>(d_atom_starts, d_bond_starts, d_atom_inv, d_bond_inv,
                                                                  d_bond_a, d_bond_b, static_cast<int>(nMols), maxA, maxB,
                                                                  radius, fpBits, nullptr, d_out, err.get());
       B200_LAUNCHED();
@@ -311,7 +332,7 @@ extern "C" int b200mol_morgan(const int32_t* d_atom_starts, const int32_t* d_bon
       const int      perCta = static_cast<int>(std::min<long long>(warps, 8));
       const unsigned blocks = static_cast<unsigned>(warps / perCta);
       Scratch<uint8_t> slabs(static_cast<size_t>(blocks) * perCta * slabBytes, s);
-      morganKernel<true><<<blocks, perCta * 32, 0, s>>>(d_atom_starts, d_bond_starts, d_atom_inv, d_bond_inv, d_bond_a,
+      morganKernel<true, kCounts><<<blocks, perCta * 32, 0, s>>>(d_atom_starts, d_bond_starts, d_atom_inv, d_bond_inv, d_bond_a,
                                                         d_bond_b, static_cast<int>(nMols), maxA, maxB, radius, fpBits,
                                                         slabs.get(), d_out, err.get());
       B200_LAUNCHED();
@@ -323,4 +344,20 @@ extern "C" int b200mol_morgan(const int32_t* d_atom_starts, const int32_t* d_bon
     B200_REQUIRE(hErr != 1, "a molecule exceeds maxAtomsPerMol/maxBondsPerMol");
     B200_REQUIRE(hErr != 2, "an atom has more than %d bonds", kMaxDeg);
   });
+}
+
+extern "C" int b200mol_morgan(const int32_t* d_atom_starts, const int32_t* d_bond_starts, const uint32_t* d_atom_inv,
+                              const uint32_t* d_bond_inv, const uint16_t* d_bond_a, const uint16_t* d_bond_b,
+                              size_t nMols, int maxAtomsPerMol, int maxBondsPerMol, int radius, int fpBits,
+                              uint32_t* d_out, void* stream) {
+  return morganEntry<false>(d_atom_starts, d_bond_starts, d_atom_inv, d_bond_inv, d_bond_a, d_bond_b, nMols, maxAtomsPerMol,
+                            maxBondsPerMol, radius, fpBits, d_out, stream);
+}
+
+extern "C" int b200mol_morgan_counts(const int32_t* d_atom_starts, const int32_t* d_bond_starts, const uint32_t* d_atom_inv,
+                                     const uint32_t* d_bond_inv, const uint16_t* d_bond_a, const uint16_t* d_bond_b,
+                                     size_t nMols, int maxAtomsPerMol, int maxBondsPerMol, int radius, int fpBits,
+                                     int32_t* d_out, void* stream) {
+  return morganEntry<true>(d_atom_starts, d_bond_starts, d_atom_inv, d_bond_inv, d_bond_a, d_bond_b, nMols, maxAtomsPerMol,
+                           maxBondsPerMol, radius, fpBits, d_out, stream);
 }

@@ -1,6 +1,7 @@
 // Internal interface of the fingerprint-similarity stack: the measure of a call, the N x M popcount tiles that serve it
 // (tanimoto.cu: SIMT, tanimoto_tc.cu: wgmma) and the fp64 value of a pair from its integer counts.
 #pragma once
+#include <cstddef>
 #include <cstdint>
 
 #include "common.cuh"
@@ -132,5 +133,14 @@ bool topkTileEligible(int words);  // the tile takes widths that are multiples o
 void launchTopkTile(const Measure& m, const uint8_t* expQ, size_t nQ, const int32_t* popQ, const uint8_t* expLib, size_t nCols,
                     const int32_t* popCols, int words, const int4* bar, uint32_t* cand, uint32_t* count, uint32_t cap,
                     uint32_t colBase, cudaStream_t s);
+
+// ---- threshold search: the assembly of threshold.cu, steps (b) to (d) ----
+// list[0 .. listed) the listed pairs (i, j) (i = -1: dropped) with their values vals[], nnz the entries they give (kept
+// pairs, twice in a symmetric search, plus one diagonal entry per row of popX > 0 then): written to the caller's CSR
+// indptr [nX + 1], indices / values [nnz], columns ascending. nCols: the column count; stat: threshold.cu's four
+// counters, of which stat[3], zero on entry, is the fill cursor.
+void assembleThresholdCsr(const int2* list, const double* vals, unsigned long long listed, bool symmetric, const int32_t* popX,
+                          size_t nX, size_t nCols, MeasureKind kind, unsigned long long nnz, unsigned long long* stat,
+                          int64_t* indptr, int32_t* indices, double* values, cudaStream_t s);
 
 }  // namespace b200

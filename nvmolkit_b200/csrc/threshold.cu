@@ -227,13 +227,22 @@ void thresholdSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t n
   *hNnz                           = nnz;
   if (nnz > cap) return;  // the caller asks again with room for nnz
 
-  PhaseTimer                  timer("threshold_assembly", s);
-  const int                   colBits = bitsFor(self ? nQ : nLib), endBit = std::max(1, colBits + bitsFor(nQ));
+  PhaseTimer timer("threshold_assembly", s);
+  assembleThresholdCsr(list.get(), vals.get(), listed, self, popQ.get(), nQ, self ? nQ : nLib, m.kind, nnz, stat.get(), indptr,
+                       indices, values, s);
+}
+
+}  // namespace
+
+void assembleThresholdCsr(const int2* list, const double* vals, unsigned long long listed, bool symmetric, const int32_t* popX,
+                          size_t nX, size_t nCols, MeasureKind kind, unsigned long long nnz, unsigned long long* stat,
+                          int64_t* indptr, int32_t* indices, double* values, cudaStream_t s) {
+  const int                   colBits = bitsFor(nCols), endBit = std::max(1, colBits + bitsFor(nX));
   Scratch<unsigned long long> keysIn(nnz, s), keysOut(nnz, s);
   Scratch<double>             valsIn(nnz, s);
-  if (listed + (self ? nQ : 0) > 0) {
-    fillKernel<<<blocksFor(listed + (self ? nQ : 0), 256), 256, 0, s>>>(list.get(), vals.get(), listed, self ? 1 : 0, popQ.get(), nQ,
-                                                                        m.kind, colBits, keysIn.get(), valsIn.get(), stat.get());
+  if (listed + (symmetric ? nX : 0) > 0) {
+    fillKernel<<<blocksFor(listed + (symmetric ? nX : 0), 256), 256, 0, s>>>(list, vals, listed, symmetric ? 1 : 0, popX, nX, kind,
+                                                                             colBits, keysIn.get(), valsIn.get(), stat);
     B200_LAUNCHED();
   }
   if (nnz) {
@@ -244,11 +253,10 @@ void thresholdSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t n
     B200_CUDA(cub::DeviceRadixSort::SortPairs(tmp.get(), tmpBytes, keysIn.get(), keysOut.get(), valsIn.get(), values, n, 0, endBit, s));
     g_launchCount.fetch_add(1);
   }
-  csrKernel<<<blocksFor(std::max<unsigned long long>(nnz, nQ + 1), 256), 256, 0, s>>>(keysOut.get(), nnz, nQ, colBits, indices, indptr);
+  csrKernel<<<blocksFor(std::max<unsigned long long>(nnz, nX + 1), 256), 256, 0, s>>>(keysOut.get(), nnz, nX, colBits, indices, indptr);
   B200_LAUNCHED();
 }
 
-}  // namespace
 }  // namespace b200
 
 using namespace b200;

@@ -127,6 +127,9 @@ PYBIND11_MODULE(_core, m) {
   DEF(b200mol_tversky_cross_host);
   DEF(b200mol_tversky_topk);
   DEF(b200mol_tversky_threshold);
+  DEF(b200mol_count_cross);
+  DEF(b200mol_count_topk);
+  DEF(b200mol_count_threshold);
   DEF(b200mol_maxmin_pick);
   DEF(b200mol_leader_pick);
   DEF(b200mol_butina_fused);
@@ -134,6 +137,7 @@ PYBIND11_MODULE(_core, m) {
   DEF(b200mol_butina_from_edges);
   DEF(b200mol_butina_dense);
   DEF(b200mol_morgan);
+  DEF(b200mol_morgan_counts);
   DEF(b200mol_schedule_waves);
   DEF(b200mol_dg_terms_from_bounds);
   DEF(b200mol_etk_terms_from_details);

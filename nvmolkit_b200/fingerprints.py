@@ -51,14 +51,25 @@ class MorganFingerprintGenerator:
         sptr = stream_ptr(stream)
         require_cuda()
         batch = mols if isinstance(mols, MolGraphBatch) else from_rdkit(list(mols))
-        return AsyncGpuResult(self._run(batch, stream, sptr))
+        return AsyncGpuResult(self._run(batch, stream, sptr, "b200mol_morgan", self.fpSize // 32))
 
-    def _run(self, batch: MolGraphBatch, stream, sptr: int) -> torch.Tensor:
+    def GetCountFingerprints(self, mols, num_threads: int = 0,
+                             stream: torch.cuda.Stream | None = None) -> AsyncGpuResult:
+        """Count twin of ``GetFingerprints``: int32 (n, fpSize), row i, bin j the number of accepted environments of
+        molecule i whose code is j modulo fpSize (every atom at radius 0; an environment whose bond set an earlier one
+        already had does not count). RDKit's ``GetCountFingerprintAsNumPy`` of ``GetMorganGenerator(radius, fpSize)``;
+        ``pack_fingerprint(counts > 0)`` is ``GetFingerprints`` bit for bit. Same inputs, size classes and refusals."""
+        sptr = stream_ptr(stream)
+        require_cuda()
+        batch = mols if isinstance(mols, MolGraphBatch) else from_rdkit(list(mols))
+        return AsyncGpuResult(self._run(batch, stream, sptr, "b200mol_morgan_counts", self.fpSize))
+
+    def _run(self, batch: MolGraphBatch, stream, sptr: int, entry: str, width: int) -> torch.Tensor:
+        """(n, width) int32 from ``entry`` (b200mol_morgan or b200mol_morgan_counts), one call per size class"""
         n = len(batch)
-        words = self.fpSize // 32
         dev = torch.device("cuda", torch.cuda.current_device())
         with stream_ctx(stream):
-            out = torch.empty((n, words), dtype=torch.int32, device=dev)
+            out = torch.empty((n, width), dtype=torch.int32, device=dev)
             if n == 0:
                 return out
             size = np.maximum(batch.atoms_per_mol, batch.bonds_per_mol)
@@ -69,8 +80,8 @@ class MorganFingerprintGenerator:
                 t = [torch.from_numpy(a.view(np.int32) if a.dtype == np.uint32 else
                                       (a.view(np.int16) if a.dtype == np.uint16 else a)).to(dev, non_blocking=True)
                      for a in (sub.atom_starts, sub.bond_starts, sub.atom_inv, sub.bond_inv, sub.bond_a, sub.bond_b)]
-                dst = out if len(idx) == n else torch.empty((len(idx), words), dtype=torch.int32, device=dev)
-                _lib.call("b200mol_morgan", t[0].data_ptr(), t[1].data_ptr(), t[2].data_ptr(), t[3].data_ptr(),
+                dst = out if len(idx) == n else torch.empty((len(idx), width), dtype=torch.int32, device=dev)
+                _lib.call(entry, t[0].data_ptr(), t[1].data_ptr(), t[2].data_ptr(), t[3].data_ptr(),
                           t[4].data_ptr(), t[5].data_ptr(), len(idx), int(sub.atoms_per_mol.max(initial=0)),
                           int(sub.bonds_per_mol.max(initial=0)), self.radius, self.fpSize, dst.data_ptr(), sptr)
                 if dst is not out:

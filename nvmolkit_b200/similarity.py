@@ -8,7 +8,7 @@ import numpy as np
 import torch
 
 from nvmolkit_b200 import _lib
-from nvmolkit_b200._interop import fingerprint_matrix, require_cuda, stream_ctx, stream_ptr
+from nvmolkit_b200._interop import as_tensor, fingerprint_matrix, require_cuda, stream_ctx, stream_ptr
 from nvmolkit_b200.types import AsyncGpuResult
 
 
@@ -277,3 +277,163 @@ def crossTverskySimilarityMemoryConstrained(fingerprint_group_one, fingerprint_g
     """Host-in / host-out Tversky matrix as a NumPy array, computed in row blocks with overlapped D2H."""
     weights = _check_weights(alpha, beta)
     return _cross_host(weights, fingerprint_group_one, fingerprint_group_two)
+
+
+# ---- count vectors ----
+# The measures above on count vectors (RDKit's SparseIntVect similarities, e.g. of GetCountFingerprint): with a the sum
+# of the row's counts (group one), b the column's and c = sum over bins of min(row, column), the value is the Tversky
+# expression above of (c, a, b). Tanimoto is (1, 1): c / (a + b - c); Dice (1/2, 1/2): 2c / (a + b); both bit for bit
+# RDKit's, every intermediate an exact integer. The module's note on non-dyadic Tversky weights applies unchanged.
+# Counts must lie in 0 .. 65535 (every sum then fits int32 and is exact in fp64); that is checked on the device and its
+# flag read once, so every count call synchronises its stream, and a count out of range raises ValueError.
+COUNT_MAX_BINS = 4096
+COUNT_MAX = 65535
+_COUNT_DTYPES = (torch.uint8, torch.int16, torch.int32)
+TANIMOTO = (1.0, 1.0)
+
+
+def _count_matrix(obj, name: str) -> torch.Tensor:
+    t = as_tensor(obj)
+    if not t.is_cuda:
+        raise ValueError(f"{name} must be a CUDA tensor")
+    if t.dtype not in _COUNT_DTYPES:
+        raise ValueError(f"{name} must have dtype uint8, int16 or int32 (counts), got {t.dtype}")
+    if t.ndim != 2:
+        raise ValueError(f"{name} must be 2D, got shape={tuple(t.shape)}")
+    if not 1 <= t.shape[1] <= COUNT_MAX_BINS:
+        raise ValueError(f"{name} must have 1 to {COUNT_MAX_BINS} bins, got {t.shape[1]}")
+    return t
+
+
+def _count_operands(one, two):
+    """Both count matrices, checked (b None: group one against itself)."""
+    require_cuda()
+    a = _count_matrix(one, "fingerprint_group_one")
+    b = None if two is None else _count_matrix(two, "fingerprint_group_two")
+    if b is not None and a.shape[1] != b.shape[1]:
+        raise ValueError(f"count vector widths differ: {a.shape[1]} vs {b.shape[1]} bins")
+    return a, b
+
+
+def _int32(*xs):
+    """the count matrices as the binding passes them (on the call's stream, after every check)"""
+    return tuple(None if x is None else x.to(torch.int32).contiguous() for x in xs)
+
+
+def _count_cross(weights, one, two, stream) -> AsyncGpuResult:
+    sptr = stream_ptr(stream)
+    a, b = _count_operands(one, two)
+    n_b = a.shape[0] if b is None else b.shape[0]
+    with stream_ctx(stream):
+        a, b = _int32(a, b)
+        out = torch.empty((a.shape[0], n_b), dtype=torch.float64, device=a.device)
+        _lib.call("b200mol_count_cross", a.data_ptr(), a.shape[0], None if b is None else b.data_ptr(), n_b, a.shape[1],
+                  *weights, out.data_ptr(), sptr)
+        _keep_alive(a, b)
+    return AsyncGpuResult(out)
+
+
+def _count_topk(weights, one, two, k, stream):
+    sptr = stream_ptr(stream)
+    a, b = _count_operands(one, two)
+    n_b = a.shape[0] if b is None else b.shape[0]
+    k = _check_k(k, n_b)
+    with stream_ctx(stream):
+        a, b = _int32(a, b)
+        values = torch.empty((a.shape[0], k), dtype=torch.float64, device=a.device)
+        indices = torch.empty((a.shape[0], k), dtype=torch.int32, device=a.device)
+        _lib.call("b200mol_count_topk", a.data_ptr(), a.shape[0], None if b is None else b.data_ptr(), n_b,
+                  a.shape[1], *weights, k, values.data_ptr(), indices.data_ptr(), sptr)
+        _keep_alive(a, b)
+    return AsyncGpuResult(values), AsyncGpuResult(indices)
+
+
+def _count_threshold(weights, one, two, threshold, stream):
+    t = _check_threshold(threshold)
+    sptr = stream_ptr(stream)
+    a, b = _count_operands(one, two)
+    n_q, n_lib = a.shape[0], (a.shape[0] if b is None else b.shape[0])
+    with stream_ctx(stream):
+        a, b = _int32(a, b)
+        if n_q == 0 or n_lib == 0:  # no pair
+            return (AsyncGpuResult(torch.zeros(n_q + 1, dtype=torch.int64, device=a.device)),
+                    AsyncGpuResult(torch.empty(0, dtype=torch.int32, device=a.device)),
+                    AsyncGpuResult(torch.empty(0, dtype=torch.float64, device=a.device)))
+        indptr = torch.empty(n_q + 1, dtype=torch.int64, device=a.device)
+        # a first guess at the result size; a larger result is reported and the call is made once more with room for it
+        cap = min(max(1 << 20, 64 * n_q), n_q * n_lib)
+        for _ in range(2):
+            indices = torch.empty(cap, dtype=torch.int32, device=a.device)
+            values = torch.empty(cap, dtype=torch.float64, device=a.device)
+            nnz = C.c_uint64(0)
+            _lib.call("b200mol_count_threshold", a.data_ptr(), n_q, None if b is None else b.data_ptr(), n_lib,
+                      a.shape[1], *weights, t, indptr.data_ptr(), indices.data_ptr(), values.data_ptr(), cap,
+                      C.byref(nnz), sptr)
+            if nnz.value <= cap:
+                break
+            cap = int(nnz.value)
+        _keep_alive(a, b)
+    n = int(nnz.value)
+    return AsyncGpuResult(indptr), AsyncGpuResult(indices[:n]), AsyncGpuResult(values[:n])
+
+
+def crossTanimotoCountSimilarity(fingerprint_group_one, fingerprint_group_two=None, stream=None) -> AsyncGpuResult:
+    """(n, m) fp64 Tanimoto similarities of count vectors, c / (a + b - c) with a, b the row sums and c the sum of the
+    bin-wise minima (0 when c == 0), RDKit's ``TanimotoSimilarity`` on count fingerprints bit for bit; all-to-all within
+    group one when group two is None. Inputs: 2D uint8, int16 or int32 CUDA tensors (or ``AsyncGpuResult``) of counts in
+    ``0 .. 65535``, 1 to 4096 bins, e.g. ``GetCountFingerprints``. Synchronises ``stream`` (the range check)."""
+    return _count_cross(TANIMOTO, fingerprint_group_one, fingerprint_group_two, stream)
+
+
+def crossDiceCountSimilarity(fingerprint_group_one, fingerprint_group_two=None, stream=None) -> AsyncGpuResult:
+    """Dice twin of ``crossTanimotoCountSimilarity``: 2c / (a + b), RDKit's ``DiceSimilarity`` on count fingerprints
+    bit for bit. Synchronises ``stream``."""
+    return _count_cross(DICE, fingerprint_group_one, fingerprint_group_two, stream)
+
+
+def crossTverskyCountSimilarity(fingerprint_group_one, fingerprint_group_two=None, *, alpha, beta,
+                                stream=None) -> AsyncGpuResult:
+    """Tversky twin of ``crossTanimotoCountSimilarity``: c / ((alpha (a - c) + beta (b - c)) + c), alpha weighting what
+    only the row (group one) has. ``0 <= alpha, beta <= 1000``. See the module note on RDKit parity. Synchronises
+    ``stream``."""
+    weights = _check_weights(alpha, beta)  # (before anything touches the device)
+    return _count_cross(weights, fingerprint_group_one, fingerprint_group_two, stream)
+
+
+def topKTanimotoCountSimilarity(fingerprint_group_one, fingerprint_group_two=None, k=10, stream=None):
+    """For each count vector of group one its k most similar of group two (of group one itself, self-matches included,
+    when None): ``(values, indices)``, fp64 and int32 ``[Q, k]``, the first k columns of each row of
+    ``crossTanimotoCountSimilarity`` ordered by (value descending, column ascending), values bit-identical to the matrix.
+    The matrix is never stored. ``1 <= k <= min(len(library), TOPK_MAX)``. Synchronises ``stream`` (the range check)."""
+    return _count_topk(TANIMOTO, fingerprint_group_one, fingerprint_group_two, k, stream)
+
+
+def topKDiceCountSimilarity(fingerprint_group_one, fingerprint_group_two=None, k=10, stream=None):
+    """Dice twin of ``topKTanimotoCountSimilarity``: rows of ``crossDiceCountSimilarity``."""
+    return _count_topk(DICE, fingerprint_group_one, fingerprint_group_two, k, stream)
+
+
+def topKTverskyCountSimilarity(fingerprint_group_one, fingerprint_group_two=None, k=10, *, alpha, beta, stream=None):
+    """Tversky twin of ``topKTanimotoCountSimilarity``: rows of ``crossTverskyCountSimilarity``."""
+    weights = _check_weights(alpha, beta)
+    return _count_topk(weights, fingerprint_group_one, fingerprint_group_two, k, stream)
+
+
+def thresholdTanimotoCountSimilarity(fingerprint_group_one, fingerprint_group_two=None, *, threshold, stream=None):
+    """Every pair of count vectors at or above a Tanimoto threshold, as CSR ``(indptr, indices, values)``, int64
+    ``[Q + 1]``, int32 and fp64 ``[nnz]``: row q lists exactly the columns whose ``crossTanimotoCountSimilarity`` entry
+    is ``>= threshold``, ascending, with those values (group two None: group one against itself, self-matches
+    included). ``0 < threshold <= 1``. The matrix is never stored. Synchronises ``stream``."""
+    return _count_threshold(TANIMOTO, fingerprint_group_one, fingerprint_group_two, threshold, stream)
+
+
+def thresholdDiceCountSimilarity(fingerprint_group_one, fingerprint_group_two=None, *, threshold, stream=None):
+    """Dice twin of ``thresholdTanimotoCountSimilarity``: entries of ``crossDiceCountSimilarity``."""
+    return _count_threshold(DICE, fingerprint_group_one, fingerprint_group_two, threshold, stream)
+
+
+def thresholdTverskyCountSimilarity(fingerprint_group_one, fingerprint_group_two=None, *, alpha, beta, threshold,
+                                    stream=None):
+    """Tversky twin of ``thresholdTanimotoCountSimilarity``: entries of ``crossTverskyCountSimilarity``."""
+    weights = _check_weights(alpha, beta)
+    return _count_threshold(weights, fingerprint_group_one, fingerprint_group_two, threshold, stream)

@@ -9,6 +9,8 @@ and commit the resulting .npz. `tests/test_rdkit_fixtures.py` then replays it (s
   * Morgan: the flattened molecular graphs + RDKit's own ECFP bits (radius 0..3, 2048 bits)   -> oracle / GPU bit-exact
   * Tanimoto: RDKit BulkTanimotoSimilarity matrix of those bit vectors                         -> bit-exact (fp64)
   * Butina: RDKit ML.Cluster.Butina.ClusterData(reordering=True) on the distance matrix        -> identical clusters
+  * Morgan counts: GetCountFingerprintAsNumPy (radius 0..3, 2048 bins), and BulkTanimotoSimilarity /
+    BulkDiceSimilarity of the radius-2 count fingerprints (tests/test_count_*.py)              -> bit-exact
   * MMFF / UFF: the flattened term tables (nvmolkit_b200.rdkit_adapter) + RDKit's energies, gradients and 200-iteration
     minimised energies on the same conformers (tests/test_mmff.cu:1521-1608 style)              -> <= 1e-4 relative
   * ETKDG: raw + smoothed bounds matrices, flattened DG / ETK / check tables, RDKit's EmbedMultipleConfs coordinates
@@ -100,6 +102,14 @@ def main() -> None:
         key = str(cutoff).replace(".", "p")
         out[f"butina_ids_{key}"] = ids
         out[f"butina_centroids_{key}"] = np.array([c[0] for c in clusters], dtype=np.int32)
+
+    # ---- Morgan counts, and Tanimoto / Dice on count vectors (tests/test_count_fingerprints.py, _similarity.py)
+    for radius in range(4):
+        gen = rdFingerprintGenerator.GetMorganGenerator(radius=radius, fpSize=2048)
+        out[f"morgan_counts_r{radius}"] = np.stack([gen.GetCountFingerprintAsNumPy(m) for m in mols]).astype(np.int32)
+    cfps = [rdFingerprintGenerator.GetMorganGenerator(radius=2, fpSize=2048).GetCountFingerprint(m) for m in mols]
+    out["count_tanimoto_r2"] = np.array([DataStructs.BulkTanimotoSimilarity(cfps[i], cfps) for i in range(n)])
+    out["count_dice_r2"] = np.array([DataStructs.BulkDiceSimilarity(cfps[i], cfps) for i in range(n)])
 
     # ---- conformers, MMFF / UFF
     hmols = []
