@@ -103,7 +103,8 @@ int b200mol_set_option(const char* key, long long value);
  * "leader_block_pairs_last" (pairs the resolver compared against earlier picks of the same window / of the same block;
  * these two synchronise the device). Of the last b200mol_conformer_rmsd_mapped: "rmsd_match_chunks_last" (chunks of
  * mappings it ran). Of the last b200mol_morgan that launched: "morgan_global_slab_last" (1: the per-molecule slabs were
- * in device memory, 0: in shared memory). */
+ * in device memory, 0: in shared memory). Of the last b200mol_count_neighbor_edges over at least one vector:
+ * "count_neighbor_pairs_last" (pairs (i, j), i < j, its pass compared after the sum band; synchronises the device). */
 int b200mol_get_option(const char* key, long long* value);
 /* Per-phase CUDA-event timing inside the library (off by default). Phases: "neighbor_pass" (the N^2 tile kernel
  * alone), "csr_build", "cluster_loop", "bfgs". b200mol_profile_read waits for the phase's stop event. */
@@ -294,6 +295,28 @@ int b200mol_neighbor_edges(const uint32_t* d_fp, size_t n, int words, int metric
 int b200mol_butina_from_edges(size_t n, int32_t* d_counts, const int32_t* d_edges, uint64_t n_edges,
                               int32_t* d_cluster_ids, int32_t* d_centroids, int32_t* d_n_clusters,
                               int32_t* h_n_clusters, void* stream);
+/* The two stages and the whole of Butina on COUNT vectors (the rows, bins, count range and refusals of b200mol_count_*):
+ * points i != j are neighbours iff 1.0 - s(i, j) <= cutoff in fp64, s the value b200mol_count_cross stores for the pair
+ * with (alpha, beta) = (1, 1) (Tanimoto) or (0.5, 0.5) (Dice); any other weights, and a cutoff outside [0, 1], are
+ * B200MOL_ERR_INVALID before any device work. Ids and centroids are those of b200mol_butina_dense on the matrix
+ * 1.0 - s. No similarity matrix is stored: O(N + edges) memory.
+ *   b200mol_count_neighbor_edges  d_counts[n] += degrees, d_edges (i, j), i < j, the caller's indices; the edge_cap /
+ *                                 *h_n_edges protocol of b200mol_neighbor_edges. It SYNCHRONISES `stream` once for the
+ *                                 range check and the list sizes (as b200mol_count_*; a count out of range is refused
+ *                                 then, with nothing written) and, when h_n_edges is not NULL, once for the edge total.
+ *   b200mol_count_butina_fused    as b200mol_butina_fused: an edge list of 64 per point, one rerun at the exact size for
+ *                                 a denser graph, then b200mol_butina_from_edges; it synchronises for the range check,
+ *                                 the edge total and, when h_n_clusters is not NULL, *h_n_clusters.
+ * The pass visits each unordered pair at most once, with the rows in (sum, index) order, and skips the pairs that a sum
+ * bound rules out (csrc/count_similarity.cu); option "count_neighbor_pairs_last" reports how many it compared. Scratch
+ * is stream-ordered: that of b200mol_count_*, about 24 bytes per row for the order and 20 bytes per block of 32 rows (16
+ * above 2048 bins) for the band; the fused call adds 8 bytes per edge and 12 per point, and b200mol_butina_from_edges's. */
+int b200mol_count_neighbor_edges(const int32_t* d_x, size_t n, int bins, double alpha, double beta, double cutoff,
+                                 int32_t* d_counts /* [n], += degrees */, int32_t* d_edges /* [cap][2], i < j */,
+                                 uint64_t edge_cap, uint64_t* h_n_edges, void* stream);
+int b200mol_count_butina_fused(const int32_t* d_x, size_t n, int bins, double alpha, double beta, double cutoff,
+                               int32_t* d_cluster_ids, int32_t* d_centroids, int32_t* d_n_clusters, int32_t* h_n_clusters,
+                               void* stream);
 /* Dense fp64 distance matrix in (neighbours: dist <= cutoff, src/butina.cu:1043-1051).
  * Replaces butinaGpu (src/butina.h:45-50, src/butina.cu:914-1071). */
 int b200mol_butina_dense(const double* d_dist, size_t n, double cutoff, int32_t* d_cluster_ids, int32_t* d_centroids,

@@ -50,6 +50,10 @@ SIGNATURES = {
                                      _vp, _vp]),
     "b200mol_count_threshold": (C.c_int, [_vp, C.c_size_t, _vp, C.c_size_t, C.c_int, C.c_double, C.c_double,
                                           C.c_double, _vp, _vp, _vp, C.c_uint64, C.POINTER(C.c_uint64), _vp]),
+    "b200mol_count_neighbor_edges": (C.c_int, [_vp, C.c_size_t, C.c_int, C.c_double, C.c_double, C.c_double, _vp, _vp,
+                                               C.c_uint64, C.POINTER(C.c_uint64), _vp]),
+    "b200mol_count_butina_fused": (C.c_int, [_vp, C.c_size_t, C.c_int, C.c_double, C.c_double, C.c_double, _vp, _vp, _vp,
+                                             _vp, _vp]),
     "b200mol_maxmin_pick": (C.c_int, [_vp, C.c_size_t, C.c_int, C.c_int, _vp, C.c_int, C.c_int, C.c_double, _vp, _vp,
                                       _vp]),
     "b200mol_leader_pick": (C.c_int, [_vp, C.c_size_t, C.c_int, C.c_int, C.c_double, _vp, C.c_int, C.c_int, _vp, _vp,

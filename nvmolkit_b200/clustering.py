@@ -133,6 +133,54 @@ def fused_butina(x, cutoff: float, return_centroids: bool = False, stream=None, 
     return clusters, sizes
 
 
+_COUNT_METRICS = {"tanimoto": (1.0, 1.0), "dice": (0.5, 0.5)}  # (alpha, beta) of b200mol_count_butina_fused
+
+
+def fused_butina_counts_device(x, cutoff: float, stream=None, metric: str = "tanimoto"):
+    """Device-resident result of :func:`fused_butina_counts`: (ids int32[N], centroids int32[nClusters])."""
+    from nvmolkit_b200 import similarity
+
+    if metric not in _COUNT_METRICS:
+        raise ValueError(f"metric must be one of {sorted(_COUNT_METRICS)} on count vectors, got {metric!r}")
+    if not 0.0 <= cutoff <= 1.0:
+        raise ValueError(f"cutoff must be in [0, 1], got {cutoff}")
+    sptr = stream_ptr(stream)
+    x = similarity._count_matrix(x, "x")
+    require_cuda()
+    n = x.shape[0]
+    with stream_ctx(stream):
+        (x,) = similarity._int32(x)
+        ids = torch.empty(n, dtype=torch.int32, device=x.device)
+        cen = torch.empty(max(n, 1), dtype=torch.int32, device=x.device)
+        ncl = torch.zeros(1, dtype=torch.int32, device=x.device)
+        _lib.call("b200mol_count_butina_fused", x.data_ptr(), n, x.shape[1], *_COUNT_METRICS[metric], float(cutoff),
+                  ids.data_ptr(), cen.data_ptr(), ncl.data_ptr(), None, sptr)
+        x.record_stream(torch.cuda.current_stream())
+        k = int(ncl.item())
+    return ids, cen[:k]
+
+
+def fused_butina_counts(x, cutoff: float, return_centroids: bool = False, stream=None, metric: str = "tanimoto"):
+    """Butina straight from count fingerprints (e.g. ``GetCountFingerprints``), O(N + edges) memory: the similarity
+    matrix is never stored. Returns ``(clusters, cluster_sizes[, centroids])`` like :func:`fused_butina`.
+
+    ``x``: a 2D uint8, int16 or int32 CUDA tensor (or ``AsyncGpuResult``) of counts in ``0 .. 65535``, 1 to 4096 bins,
+    as the count similarity calls take it. ``metric``: ``"tanimoto"`` or ``"dice"``. Points i != j are neighbours iff
+    ``1.0 - s(i, j) <= cutoff`` in fp64, s the value ``crossTanimotoCountSimilarity`` / ``crossDiceCountSimilarity``
+    stores for the pair, so ids and centroids equal, bit for bit, those of
+    ``butina(1.0 - crossTanimotoCountSimilarity(x).torch(), cutoff, return_centroids=True)`` (Dice alike), which needs
+    N^2 fp64 values. Ties go to the highest index; cluster 0 is the largest.
+
+    Synchronises ``stream``: once for the count range check (a count out of range raises ``ValueError``), once for the
+    edge total, a rerun of the pass when the graph has more than 64 edges per point, and once for the cluster count.
+    """
+    ids, cen = fused_butina_counts_device(x, cutoff, stream=stream, metric=metric)
+    clusters, sizes = clusters_from_ids(ids.cpu().numpy(), cen.cpu().numpy())
+    if return_centroids:
+        return clusters, sizes, cen.cpu().numpy().tolist()
+    return clusters, sizes
+
+
 def clusters_from_ids(ids_h, cen_h):
     """(cluster ids [N], centroids [K]) -> the reference's output format (nvmolkit/clustering.py:171-189): list of
     tuples, centroid first then the other members in ascending index order, and the cumulative sizes starting at 0.

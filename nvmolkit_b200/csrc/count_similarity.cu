@@ -17,12 +17,33 @@
 //                 select that merges a row's slots into its list, and a scan that redoes a slab for the rows whose
 //                 candidates did not fit;
 //     threshold   a pair with value >= t is listed with its value; threshold.cu's assembly (keys, one radix sort,
-//                 indptr by bisection) makes the CSR. A self search runs the full pass (it needs no diagonal step).
+//                 indptr by bisection) makes the CSR. A self search runs the full pass (it needs no diagonal step);
+//     neighbours  (Butina: b200mol_count_neighbor_edges, Tanimoto and Dice only) a self pass over the rows compacted
+//                 in (row sum, index) order (a stable radix sort; the stats and pack kernels gather through it). Query
+//                 block [q0, q0 + QB) visits only columns >= q0, and in its own block only col > row, so each
+//                 unordered pair is tested once; a pair with 1 - value <= cutoff (fp64) adds to both degrees and is
+//                 written as the caller's (i, j), i < j.
 // Query blocks are 32 rows up to 2048 bins and 16 rows above, where a warp takes two library rows at a time (half a
 // warp each), so that the block stays within 128 KiB of shared memory.
+//
+// The sum band of the neighbour pass (exact). For Tanimoto and Dice the value is the correctly rounded quotient of
+// exact integers, c / (a + b - c) or c / ((a + b) / 2), every intermediate exact (sums < 2^31). For a row of sum a and
+// a column of sum b >= a, c <= min(a, b) = a, and the exact quotient grows with c and, c fixed, falls as a falls, so it
+// is at most that of (c = a, a, b), which for A >= a is at most that of (c = A, a = A, b) (A / b, 2A / (A + b): both
+// grow with A). Rounding to nearest is monotone, so value(c, a, b) <= value(A, A, b); and RN(1 - s) does not increase
+// as s grows. Let A be the largest sum of a query block (its last row, in sum order). Every column past the block has
+// b >= A, and value(A, A, b) does not increase as b grows (A / b, 2A / (A + b)). So once
+// 1 - value(A, A, b) <= cutoff fails at a sorted column, it fails at every later one, and no row of the block has a
+// neighbour there. countBandKernel bisects the sorted sums once per block for the first such column; the block's
+// columns end there. (A = 0: every value of the block is 0, and the band is everything at cutoff 1, else nothing past
+// the block.) The bound and the kernel's value are the same tverskyFromCounts of intrinsics, never contracted into an
+// FMA, and the comparison is __dsub_rn. The band's lengths differ widely from block to block, so the pass takes work
+// from a flat list of (block, kUnitCols-column chunk) units, a persistent grid walking it in order.
 #include <algorithm>
+#include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
+#include "options.cuh"
 #include "similarity.cuh"
 #include "topk.cuh"
 
@@ -36,7 +57,12 @@ constexpr int kTileCols  = 16;             // columns a warp stages before writi
 constexpr int kStagePad  = kTileCols + 1;  // (row stride of the stage, in doubles)
 constexpr unsigned kFull = 0xffffffffu;
 
-enum CountOp : int { kCountMatrix = 0, kCountTopk = 1, kCountThreshold = 2 };
+constexpr uint32_t kUnitCols = 4096;       // columns of a neighbour-pass work unit (a multiple of kPassWarps * kTileCols)
+static_assert(kUnitCols % (kPassWarps * kTileCols) == 0, "a unit is whole sweeps of the CTA's warps");
+
+enum CountOp : int { kCountMatrix = 0, kCountTopk = 1, kCountThreshold = 2, kCountNeighbors = 3 };
+
+__device__ unsigned long long g_countStat[1];  // [0] pairs the last neighbour pass compared
 
 // One group in the form the pass reads: row r's non-zero bins, ascending, as (bin << 16 | count) at
 // pairs[start[r] .. start[r + 1]), and sum[r] the sum of its counts.
@@ -46,13 +72,19 @@ struct CountRows {
   const int32_t*   sum   = nullptr;
 };
 
+// Row r of a compaction is the caller's row perm[r] (perm = NULL: row r).
+__device__ __forceinline__ const int32_t* compactRow(const int32_t* rows, const int32_t* perm, size_t r, int bins) {
+  return rows + (perm ? static_cast<size_t>(perm[r]) : r) * bins;
+}
+
 // sum[r], nnz[r] (nnz[n] = 0, for the scan) and *bad = 1 if a count lies outside 0 .. kMaxCount; a warp per row
-__global__ void __launch_bounds__(256) countStatsKernel(const int32_t* __restrict__ rows, size_t n, int bins, int32_t* __restrict__ sum,
-                                                        long long* __restrict__ nnz, int* __restrict__ bad) {
+__global__ void __launch_bounds__(256) countStatsKernel(const int32_t* __restrict__ rows, const int32_t* __restrict__ perm, size_t n,
+                                                        int bins, int32_t* __restrict__ sum, long long* __restrict__ nnz,
+                                                        int* __restrict__ bad) {
   const int    lane  = threadIdx.x & 31;
   const size_t warps = static_cast<size_t>(gridDim.x) * (blockDim.x / 32);
   for (size_t r = (static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x) / 32; r < n; r += warps) {
-    const int32_t* row = rows + r * bins;
+    const int32_t* row = compactRow(rows, perm, r, bins);
     unsigned       s = 0;
     int            z = 0;
     bool           out = false;
@@ -74,12 +106,12 @@ __global__ void __launch_bounds__(256) countStatsKernel(const int32_t* __restric
 }
 
 // row r's non-zeros, ascending, at pairs[start[r] ..]; a warp per row
-__global__ void __launch_bounds__(256) countPackKernel(const int32_t* __restrict__ rows, size_t n, int bins,
-                                                       const long long* __restrict__ start, uint32_t* __restrict__ pairs) {
+__global__ void __launch_bounds__(256) countPackKernel(const int32_t* __restrict__ rows, const int32_t* __restrict__ perm, size_t n,
+                                                       int bins, const long long* __restrict__ start, uint32_t* __restrict__ pairs) {
   const int    lane  = threadIdx.x & 31;
   const size_t warps = static_cast<size_t>(gridDim.x) * (blockDim.x / 32);
   for (size_t r = (static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x) / 32; r < n; r += warps) {
-    const int32_t* row = rows + r * bins;
+    const int32_t* row = compactRow(rows, perm, r, bins);
     long long      at  = start[r];
     for (int base = 0; base < bins; base += 32) {
       const int      j = base + lane;
@@ -116,20 +148,24 @@ struct PassArgs {
   double*             vals    = nullptr;
   unsigned long long* cursor  = nullptr;
   unsigned long long  listCap = 0;
+  // neighbours (a self pass over rows in sum order): a pair (row, col), col > row, with 1 - value <= cutoff adds one to
+  // both rows' degrees and is appended to `list` as the caller's (i, j), i < j, by the cursor protocol of threshold.
+  // Query block b (rows [b QB, b QB + QB)) visits the columns [b QB, bandEnd[b]) as units of kUnitCols columns; its
+  // units are unitStart[b] .. unitStart[b + 1], and unitStart[nBlocks] is their total.
+  double                    cutoff    = 0.0;
+  const int32_t*            perm      = nullptr;  // [nQ] the caller's index of each row
+  int32_t*                  degrees   = nullptr;  // [nQ] (the caller's indices)
+  const unsigned long long* unitStart = nullptr;  // [nBlocks + 1]
+  const uint32_t*           bandEnd   = nullptr;  // [nBlocks]
+  size_t                    nBlocks   = 0;
 };
 
 __host__ __device__ constexpr size_t queryBlockBytes(int bins, int qb) { return (static_cast<size_t>(bins) * qb * 2 + 15) & ~size_t(15); }
 
-// Grid (query blocks of QB rows, column parts). Lane `sub` of a group of QB lanes serves query q0 + sub; a warp takes
-// 32 / QB library columns at a time, one per group.
-template <int QB, int OP>
-__global__ void __launch_bounds__(kPassWarps * 32) countPassKernel(const PassArgs a) {
-  constexpr int G = 32 / QB;
-  extern __shared__ __align__(16) uint8_t smem[];
-  uint16_t*     qs   = reinterpret_cast<uint16_t*>(smem);  // [bins][QB]
-  const int     lane = threadIdx.x & 31, warp = threadIdx.x >> 5, sub = lane % QB, grp = lane / QB;
-  const size_t  q0   = static_cast<size_t>(blockIdx.x) * QB;
-  const int     nq   = static_cast<int>(min(static_cast<size_t>(QB), a.nQ - q0));
+// Query rows [q0, q0 + QB) dense in shared memory as qs[bin][query] (u16); every thread of the CTA takes part
+template <int QB>
+__device__ __forceinline__ void loadQueryBlock(const PassArgs& a, uint16_t* qs, size_t q0, int nq) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   for (int i = threadIdx.x; i < a.bins * QB / 2; i += blockDim.x) reinterpret_cast<uint32_t*>(qs)[i] = 0;
   __syncthreads();
   for (int j = warp; j < nq; j += kPassWarps)
@@ -138,16 +174,24 @@ __global__ void __launch_bounds__(kPassWarps * 32) countPassKernel(const PassArg
       qs[(v >> 16) * QB + j] = static_cast<uint16_t>(v & 0xffffu);
     }
   __syncthreads();
+}
 
-  const bool   live = sub < nq;
-  const size_t row  = q0 + sub;
-  const int    sa   = live ? a.q.sum[row] : 0;
-  double       barV = -1.0;
-  int32_t      barI = kNoIdx;
+// The loaded query block against library columns [c0, c1). Lane `sub` of a group of QB lanes serves query q0 + sub; a
+// warp takes 32 / QB library columns at a time, one per group.
+template <int QB, int OP>
+__device__ __forceinline__ void passColumns(const PassArgs& a, const uint16_t* qs, uint8_t* smem, size_t q0, int nq, uint32_t c0,
+                                            uint32_t c1) {
+  constexpr int G = 32 / QB;
+  const int     lane = threadIdx.x & 31, warp = threadIdx.x >> 5, sub = lane % QB, grp = lane / QB;
+  const bool    live = sub < nq;
+  const size_t  row  = q0 + sub;
+  const int     sa   = live ? a.q.sum[row] : 0;
+  double        barV = -1.0;
+  int32_t       barI = kNoIdx;
   if constexpr (OP == kCountTopk)
     if (live) barV = a.listV[row * a.k + a.k - 1], barI = a.listI[row * a.k + a.k - 1];
+  int deg = 0;  // (neighbours) of the lane's row in these columns
   double* stage = reinterpret_cast<double*>(smem + queryBlockBytes(a.bins, QB)) + warp * QB * kStagePad;  // (matrix)
-  const uint32_t c0 = a.colBeg + blockIdx.y * a.colsPerCta, c1 = min(a.colEnd, c0 + a.colsPerCta);
   for (uint32_t tile = c0 + warp * kTileCols; tile < c1; tile += kPassWarps * kTileCols) {
     for (int i = 0; i < kTileCols; i += G) {
       const uint32_t col  = tile + i + grp;
@@ -176,15 +220,27 @@ __global__ void __launch_bounds__(kPassWarps * 32) countPassKernel(const PassArg
           if (at < a.cap) a.candV[row * a.cap + at] = v, a.candI[row * a.cap + at] = col;
         }
       } else {
-        const bool     keep = live && have && v >= a.t;
-        const unsigned m    = __ballot_sync(kFull, keep);
+        bool keep;
+        if constexpr (OP == kCountNeighbors) keep = live && have && col > row && __dsub_rn(1.0, v) <= a.cutoff;
+        else keep = live && have && v >= a.t;
+        const unsigned m = __ballot_sync(kFull, keep);
         if (m) {
           const int          first = __ffs(m) - 1;
           unsigned long long base  = 0;
           if (lane == first) base = atomicAdd(a.cursor, static_cast<unsigned long long>(__popc(m)));
           base = __shfl_sync(kFull, base, first);
           const unsigned long long at = base + __popc(m & ((1u << lane) - 1u));
-          if (keep && at < a.listCap) a.list[at] = make_int2(static_cast<int>(row), static_cast<int>(col)), a.vals[at] = v;
+          if constexpr (OP == kCountNeighbors) {
+            deg += keep;
+            const unsigned mine = m & (G == 1 ? kFull : 0xffffu << (grp * 16));  // the hits of this group's column
+            if (sub == 0 && mine) atomicAdd(a.degrees + a.perm[col], __popc(mine));
+            if (keep && at < a.listCap) {
+              const int i = a.perm[row], j = a.perm[col];
+              a.list[at]  = make_int2(min(i, j), max(i, j));
+            }
+          } else {
+            if (keep && at < a.listCap) a.list[at] = make_int2(static_cast<int>(row), static_cast<int>(col)), a.vals[at] = v;
+          }
         }
       }
     }
@@ -196,11 +252,58 @@ __global__ void __launch_bounds__(kPassWarps * 32) countPassKernel(const PassArg
       __syncwarp();  // (the stage is read before the next tile overwrites it)
     }
   }
+  if constexpr (OP == kCountNeighbors)
+    if (deg) atomicAdd(a.degrees + a.perm[row], deg);
+}
+
+// Matrix, top-k and threshold: grid (query blocks of QB rows, column parts). Neighbours: a persistent grid; CTA x of X
+// walks the units [total x / X, total (x + 1) / X) in order, and reloads the query block only when a unit starts a
+// new one.
+template <int QB, int OP>
+__global__ void __launch_bounds__(kPassWarps * 32) countPassKernel(const PassArgs a) {
+  extern __shared__ __align__(16) uint8_t smem[];
+  uint16_t* qs = reinterpret_cast<uint16_t*>(smem);  // [bins][QB]
+  if constexpr (OP == kCountNeighbors) {
+    __shared__ unsigned long long u1;  // (in shared memory: it stays live over the whole walk)
+    const unsigned long long total = a.unitStart[a.nBlocks];
+    const unsigned long long u0    = total * blockIdx.x / gridDim.x;
+    if (threadIdx.x == 0) u1 = total * (blockIdx.x + 1) / gridDim.x;
+    __syncthreads();
+    if (u0 >= u1) return;
+    uint32_t lo = 0, hi = static_cast<uint32_t>(a.nBlocks);  // the block of u0: the last b with unitStart[b] <= u0
+    while (hi - lo > 1) {                                      // (every block has a unit)
+      const uint32_t mid = (lo + hi) / 2;
+      if (a.unitStart[mid] <= u0) lo = mid;
+      else hi = mid;
+    }
+    uint32_t b = lo, loaded = ~0u;
+    for (unsigned long long u = u0; u < u1; ++u) {
+      while (a.unitStart[b + 1] <= u) ++b;
+      const size_t q0 = static_cast<size_t>(b) * QB;
+      const int    nq = static_cast<int>(min(static_cast<size_t>(QB), a.nQ - q0));
+      if (b != loaded) {
+        __syncthreads();  // (every warp is done with the previous block)
+        loadQueryBlock<QB>(a, qs, q0, nq);
+        loaded = b;
+      }
+      const uint32_t c0 = static_cast<uint32_t>(q0 + (u - a.unitStart[b]) * kUnitCols);
+      passColumns<QB, OP>(a, qs, smem, q0, nq, c0, min(a.bandEnd[b], c0 + kUnitCols));
+    }
+  } else {
+    const size_t q0 = static_cast<size_t>(blockIdx.x) * QB;
+    const int    nq = static_cast<int>(min(static_cast<size_t>(QB), a.nQ - q0));
+    loadQueryBlock<QB>(a, qs, q0, nq);
+    const uint32_t c0 = a.colBeg + blockIdx.y * a.colsPerCta;
+    passColumns<QB, OP>(a, qs, smem, q0, nq, c0, min(a.colEnd, c0 + a.colsPerCta));
+  }
 }
 
 size_t passSmemBytes(int op, int bins, int qb) {
   return queryBlockBytes(bins, qb) + (op == kCountMatrix ? static_cast<size_t>(kPassWarps) * qb * kStagePad * sizeof(double) : 0);
 }
+
+// 32-row query blocks up to 2048 bins, 16-row ones above
+int passQueryRows(int bins) { return bins <= 2048 ? 32 : 16; }
 
 template <int QB, int OP>
 void launchPassAs(const PassArgs& a, dim3 grid, cudaStream_t s) {
@@ -210,22 +313,30 @@ void launchPassAs(const PassArgs& a, dim3 grid, cudaStream_t s) {
     B200_CUDA(cudaFuncSetAttribute(countPassKernel<QB, OP>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
     configured[currentDeviceSlot()] = smem;
   }
+  if constexpr (OP == kCountNeighbors) {  // as many CTAs as the device holds at once
+    int perSm = 0;
+    B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, countPassKernel<QB, OP>, kPassWarps * 32, smem));
+    grid = dim3(static_cast<unsigned>(std::max(1, perSm) * smCount()));
+  }
   countPassKernel<QB, OP><<<grid, kPassWarps * 32, smem, s>>>(a);
   B200_LAUNCHED();
 }
 
-// The pass over columns [a.colBeg, a.colEnd): 32-row query blocks up to 2048 bins, 16-row ones above; enough column parts
-// per query block to give the device several CTAs per SM.
+// The pass over columns [a.colBeg, a.colEnd) (neighbours: over the units of a.unitStart); enough column parts per query
+// block to give the device several CTAs per SM.
 template <int OP>
 void launchPass(PassArgs a, cudaStream_t s) {
-  const int      qb     = a.bins <= 2048 ? 32 : 16;
-  const size_t   blocks = (a.nQ + qb - 1) / qb;
-  const uint32_t cols   = a.colEnd - a.colBeg, unit = kPassWarps * kTileCols;
-  const size_t   parts  = std::max<size_t>(1, (8 * static_cast<size_t>(smCount()) + blocks - 1) / blocks);
-  uint32_t       per    = static_cast<uint32_t>((cols + parts - 1) / parts);
-  per                   = std::max<uint32_t>(per, (cols + 65534) / 65535);  // (grid.y)
-  a.colsPerCta          = (per + unit - 1) / unit * unit;
-  const dim3 grid(static_cast<unsigned>(blocks), (cols + a.colsPerCta - 1) / a.colsPerCta);
+  const int qb = passQueryRows(a.bins);
+  dim3      grid;
+  if constexpr (OP != kCountNeighbors) {
+    const size_t   blocks = (a.nQ + qb - 1) / qb;
+    const uint32_t cols   = a.colEnd - a.colBeg, unit = kPassWarps * kTileCols;
+    const size_t   parts  = std::max<size_t>(1, (8 * static_cast<size_t>(smCount()) + blocks - 1) / blocks);
+    uint32_t       per    = static_cast<uint32_t>((cols + parts - 1) / parts);
+    per                   = std::max<uint32_t>(per, (cols + 65534) / 65535);  // (grid.y)
+    a.colsPerCta          = (per + unit - 1) / unit * unit;
+    grid                  = dim3(static_cast<unsigned>(blocks), (cols + a.colsPerCta - 1) / a.colsPerCta);
+  }
   if (qb == 32) launchPassAs<32, OP>(a, grid, s);
   else launchPassAs<16, OP>(a, grid, s);
 }
@@ -361,20 +472,27 @@ struct CompactRows {
   CountRows          view() const { return {pairs.get(), start.get(), sum.get()}; }
 };
 
-// Both groups compacted (b = NULL: one group, used as both), after the range check: the call's one host read.
+__global__ void iotaKernel(int32_t* p, size_t n) {
+  for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x)
+    p[i] = static_cast<int32_t>(i);
+}
+
+// Both groups compacted (b = NULL: one group, used as both), after the range check: the call's one host read. bySum
+// (one group only): the rows are compacted in (row sum, index) order, compact row r being the caller's row order[r].
 struct CountInputs {
-  CompactRows a, bOwn;
-  CountRows   q, lib;
-  CountInputs(const int32_t* da, size_t nA, const int32_t* db, size_t nB, int bins, cudaStream_t s) {
+  CompactRows      a, bOwn;
+  CountRows        q, lib;
+  Scratch<int32_t> order;
+  CountInputs(const int32_t* da, size_t nA, const int32_t* db, size_t nB, int bins, cudaStream_t s, bool bySum = false) {
     Scratch<int> bad(1, s);
     B200_CUDA(cudaMemsetAsync(bad.get(), 0, sizeof(int), s));
     long long total[2] = {0, 0};
     int       hBad     = 0;
-    auto      stats    = [&](const int32_t* d, size_t n, CompactRows& c, long long* hTotal) {
+    auto      stats    = [&](const int32_t* d, const int32_t* perm, size_t n, CompactRows& c, long long* hTotal) {
       c.nnz   = Scratch<long long>(n + 1, s);
       c.start = Scratch<long long>(n + 1, s);
       c.sum   = Scratch<int32_t>(n, s);
-      countStatsKernel<<<blocksFor(n, 8), 256, 0, s>>>(d, n, bins, c.sum.get(), c.nnz.get(), bad.get());
+      countStatsKernel<<<blocksFor(n, 8), 256, 0, s>>>(d, perm, n, bins, c.sum.get(), c.nnz.get(), bad.get());
       B200_LAUNCHED();
       size_t tmpBytes = 0;
       B200_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmpBytes, c.nnz.get(), c.start.get(), static_cast<uint32_t>(n + 1), s));
@@ -383,18 +501,38 @@ struct CountInputs {
       g_launchCount.fetch_add(1);
       B200_CUDA(cudaMemcpyAsync(hTotal, c.start.get() + n, sizeof(long long), cudaMemcpyDeviceToHost, s));
     };
-    stats(da, nA, a, &total[0]);
-    if (db) stats(db, nB, bOwn, &total[1]);
+    if (bySum) {
+      // the sums in the caller's order (their stats are then recomputed in sum order), and a stable radix sort of
+      // (sum, index); a count out of range gives a meaningless order, refused below before it is used
+      CompactRows first;
+      first.nnz = Scratch<long long>(nA + 1, s);
+      first.sum = Scratch<int32_t>(nA, s);
+      countStatsKernel<<<blocksFor(nA, 8), 256, 0, s>>>(da, nullptr, nA, bins, first.sum.get(), first.nnz.get(), bad.get());
+      B200_LAUNCHED();
+      Scratch<int32_t> index(nA, s), sorted(nA, s);
+      order = Scratch<int32_t>(nA, s);
+      iotaKernel<<<blocksFor(nA, 256), 256, 0, s>>>(index.get(), nA);
+      B200_LAUNCHED();
+      size_t tmpBytes = 0;
+      B200_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmpBytes, first.sum.get(), sorted.get(), index.get(), order.get(),
+                                                static_cast<int>(nA), 0, 32, s));
+      Scratch<uint8_t> tmp(tmpBytes, s);
+      B200_CUDA(cub::DeviceRadixSort::SortPairs(tmp.get(), tmpBytes, first.sum.get(), sorted.get(), index.get(), order.get(),
+                                                static_cast<int>(nA), 0, 32, s));
+      g_launchCount.fetch_add(1);
+    }
+    stats(da, order.get(), nA, a, &total[0]);
+    if (db) stats(db, nullptr, nB, bOwn, &total[1]);
     B200_CUDA(cudaMemcpyAsync(&hBad, bad.get(), sizeof(int), cudaMemcpyDeviceToHost, s));
     B200_CUDA(cudaStreamSynchronize(s));  // documented sync: the range check and the list sizes
     B200_REQUIRE(hBad == 0, "a count lies outside 0 .. %d", kMaxCount);
-    auto pack = [&](const int32_t* d, size_t n, CompactRows& c, long long nnz) {
+    auto pack = [&](const int32_t* d, const int32_t* perm, size_t n, CompactRows& c, long long nnz) {
       c.pairs = Scratch<uint32_t>(static_cast<size_t>(nnz), s);
-      countPackKernel<<<blocksFor(n, 8), 256, 0, s>>>(d, n, bins, c.start.get(), c.pairs.get());
+      countPackKernel<<<blocksFor(n, 8), 256, 0, s>>>(d, perm, n, bins, c.start.get(), c.pairs.get());
       B200_LAUNCHED();
     };
-    pack(da, nA, a, total[0]);
-    if (db) pack(db, nB, bOwn, total[1]);
+    pack(da, order.get(), nA, a, total[0]);
+    if (db) pack(db, nullptr, nB, bOwn, total[1]);
     q   = a.view();
     lib = db ? bOwn.view() : q;
   }
@@ -406,7 +544,63 @@ void requireCountInputs(const int32_t* d_a, size_t nA, size_t nB, int bins) {
   B200_REQUIRE(nA == 0 || d_a, "null count-vector pointer");
 }
 
+// ---- the neighbour pass's band (see the file header) ----
+
+// Block b of QB rows in sum order: bandEnd[b] = the end of the columns it visits, units[b] = their units of kUnitCols
+// (units[nBlocks] = 0, for the scan), and g_countStat[0] += the pairs (row, col > row) in them. A thread per block
+// bisects the sorted sums for the first column past the block that its largest sum A cannot reach:
+// 1 - value(c = A, a = A, b) <= cutoff fails from there on.
+__global__ void countBandKernel(const int32_t* __restrict__ sum, size_t n, int qb, const Measure m, double cutoff,
+                                uint32_t* __restrict__ bandEnd, unsigned long long* __restrict__ units) {
+  const size_t       nBlocks = (n + qb - 1) / qb;
+  unsigned long long pairs   = 0;
+  for (size_t b = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; b < nBlocks; b += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const size_t q0 = b * qb, e = min(n, q0 + qb);
+    const int    A  = sum[e - 1];
+    size_t       lo = e, hi = n;
+    while (lo < hi) {
+      const size_t mid = (lo + hi) / 2;
+      if (__dsub_rn(1.0, tverskyFromCounts(A, A, sum[mid], m.alpha, m.beta)) <= cutoff) lo = mid + 1;
+      else hi = mid;
+    }
+    bandEnd[b] = static_cast<uint32_t>(lo);
+    units[b]   = (lo - q0 + kUnitCols - 1) / kUnitCols;
+    const unsigned long long nq = e - q0;
+    pairs += nq * (nq - 1) / 2 + nq * (lo - e);
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) units[nBlocks] = 0;
+  for (int o = 16; o; o >>= 1) pairs += __shfl_xor_sync(kFull, pairs, o);
+  if ((threadIdx.x & 31) == 0 && pairs) atomicAdd(&g_countStat[0], pairs);
+}
+
+// counts[] += the degrees and edges[] the (i < j) pairs, caller's indices, of the neighbour graph of x (cursor protocol
+// of b200mol_neighbor_edges), after the range check
+void countNeighborEdges(const int32_t* d_x, size_t n, int bins, const Measure& m, double cutoff, int32_t* counts, int2* edges,
+                        unsigned long long cap, unsigned long long* cursor, cudaStream_t s) {
+  resetDeviceCounters(g_countStat, s);
+  CountInputs                 in(d_x, n, nullptr, n, bins, s, true);
+  const int                   qb      = passQueryRows(bins);
+  const size_t                nBlocks = (n + qb - 1) / qb;
+  Scratch<uint32_t>           bandEnd(nBlocks, s);
+  Scratch<unsigned long long> units(nBlocks + 1, s), unitStart(nBlocks + 1, s);
+  countBandKernel<<<blocksFor(nBlocks, 256), 256, 0, s>>>(in.q.sum, n, qb, m, cutoff, bandEnd.get(), units.get());
+  B200_LAUNCHED();
+  size_t tmpBytes = 0;
+  B200_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmpBytes, units.get(), unitStart.get(), static_cast<uint32_t>(nBlocks + 1), s));
+  Scratch<uint8_t> tmp(tmpBytes, s);
+  B200_CUDA(cub::DeviceScan::ExclusiveSum(tmp.get(), tmpBytes, units.get(), unitStart.get(), static_cast<uint32_t>(nBlocks + 1), s));
+  g_launchCount.fetch_add(1);
+  PassArgs p;
+  p.q = in.q, p.lib = in.lib, p.nQ = n, p.bins = bins, p.measure = m;
+  p.cutoff = cutoff, p.perm = in.order.get(), p.degrees = counts, p.list = edges, p.cursor = cursor, p.listCap = cap;
+  p.unitStart = unitStart.get(), p.bandEnd = bandEnd.get(), p.nBlocks = nBlocks;
+  launchPass<kCountNeighbors>(p, s);
+}
+
 }  // namespace
+
+unsigned long long readCountStat(int i) { return readDeviceCounter(g_countStat, i); }
+
 }  // namespace b200
 
 using namespace b200;
@@ -523,5 +717,67 @@ extern "C" int b200mol_count_threshold(const int32_t* d_q, size_t nQ, const int3
     if (listed > cap) return;  // the caller asks again with room for nnz
     assembleThresholdCsr(list.get(), vals.get(), listed, false, nullptr, nQ, nLib, m.kind, listed, stat.get(), d_indptr, d_indices,
                          d_values, s);
+  });
+}
+
+extern "C" int b200mol_count_neighbor_edges(const int32_t* d_x, size_t n, int bins, double alpha, double beta, double cutoff,
+                                            int32_t* d_counts, int32_t* d_edges, uint64_t edge_cap, uint64_t* h_n_edges,
+                                            void* stream) {
+  return guarded([&] {
+    const Measure m = measureOfWeights(alpha, beta);
+    B200_REQUIRE(m.kind == kTanimoto || m.kind == kDice,
+                 "count neighbours take Tanimoto (1, 1) or Dice (0.5, 0.5) weights (got alpha = %g, beta = %g)", alpha, beta);
+    B200_REQUIRE(cutoff >= 0.0 && cutoff <= 1.0, "cutoff must be in [0, 1], got %g", cutoff);
+    requireCountInputs(d_x, n, n, bins);
+    const cudaStream_t s = asStream(stream);
+    if (h_n_edges) *h_n_edges = 0;
+    if (n == 0) return;
+    B200_REQUIRE(d_counts && (d_edges || edge_cap == 0), "null pointer");
+    Scratch<unsigned long long> cursor(1, s);
+    B200_CUDA(cudaMemsetAsync(cursor.get(), 0, sizeof(unsigned long long), s));
+    countNeighborEdges(d_x, n, bins, m, cutoff, d_counts, reinterpret_cast<int2*>(d_edges), edge_cap, cursor.get(), s);
+    if (h_n_edges) {
+      unsigned long long v = 0;
+      B200_CUDA(cudaMemcpyAsync(&v, cursor.get(), sizeof(v), cudaMemcpyDeviceToHost, s));
+      B200_CUDA(cudaStreamSynchronize(s));  // documented sync: the edge total sizes the CSR
+      *h_n_edges = v;
+    }
+  });
+}
+
+extern "C" int b200mol_count_butina_fused(const int32_t* d_x, size_t n, int bins, double alpha, double beta, double cutoff,
+                                          int32_t* d_cluster_ids, int32_t* d_centroids, int32_t* d_n_clusters,
+                                          int32_t* h_n_clusters, void* stream) {
+  return guarded([&] {
+    const Measure m = measureOfWeights(alpha, beta);  // (checked first, as b200mol_count_neighbor_edges does)
+    B200_REQUIRE(m.kind == kTanimoto || m.kind == kDice,
+                 "count neighbours take Tanimoto (1, 1) or Dice (0.5, 0.5) weights (got alpha = %g, beta = %g)", alpha, beta);
+    B200_REQUIRE(cutoff >= 0.0 && cutoff <= 1.0, "cutoff must be in [0, 1], got %g", cutoff);
+    requireCountInputs(d_x, n, n, bins);
+    const cudaStream_t s = asStream(stream);
+    if (n == 0) {
+      if (h_n_clusters) *h_n_clusters = 0;
+      if (d_n_clusters) B200_CUDA(cudaMemsetAsync(d_n_clusters, 0, sizeof(int32_t), s));
+      return;
+    }
+    B200_REQUIRE(d_cluster_ids, "null pointer");
+    Scratch<int32_t> counts(n, s);
+    // the edge list of b200mol_butina_fused: 64 per point, and one rerun at the exact size for a denser graph
+    unsigned long long cap = static_cast<unsigned long long>(n) * 64ull;
+    Scratch<int2>      edges;
+    uint64_t           nEdges = 0;
+    for (int attempt = 0; attempt < 2; ++attempt) {
+      edges = Scratch<int2>(cap, s);
+      B200_CUDA(cudaMemsetAsync(counts.get(), 0, n * sizeof(int32_t), s));
+      const int rc = b200mol_count_neighbor_edges(d_x, n, bins, alpha, beta, cutoff, counts.get(),
+                                                  reinterpret_cast<int32_t*>(edges.get()), cap, &nEdges, stream);
+      if (rc != B200MOL_OK) fail(rc, "%s", g_lastError.c_str());
+      if (nEdges <= cap) break;
+      B200_REQUIRE(attempt == 0, "edge list overflow after resize");
+      cap = nEdges;
+    }
+    const int rc = b200mol_butina_from_edges(n, counts.get(), reinterpret_cast<const int32_t*>(edges.get()), nEdges,
+                                             d_cluster_ids, d_centroids, d_n_clusters, h_n_clusters, stream);
+    if (rc != B200MOL_OK) fail(rc, "%s", g_lastError.c_str());
   });
 }

@@ -82,6 +82,7 @@ constexpr Option kOptions[] = {
     {"leader_bulk_pairs_last", &g_leaderBulkPairsLast, kReadOnly},
     {"leader_window_pairs_last", {readLeaderStat, 0}, kReadOnly},
     {"leader_block_pairs_last", {readLeaderStat, 1}, kReadOnly},
+    {"count_neighbor_pairs_last", {readCountStat, 0}, kReadOnly},
     {"rmsd_match_chunk", &g_rmsdMatchChunk, kRange, 0, kBelow2To31, "must be in [0, 2^31)"},
     {"rmsd_match_chunks_last", &g_rmsdMatchChunksLast, kReadOnly},
     {"morgan_global_slab_last", &g_morganGlobalSlabLast, kReadOnly},

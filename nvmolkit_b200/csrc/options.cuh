@@ -43,5 +43,6 @@ unsigned long long readWalkCounter(int i);  // tanimoto_tc.cu: [0] units, [1] ti
 unsigned long long readTopkStat(int i);     // topk.cu: [0] candidates listed, [1] rows redone
 unsigned long long readMaxminStat(int i);   // maxmin.cu: [0] distances evaluated, [1] skipped by the popcount bound
 unsigned long long readLeaderStat(int i);   // leader.cu: [0] pairs compared in a window, [1] in a block
+unsigned long long readCountStat(int i);    // count_similarity.cu: [0] pairs the neighbour pass compared
 
 }  // namespace b200

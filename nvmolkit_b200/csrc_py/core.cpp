@@ -136,6 +136,8 @@ PYBIND11_MODULE(_core, m) {
   DEF(b200mol_neighbor_edges);
   DEF(b200mol_butina_from_edges);
   DEF(b200mol_butina_dense);
+  DEF(b200mol_count_neighbor_edges);
+  DEF(b200mol_count_butina_fused);
   DEF(b200mol_morgan);
   DEF(b200mol_morgan_counts);
   DEF(b200mol_schedule_waves);
