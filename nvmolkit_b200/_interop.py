@@ -45,9 +45,13 @@ def fingerprint_matrix(obj, name: str) -> torch.Tensor:
     return t.contiguous()
 
 
-def stream_ptr(stream) -> int:
+def check_stream(stream) -> None:
     if stream is not None and not isinstance(stream, torch.cuda.Stream):
         raise TypeError(f"stream must be a torch.cuda.Stream or None, got {type(stream).__name__}")
+
+
+def stream_ptr(stream) -> int:
+    check_stream(stream)
     return (stream if stream is not None else torch.cuda.current_stream()).cuda_stream
 
 

@@ -10,9 +10,16 @@ import torch
 
 from nvmolkit_b200 import _lib
 from nvmolkit_b200._interop import as_tensor, require_cuda, stream_ctx, stream_ptr
+from nvmolkit_b200.similarity import _count_matrix, _prepare
 from nvmolkit_b200.types import AsyncGpuResult
 
 _VALID_NEIGHBORLIST_SIZES = frozenset({8, 16, 24, 32, 64, 128})
+
+
+def _outputs(n: int, device):
+    """Cluster ids [n], centroids [max(n, 1)] and the cluster count [1] of a clustering call, on the current stream."""
+    return (torch.empty(n, dtype=torch.int32, device=device), torch.empty(max(n, 1), dtype=torch.int32, device=device),
+            torch.zeros(1, dtype=torch.int32, device=device))
 
 
 def butina(distance_matrix, cutoff: float, neighborlist_max_size: int = 64, return_centroids: bool = False,
@@ -34,9 +41,7 @@ def butina(distance_matrix, cutoff: float, neighborlist_max_size: int = 64, retu
     d = d.contiguous()
     n = d.shape[0]
     with stream_ctx(stream):
-        ids = torch.empty(n, dtype=torch.int32, device=d.device)
-        cen = torch.empty(max(n, 1), dtype=torch.int32, device=d.device)
-        ncl = torch.zeros(1, dtype=torch.int32, device=d.device)
+        ids, cen, ncl = _outputs(n, d.device)
         _lib.call("b200mol_butina_dense", d.data_ptr(), n, float(cutoff), ids.data_ptr(), cen.data_ptr(),
                   ncl.data_ptr(), None, sptr)
         d.record_stream(torch.cuda.current_stream())
@@ -62,17 +67,29 @@ def fused_butina_device(x, cutoff: float, stream=None, metric: str = "tanimoto")
     if cutoff < 0 or cutoff > 1:
         raise ValueError(f"cutoff must be in [0, 1], got {cutoff}")
     require_cuda()
-    x = x.contiguous()
+    return _fused(x.contiguous(), "b200mol_butina_fused", (_lib.METRIC[metric],), cutoff, stream, sptr)
+
+
+def _fused(x, fn: str, measure: tuple, cutoff: float, stream, sptr, counts: bool = False):
+    """The fused Butina entry point fn on x, checked (count vectors when counts), with the measure's arguments:
+    (ids int32[N], centroids int32[nClusters]) on the device."""
     n = x.shape[0]
     with stream_ctx(stream):
-        ids = torch.empty(n, dtype=torch.int32, device=x.device)
-        cen = torch.empty(max(n, 1), dtype=torch.int32, device=x.device)
-        ncl = torch.zeros(1, dtype=torch.int32, device=x.device)
-        _lib.call("b200mol_butina_fused", x.data_ptr(), n, x.shape[1], _lib.METRIC[metric], float(cutoff),
-                  ids.data_ptr(), cen.data_ptr(), ncl.data_ptr(), None, sptr)
+        x = _prepare(x, counts)
+        ids, cen, ncl = _outputs(n, x.device)
+        _lib.call(fn, x.data_ptr(), n, x.shape[1], *measure, float(cutoff), ids.data_ptr(), cen.data_ptr(),
+                  ncl.data_ptr(), None, sptr)
         x.record_stream(torch.cuda.current_stream())
         k = int(ncl.item())
     return ids, cen[:k]
+
+
+def _host_clusters(ids, cen, return_centroids: bool):
+    """The device result as the reference returns it: (clusters, cluster_sizes[, centroids])."""
+    clusters, sizes = clusters_from_ids(ids.cpu().numpy(), cen.cpu().numpy())
+    if return_centroids:
+        return clusters, sizes, cen.cpu().numpy().tolist()
+    return clusters, sizes
 
 
 def fused_butina_sharded(x, cutoff: float, stream=None, metric: str = "tanimoto", group=None):
@@ -105,9 +122,7 @@ def fused_butina_sharded(x, cutoff: float, stream=None, metric: str = "tanimoto"
         dist.all_reduce(counts, group=group)
         all_edges, _ = all_gather_v(edges[: found.value], group=group)
         all_edges = all_edges.contiguous()
-        ids = torch.empty(n, dtype=torch.int32, device=x.device)
-        cen = torch.empty(max(n, 1), dtype=torch.int32, device=x.device)
-        ncl = torch.zeros(1, dtype=torch.int32, device=x.device)
+        ids, cen, ncl = _outputs(n, x.device)
         _lib.call("b200mol_butina_from_edges", n, counts.data_ptr(), all_edges.data_ptr(), all_edges.shape[0],
                   ids.data_ptr(), cen.data_ptr(), ncl.data_ptr(), None, sptr)
         k = int(ncl.item())
@@ -126,11 +141,7 @@ def fused_butina(x, cutoff: float, return_centroids: bool = False, stream=None, 
     sit exactly on the boundary as a ratio of small integers (cutoff 0.3, sim = 7/10: 1 - 0.7 = 0.30000000000000004 > 0.3)
     are neighbours there and not here. Deliberate: this path agrees with the dense path and with RDKit bit for bit.
     """
-    ids, cen = fused_butina_device(x, cutoff, stream=stream, metric=metric)
-    clusters, sizes = clusters_from_ids(ids.cpu().numpy(), cen.cpu().numpy())
-    if return_centroids:
-        return clusters, sizes, cen.cpu().numpy().tolist()
-    return clusters, sizes
+    return _host_clusters(*fused_butina_device(x, cutoff, stream=stream, metric=metric), return_centroids)
 
 
 _COUNT_METRICS = {"tanimoto": (1.0, 1.0), "dice": (0.5, 0.5)}  # (alpha, beta) of b200mol_count_butina_fused
@@ -138,26 +149,14 @@ _COUNT_METRICS = {"tanimoto": (1.0, 1.0), "dice": (0.5, 0.5)}  # (alpha, beta) o
 
 def fused_butina_counts_device(x, cutoff: float, stream=None, metric: str = "tanimoto"):
     """Device-resident result of :func:`fused_butina_counts`: (ids int32[N], centroids int32[nClusters])."""
-    from nvmolkit_b200 import similarity
-
     if metric not in _COUNT_METRICS:
         raise ValueError(f"metric must be one of {sorted(_COUNT_METRICS)} on count vectors, got {metric!r}")
     if not 0.0 <= cutoff <= 1.0:
         raise ValueError(f"cutoff must be in [0, 1], got {cutoff}")
     sptr = stream_ptr(stream)
-    x = similarity._count_matrix(x, "x")
+    x = _count_matrix(x, "x")
     require_cuda()
-    n = x.shape[0]
-    with stream_ctx(stream):
-        (x,) = similarity._int32(x)
-        ids = torch.empty(n, dtype=torch.int32, device=x.device)
-        cen = torch.empty(max(n, 1), dtype=torch.int32, device=x.device)
-        ncl = torch.zeros(1, dtype=torch.int32, device=x.device)
-        _lib.call("b200mol_count_butina_fused", x.data_ptr(), n, x.shape[1], *_COUNT_METRICS[metric], float(cutoff),
-                  ids.data_ptr(), cen.data_ptr(), ncl.data_ptr(), None, sptr)
-        x.record_stream(torch.cuda.current_stream())
-        k = int(ncl.item())
-    return ids, cen[:k]
+    return _fused(x, "b200mol_count_butina_fused", _COUNT_METRICS[metric], cutoff, stream, sptr, counts=True)
 
 
 def fused_butina_counts(x, cutoff: float, return_centroids: bool = False, stream=None, metric: str = "tanimoto"):
@@ -174,11 +173,7 @@ def fused_butina_counts(x, cutoff: float, return_centroids: bool = False, stream
     Synchronises ``stream``: once for the count range check (a count out of range raises ``ValueError``), once for the
     edge total, a rerun of the pass when the graph has more than 64 edges per point, and once for the cluster count.
     """
-    ids, cen = fused_butina_counts_device(x, cutoff, stream=stream, metric=metric)
-    clusters, sizes = clusters_from_ids(ids.cpu().numpy(), cen.cpu().numpy())
-    if return_centroids:
-        return clusters, sizes, cen.cpu().numpy().tolist()
-    return clusters, sizes
+    return _host_clusters(*fused_butina_counts_device(x, cutoff, stream=stream, metric=metric), return_centroids)
 
 
 def clusters_from_ids(ids_h, cen_h):

@@ -307,10 +307,6 @@ __global__ void __launch_bounds__(kRoundThreads) butinaRoundsKernel(LoopState st
   }
 }
 
-__global__ void iotaKernel(int* p, int n) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) p[i] = i;
-}
 // sorted (key descending, point): rank r -> centroids[r], idOf[point] = r
 __global__ void rankCentresKernel(const unsigned long long* __restrict__ keys, const int* __restrict__ pts, int n,
                                   int32_t* __restrict__ centroids, int* __restrict__ idOf) {
@@ -482,8 +478,69 @@ void clusterFromEdges(int N, int32_t* counts, const int2* edges, unsigned long l
   clusterFromCsr(N, offsets.get(), adj.get(), counts, ids, centroids, dNCl, s);
 }
 
+// The clusters of an edge list (b200mol_butina_from_edges past its checks): centroids and the device cluster count may
+// be NULL (then the library keeps its own), and the host count, when asked for, is read with a stream synchronise.
+void clusterEdgeList(size_t n, int32_t* counts, const int2* edges, unsigned long long nEdges, int32_t* ids,
+                     int32_t* centroids, int32_t* dNClusters, int32_t* hNClusters, cudaStream_t s) {
+  Scratch<int32_t> centroidsOwn(centroids ? 0 : n, s);
+  Scratch<int32_t> nClOwn(1, s);
+  int32_t*         dNCl = dNClusters ? dNClusters : nClOwn.get();
+  clusterFromEdges(static_cast<int>(n), counts, edges, nEdges, ids, centroids ? centroids : centroidsOwn.get(), dNCl, s);
+  if (hNClusters) {
+    B200_CUDA(cudaMemcpyAsync(hNClusters, dNCl, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    B200_CUDA(cudaStreamSynchronize(s));
+  }
+}
+
 }  // namespace
+
+void noClusters(int32_t* dNClusters, int32_t* hNClusters, cudaStream_t s) {
+  if (hNClusters) *hNClusters = 0;
+  if (dNClusters) B200_CUDA(cudaMemsetAsync(dNClusters, 0, sizeof(int32_t), s));
+}
+
+void edgePassWithTotal(const EdgePass& pass, int32_t* counts, int2* edges, unsigned long long cap, uint64_t* hNEdges,
+                       cudaStream_t s) {
+  Scratch<unsigned long long> cursor(1, s);
+  B200_CUDA(cudaMemsetAsync(cursor.get(), 0, sizeof(unsigned long long), s));
+  pass(counts, edges, cap, cursor.get());
+  if (hNEdges) {
+    unsigned long long v = 0;
+    B200_CUDA(cudaMemcpyAsync(&v, cursor.get(), sizeof(v), cudaMemcpyDeviceToHost, s));
+    B200_CUDA(cudaStreamSynchronize(s));  // documented sync: the edge total sizes the CSR
+    *hNEdges = v;
+  }
+}
+
+void fusedButina(size_t n, const EdgePass& pass, int32_t* ids, int32_t* centroids, int32_t* dNClusters, int32_t* hNClusters,
+                 cudaStream_t s) {
+  Scratch<int32_t> counts(n, s);
+  // One pass over the pairs: counts + edge list. The capacity grows (and the deterministic pass repeats) only when the
+  // graph is denser than 64 neighbours per point on average.
+  unsigned long long cap = static_cast<unsigned long long>(n) * 64ull;
+  Scratch<int2>      edges;
+  uint64_t           nEdges = 0;
+  for (int attempt = 0; attempt < 2; ++attempt) {
+    edges = Scratch<int2>(cap, s);
+    B200_CUDA(cudaMemsetAsync(counts.get(), 0, n * sizeof(int32_t), s));
+    edgePassWithTotal(pass, counts.get(), edges.get(), cap, &nEdges, s);
+    if (nEdges <= cap) break;
+    B200_REQUIRE(attempt == 0, "edge list overflow after resize");
+    cap = nEdges;
+  }
+  clusterEdgeList(n, counts.get(), edges.get(), nEdges, ids, centroids, dNClusters, hNClusters, s);
+}
+
 }  // namespace b200
+
+// The bit pass of b200mol_neighbor_edges and b200mol_butina_fused, timed as the phase "neighbor_pass"
+static EdgePass bitEdgePass(const uint32_t* d_fp, size_t n, int words, const Measure& m, double cutoff, uint32_t groupOffset,
+                            uint32_t groupStride, cudaStream_t s) {
+  return [=](int32_t* counts, int2* edges, unsigned long long cap, unsigned long long* cursor) {
+    PhaseTimer t("neighbor_pass", s);
+    neighborEdges(d_fp, n, words, m, cutoff, groupOffset, groupStride, counts, edges, cap, cursor, s);
+  };
+}
 
 extern "C" int b200mol_neighbor_edges(const uint32_t* d_fp, size_t n, int words, int metric, double cutoff,
                                       uint32_t group_offset, uint32_t group_stride, int32_t* d_counts,
@@ -497,19 +554,8 @@ extern "C" int b200mol_neighbor_edges(const uint32_t* d_fp, size_t n, int words,
     if (h_n_edges) *h_n_edges = 0;
     if (n == 0) return;
     B200_REQUIRE(d_fp && d_counts && (d_edges || edge_cap == 0), "null pointer");
-    Scratch<unsigned long long> cursor(1, s);
-    B200_CUDA(cudaMemsetAsync(cursor.get(), 0, sizeof(unsigned long long), s));
-    {
-      PhaseTimer t("neighbor_pass", s);
-      neighborEdges(d_fp, n, words, m, cutoff, group_offset, group_stride, d_counts,
-                    reinterpret_cast<int2*>(d_edges), edge_cap, cursor.get(), s);
-    }
-    if (h_n_edges) {
-      unsigned long long v = 0;
-      B200_CUDA(cudaMemcpyAsync(&v, cursor.get(), sizeof(v), cudaMemcpyDeviceToHost, s));
-      B200_CUDA(cudaStreamSynchronize(s));  // documented sync: the edge total sizes the CSR
-      *h_n_edges = v;
-    }
+    edgePassWithTotal(bitEdgePass(d_fp, n, words, m, cutoff, group_offset, group_stride, s), d_counts,
+                      reinterpret_cast<int2*>(d_edges), edge_cap, h_n_edges, s);
   });
 }
 
@@ -519,22 +565,10 @@ extern "C" int b200mol_butina_from_edges(size_t n, int32_t* d_counts, const int3
   return guarded([&] {
     B200_REQUIRE(n < (1ull << 31), "too many points");
     cudaStream_t s = asStream(stream);
-    if (n == 0) {
-      if (h_n_clusters) *h_n_clusters = 0;
-      if (d_n_clusters) B200_CUDA(cudaMemsetAsync(d_n_clusters, 0, sizeof(int32_t), s));
-      return;
-    }
+    if (n == 0) return noClusters(d_n_clusters, h_n_clusters, s);
     B200_REQUIRE(d_counts && d_cluster_ids && (d_edges || n_edges == 0), "null pointer");
-    Scratch<int32_t> centroidsOwn(d_centroids ? 0 : n, s);
-    int32_t*         centroids = d_centroids ? d_centroids : centroidsOwn.get();
-    Scratch<int32_t> nClOwn(1, s);
-    int32_t*         dNCl = d_n_clusters ? d_n_clusters : nClOwn.get();
-    clusterFromEdges(static_cast<int>(n), d_counts, reinterpret_cast<const int2*>(d_edges), n_edges, d_cluster_ids,
-                     centroids, dNCl, s);
-    if (h_n_clusters) {
-      B200_CUDA(cudaMemcpyAsync(h_n_clusters, dNCl, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-      B200_CUDA(cudaStreamSynchronize(s));
-    }
+    clusterEdgeList(n, d_counts, reinterpret_cast<const int2*>(d_edges), n_edges, d_cluster_ids, d_centroids, d_n_clusters,
+                    h_n_clusters, s);
   });
 }
 
@@ -542,35 +576,13 @@ extern "C" int b200mol_butina_fused(const uint32_t* d_fp, size_t n, int words, i
                                     int32_t* d_cluster_ids, int32_t* d_centroids, int32_t* d_n_clusters,
                                     int32_t* h_n_clusters, void* stream) {
   return guarded([&] {
-    measureOfMetric(metric);  // (checked first, as b200mol_neighbor_edges does)
+    const Measure m = measureOfMetric(metric);
     B200_REQUIRE(cutoff >= 0.0 && cutoff <= 1.0, "cutoff must be in [0, 1], got %g", cutoff);
     B200_REQUIRE(n < (1ull << 31), "too many fingerprints");
     cudaStream_t s = asStream(stream);
-    if (n == 0) {
-      if (h_n_clusters) *h_n_clusters = 0;
-      if (d_n_clusters) B200_CUDA(cudaMemsetAsync(d_n_clusters, 0, sizeof(int32_t), s));
-      return;
-    }
+    if (n == 0) return noClusters(d_n_clusters, h_n_clusters, s);
     B200_REQUIRE(d_fp && d_cluster_ids, "null pointer");
-    Scratch<int32_t> counts(n, s);
-    // One N^2/2 pass: counts + edge list. The capacity grows (and the deterministic pass repeats) only when the graph
-    // is denser than 64 neighbours per point on average.
-    unsigned long long cap = static_cast<unsigned long long>(n) * 64ull;
-    Scratch<int2>      edges;
-    uint64_t           nEdges = 0;
-    for (int attempt = 0; attempt < 2; ++attempt) {
-      edges = Scratch<int2>(cap, s);
-      B200_CUDA(cudaMemsetAsync(counts.get(), 0, n * sizeof(int32_t), s));
-      const int rc = b200mol_neighbor_edges(d_fp, n, words, metric, cutoff, 0, 1, counts.get(),
-                                            reinterpret_cast<int32_t*>(edges.get()), cap, &nEdges, stream);
-      if (rc != B200MOL_OK) fail(rc, "%s", g_lastError.c_str());
-      if (nEdges <= cap) break;
-      B200_REQUIRE(attempt == 0, "edge list overflow after resize");
-      cap = nEdges;
-    }
-    const int rc = b200mol_butina_from_edges(n, counts.get(), reinterpret_cast<const int32_t*>(edges.get()), nEdges,
-                                             d_cluster_ids, d_centroids, d_n_clusters, h_n_clusters, stream);
-    if (rc != B200MOL_OK) fail(rc, "%s", g_lastError.c_str());
+    fusedButina(n, bitEdgePass(d_fp, n, words, m, cutoff, 0, 1, s), d_cluster_ids, d_centroids, d_n_clusters, h_n_clusters, s);
   });
 }
 
@@ -579,11 +591,7 @@ extern "C" int b200mol_butina_dense(const double* d_dist, size_t n, double cutof
   return guarded([&] {
     B200_REQUIRE(n < (1ull << 31), "too many points");
     cudaStream_t s = asStream(stream);
-    if (n == 0) {
-      if (h_n_clusters) *h_n_clusters = 0;
-      if (d_n_clusters) B200_CUDA(cudaMemsetAsync(d_n_clusters, 0, sizeof(int32_t), s));
-      return;
-    }
+    if (n == 0) return noClusters(d_n_clusters, h_n_clusters, s);
     B200_REQUIRE(d_dist && d_cluster_ids, "null pointer");
     const int        N = static_cast<int>(n);
     Scratch<int32_t> counts(n, s);

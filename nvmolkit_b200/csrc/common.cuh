@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <atomic>
 #include <cstdarg>
 #include <cstdint>
@@ -107,6 +108,21 @@ inline int smCount() {  // of the current device
   }
   return cached[dev];
 }
+
+// Blocks of perBlock items for a grid-stride loop over `items`: enough for one item each, at most 16 per SM, at least one.
+inline unsigned blocksFor(unsigned long long items, int perBlock) {
+  return static_cast<unsigned>(std::max<unsigned long long>(
+    1, std::min<unsigned long long>((items + perBlock - 1) / perBlock, static_cast<unsigned long long>(smCount()) * 16)));
+}
+
+namespace {
+// p[i] = i, a grid-stride loop. A template, so that only the objects that launch it hold a copy of the kernel.
+template <class T>
+__global__ void iotaKernel(T* p, size_t n) {
+  for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x)
+    p[i] = static_cast<T>(i);
+}
+}  // namespace
 
 // Function attributes (dynamic shared-memory limits) belong to the device's context: a process that drives several
 // GPUs (HardwareOptions.gpuIds / targetGpu) must set them once per DEVICE, not once per process.

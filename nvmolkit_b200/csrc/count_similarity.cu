@@ -14,11 +14,13 @@
 //     matrix      values staged per warp in shared memory, written as 128-byte row segments;
 //     top-k       a pair that beats its row's bar (the running list's k-th entry, the order of topk.cuh) takes a
 //                 candidate slot with its value; the protocol of topk.cu: slabs of library columns that double, a
-//                 select that merges a row's slots into its list, and a scan that redoes a slab for the rows whose
-//                 candidates did not fit;
-//     threshold   a pair with value >= t is listed with its value; threshold.cu's assembly (keys, one radix sort,
-//                 indptr by bisection) makes the CSR. A self search runs the full pass (it needs no diagonal step);
-//     neighbours  (Butina: b200mol_count_neighbor_edges, Tanimoto and Dice only) a self pass over the rows compacted
+//                 select that merges a row's slots into its list, and a scan (topk.cuh's scanBest) that redoes a slab
+//                 for the rows whose candidates did not fit;
+//     threshold   a pair with value >= t is listed with its value, in threshold.cu's attempt protocol (thresholdCsr),
+//                 whose assembly (keys, one radix sort, indptr by bisection) makes the CSR. A self search runs the full
+//                 pass (it needs no diagonal step);
+//     neighbours  (Butina: b200mol_count_neighbor_edges, and butina.cu's fusedButina for b200mol_count_butina_fused;
+//                 Tanimoto and Dice only) a self pass over the rows compacted
 //                 in (row sum, index) order (a stable radix sort; the stats and pack kernels gather through it). Query
 //                 block [q0, q0 + QB) visits only columns >= q0, and in its own block only col > row, so each
 //                 unordered pair is tested once; a pair with 1 - value <= cutoff (fp64) adds to both degrees and is
@@ -420,37 +422,14 @@ __global__ void __launch_bounds__(kSelThreads) countScanKernel(const TopkState a
   const uint32_t per = (colEnd - colBeg + gridDim.x - 1) / gridDim.x;
   const uint32_t c0 = min(colEnd, colBeg + blockIdx.x * per), c1 = min(colEnd, c0 + per);
   const int      sa = qr.sum[q];
-  const int      room = kSelItems - k - kSelThreads;  // pending entries from which a round could run out of slots
-  auto cut = [&]() {  // sort list + pending, keep k, raise the bar to the k-th if there is one
-    const int n2 = nextPow2(k + nPend);
-    for (int i = k + nPend + tid; i < n2; i += kSelThreads) val[i] = -1.0, idx[i] = kNoIdx;
-    sortBestFirst(val, idx, n2);
-    if (tid == 0) {
-      nPend = 0;
-      if (idx[k - 1] != kNoIdx && better(val[k - 1], idx[k - 1], barV, barI)) barV = val[k - 1], barI = idx[k - 1];
+  scanBest(val, idx, k, nPend, barV, barI, c0, c1, [&](uint32_t col) {
+    int c = 0;
+    for (long long p = lib.start[col]; p < lib.start[col + 1]; ++p) {
+      const uint32_t v = __ldg(lib.pairs + p);
+      c += min(static_cast<int>(qd[v >> 16]), static_cast<int>(v & 0xffffu));
     }
-    __syncthreads();
-  };
-  for (uint32_t base = c0; base < c1; base += kSelThreads) {
-    const uint32_t col = base + tid;
-    if (col < c1) {
-      int c = 0;
-      for (long long p = lib.start[col]; p < lib.start[col + 1]; ++p) {
-        const uint32_t v = __ldg(lib.pairs + p);
-        c += min(static_cast<int>(qd[v >> 16]), static_cast<int>(v & 0xffffu));
-      }
-      const double v = measureFromCounts<true>(m, c, sa, lib.sum[col]);
-      if (better(v, static_cast<int32_t>(col), barV, barI)) {
-        const int at = k + atomicAdd(&nPend, 1);
-        val[at] = v, idx[at] = static_cast<int32_t>(col);
-      }
-    }
-    __syncthreads();
-    const int pending = nPend;
-    __syncthreads();  // (every thread has read it before the next round adds to it)
-    if (pending > room) cut();
-  }
-  cut();
+    return measureFromCounts<true>(m, c, sa, lib.sum[col]);
+  });
   for (int i = tid; i < k; i += kSelThreads) {
     const size_t at = static_cast<size_t>(q) * a.cap + blockIdx.x * k + i;
     a.candV[at]     = val[i];
@@ -460,10 +439,6 @@ __global__ void __launch_bounds__(kSelThreads) countScanKernel(const TopkState a
 
 // ---- compaction and the checks of every entry point ----
 
-unsigned blocksFor(size_t items, int perBlock) {
-  return static_cast<unsigned>(std::max<size_t>(1, std::min<size_t>((items + perBlock - 1) / perBlock, static_cast<size_t>(smCount()) * 16)));
-}
-
 // A group's compact rows (storage of a CountRows)
 struct CompactRows {
   Scratch<long long> nnz, start;
@@ -471,11 +446,6 @@ struct CompactRows {
   Scratch<uint32_t>  pairs;
   CountRows          view() const { return {pairs.get(), start.get(), sum.get()}; }
 };
-
-__global__ void iotaKernel(int32_t* p, size_t n) {
-  for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x)
-    p[i] = static_cast<int32_t>(i);
-}
 
 // Both groups compacted (b = NULL: one group, used as both), after the range check: the call's one host read. bySum
 // (one group only): the rows are compacted in (row sum, index) order, compact row r being the caller's row order[r].
@@ -573,8 +543,8 @@ __global__ void countBandKernel(const int32_t* __restrict__ sum, size_t n, int q
   if ((threadIdx.x & 31) == 0 && pairs) atomicAdd(&g_countStat[0], pairs);
 }
 
-// counts[] += the degrees and edges[] the (i < j) pairs, caller's indices, of the neighbour graph of x (cursor protocol
-// of b200mol_neighbor_edges), after the range check
+// counts[] += the degrees and edges[] the (i < j) pairs, caller's indices, of the neighbour graph of x (an EdgePass),
+// after the range check
 void countNeighborEdges(const int32_t* d_x, size_t n, int bins, const Measure& m, double cutoff, int32_t* counts, int2* edges,
                         unsigned long long cap, unsigned long long* cursor, cudaStream_t s) {
   resetDeviceCounters(g_countStat, s);
@@ -595,6 +565,12 @@ void countNeighborEdges(const int32_t* d_x, size_t n, int bins, const Measure& m
   p.cutoff = cutoff, p.perm = in.order.get(), p.degrees = counts, p.list = edges, p.cursor = cursor, p.listCap = cap;
   p.unitStart = unitStart.get(), p.bandEnd = bandEnd.get(), p.nBlocks = nBlocks;
   launchPass<kCountNeighbors>(p, s);
+}
+
+EdgePass countEdgePass(const int32_t* d_x, size_t n, int bins, const Measure& m, double cutoff, cudaStream_t s) {
+  return [=](int32_t* counts, int2* edges, unsigned long long cap, unsigned long long* cursor) {
+    countNeighborEdges(d_x, n, bins, m, cutoff, counts, edges, cap, cursor, s);
+  };
 }
 
 }  // namespace
@@ -690,33 +666,20 @@ extern "C" int b200mol_count_threshold(const int32_t* d_q, size_t nQ, const int3
     }
     CountInputs in(d_q, nQ, d_lib, nLib, bins, s);
 
-    // the list: sized for a result that fits `cap`; a longer one is rerun once into a buffer of its exact size
-    const double                allPairs = static_cast<double>(nQ) * static_cast<double>(nLib);
-    const uint64_t              want     = std::min<uint64_t>(cap, 1ull << 27);
-    unsigned long long          listCap  = std::max<unsigned long long>(1, static_cast<unsigned long long>(
-                                                                        std::min(allPairs, static_cast<double>(std::max<uint64_t>(1ull << 20, want)))));
-    Scratch<unsigned long long> stat(4, s);  // [0] listed pairs, [3] the assembly's fill cursor
-    Scratch<int2>               list;
-    Scratch<double>             vals;
-    unsigned long long          listed = 0;
-    for (int attempt = 0;; ++attempt) {
-      list = Scratch<int2>(listCap, s);
-      vals = Scratch<double>(listCap, s);
-      B200_CUDA(cudaMemsetAsync(stat.get(), 0, 4 * sizeof(unsigned long long), s));
+    // the list: sized for a result that fits `cap`
+    const double             allPairs = static_cast<double>(nQ) * static_cast<double>(nLib);
+    const uint64_t           want     = std::min<uint64_t>(cap, 1ull << 27);
+    const unsigned long long firstCap = std::max<unsigned long long>(1, static_cast<unsigned long long>(
+                                          std::min(allPairs, static_cast<double>(std::max<uint64_t>(1ull << 20, want)))));
+    auto listPairs = [&](int2* list, double* vals, unsigned long long listCap, unsigned long long* stat) {
       PassArgs p;
       p.q = in.q, p.lib = in.lib, p.nQ = nQ, p.colBeg = 0, p.colEnd = static_cast<uint32_t>(nLib), p.bins = bins, p.measure = m;
-      p.t = threshold, p.list = list.get(), p.vals = vals.get(), p.cursor = stat.get(), p.listCap = listCap;
+      p.t = threshold, p.list = list, p.vals = vals, p.cursor = stat, p.listCap = listCap;
       launchPass<kCountThreshold>(p, s);
-      B200_CUDA(cudaMemcpyAsync(&listed, stat.get(), sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
-      B200_CUDA(cudaStreamSynchronize(s));
-      if (listed <= listCap) break;
-      B200_REQUIRE(attempt == 0, "count threshold search: the pass listed %llu pairs, then more than that on a rerun", listed);
-      listCap = listed;
-    }
-    *h_nnz = listed;
-    if (listed > cap) return;  // the caller asks again with room for nnz
-    assembleThresholdCsr(list.get(), vals.get(), listed, false, nullptr, nQ, nLib, m.kind, listed, stat.get(), d_indptr, d_indices,
-                         d_values, s);
+    };
+    // the pass lists exactly the result
+    thresholdCsr(firstCap, listPairs, [](const unsigned long long* h) { return h[0]; }, false, nullptr, nQ, nLib, m.kind, d_indptr,
+                 d_indices, d_values, cap, h_nnz, s);
   });
 }
 
@@ -733,15 +696,7 @@ extern "C" int b200mol_count_neighbor_edges(const int32_t* d_x, size_t n, int bi
     if (h_n_edges) *h_n_edges = 0;
     if (n == 0) return;
     B200_REQUIRE(d_counts && (d_edges || edge_cap == 0), "null pointer");
-    Scratch<unsigned long long> cursor(1, s);
-    B200_CUDA(cudaMemsetAsync(cursor.get(), 0, sizeof(unsigned long long), s));
-    countNeighborEdges(d_x, n, bins, m, cutoff, d_counts, reinterpret_cast<int2*>(d_edges), edge_cap, cursor.get(), s);
-    if (h_n_edges) {
-      unsigned long long v = 0;
-      B200_CUDA(cudaMemcpyAsync(&v, cursor.get(), sizeof(v), cudaMemcpyDeviceToHost, s));
-      B200_CUDA(cudaStreamSynchronize(s));  // documented sync: the edge total sizes the CSR
-      *h_n_edges = v;
-    }
+    edgePassWithTotal(countEdgePass(d_x, n, bins, m, cutoff, s), d_counts, reinterpret_cast<int2*>(d_edges), edge_cap, h_n_edges, s);
   });
 }
 
@@ -755,29 +710,8 @@ extern "C" int b200mol_count_butina_fused(const int32_t* d_x, size_t n, int bins
     B200_REQUIRE(cutoff >= 0.0 && cutoff <= 1.0, "cutoff must be in [0, 1], got %g", cutoff);
     requireCountInputs(d_x, n, n, bins);
     const cudaStream_t s = asStream(stream);
-    if (n == 0) {
-      if (h_n_clusters) *h_n_clusters = 0;
-      if (d_n_clusters) B200_CUDA(cudaMemsetAsync(d_n_clusters, 0, sizeof(int32_t), s));
-      return;
-    }
+    if (n == 0) return noClusters(d_n_clusters, h_n_clusters, s);
     B200_REQUIRE(d_cluster_ids, "null pointer");
-    Scratch<int32_t> counts(n, s);
-    // the edge list of b200mol_butina_fused: 64 per point, and one rerun at the exact size for a denser graph
-    unsigned long long cap = static_cast<unsigned long long>(n) * 64ull;
-    Scratch<int2>      edges;
-    uint64_t           nEdges = 0;
-    for (int attempt = 0; attempt < 2; ++attempt) {
-      edges = Scratch<int2>(cap, s);
-      B200_CUDA(cudaMemsetAsync(counts.get(), 0, n * sizeof(int32_t), s));
-      const int rc = b200mol_count_neighbor_edges(d_x, n, bins, alpha, beta, cutoff, counts.get(),
-                                                  reinterpret_cast<int32_t*>(edges.get()), cap, &nEdges, stream);
-      if (rc != B200MOL_OK) fail(rc, "%s", g_lastError.c_str());
-      if (nEdges <= cap) break;
-      B200_REQUIRE(attempt == 0, "edge list overflow after resize");
-      cap = nEdges;
-    }
-    const int rc = b200mol_butina_from_edges(n, counts.get(), reinterpret_cast<const int32_t*>(edges.get()), nEdges,
-                                             d_cluster_ids, d_centroids, d_n_clusters, h_n_clusters, stream);
-    if (rc != B200MOL_OK) fail(rc, "%s", g_lastError.c_str());
+    fusedButina(n, countEdgePass(d_x, n, bins, m, cutoff, s), d_cluster_ids, d_centroids, d_n_clusters, h_n_clusters, s);
   });
 }

@@ -3,6 +3,7 @@
 #pragma once
 #include <cstddef>
 #include <cstdint>
+#include <functional>
 
 #include "common.cuh"
 
@@ -134,13 +135,32 @@ void launchTopkTile(const Measure& m, const uint8_t* expQ, size_t nQ, const int3
                     const int32_t* popCols, int words, const int4* bar, uint32_t* cand, uint32_t* count, uint32_t cap,
                     uint32_t colBase, cudaStream_t s);
 
-// ---- threshold search: the assembly of threshold.cu, steps (b) to (d) ----
-// list[0 .. listed) the listed pairs (i, j) (i = -1: dropped) with their values vals[], nnz the entries they give (kept
-// pairs, twice in a symmetric search, plus one diagonal entry per row of popX > 0 then): written to the caller's CSR
-// indptr [nX + 1], indices / values [nnz], columns ascending. nCols: the column count; stat: threshold.cu's four
-// counters, of which stat[3], zero on entry, is the fill cursor.
-void assembleThresholdCsr(const int2* list, const double* vals, unsigned long long listed, bool symmetric, const int32_t* popX,
-                          size_t nX, size_t nCols, MeasureKind kind, unsigned long long nnz, unsigned long long* stat,
-                          int64_t* indptr, int32_t* indices, double* values, cudaStream_t s);
+// ---- threshold search (threshold.cu): one attempt protocol for packed bits and count vectors ----
+// listPairs(list, vals, listCap, stat) enqueues the work that lists the pairs (i, j) of one attempt, at most listCap of
+// them, with their values (i = -1: dropped), counting them at stat[0]; it may count kept pairs at stat[1] and non-empty
+// rows at stat[2]. stat is zero on entry. nnzOf(stat) is the result size those counts give.
+using ListPairs = std::function<void(int2* list, double* vals, unsigned long long listCap, unsigned long long* stat)>;
+using ResultSize = std::function<unsigned long long(const unsigned long long* stat)>;
+// The pass from a list of listCap entries, rerun once into a list of the exact size when it listed more; one host read
+// per attempt. *hNnz = the result size; when it fits `cap` the pairs are written to the caller's CSR, indptr [nX + 1],
+// indices / values [nnz], columns ascending: each kept pair, twice in a symmetric search together with one diagonal
+// entry per row of popX > 0. nCols: the column count.
+void thresholdCsr(unsigned long long listCap, const ListPairs& listPairs, const ResultSize& nnzOf, bool symmetric,
+                  const int32_t* popX, size_t nX, size_t nCols, MeasureKind kind, int64_t* indptr, int32_t* indices,
+                  double* values, uint64_t cap, uint64_t* hNnz, cudaStream_t s);
+
+// ---- fused Butina (butina.cu): one driver for the bit and the count pass ----
+// One pass over the pairs of a neighbour graph: counts[] += the degrees, and the (i < j) pairs appended to edges[] at
+// *cursor while below cap (the cursor ends at the pair total).
+using EdgePass = std::function<void(int32_t* counts, int2* edges, unsigned long long cap, unsigned long long* cursor)>;
+// The pass with a zeroed cursor of its own; *hNEdges (when given) = the pair total, read with a stream synchronise.
+void edgePassWithTotal(const EdgePass& pass, int32_t* counts, int2* edges, unsigned long long cap, uint64_t* hNEdges,
+                       cudaStream_t s);
+// Butina on n > 0 points from their pass: an edge list of 64 per point, one rerun at the exact size for a denser graph,
+// then the clusters as b200mol_butina_from_edges makes them (centroids and dNClusters may be NULL).
+void fusedButina(size_t n, const EdgePass& pass, int32_t* ids, int32_t* centroids, int32_t* dNClusters, int32_t* hNClusters,
+                 cudaStream_t s);
+// The result of clustering no points: zero clusters, in *hNClusters and *dNClusters where given.
+void noClusters(int32_t* dNClusters, int32_t* hNClusters, cudaStream_t s);
 
 }  // namespace b200

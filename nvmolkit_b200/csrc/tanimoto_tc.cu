@@ -157,11 +157,6 @@ __global__ void expandBitsSuperKernel(const uint32_t* __restrict__ fp, size_t n,
   out[2 * t + 1] = make_uint4(b[4], b[5], b[6], b[7]);
 }
 
-__global__ void iotaKernel(int32_t* __restrict__ v, size_t n) {
-  const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i < n) v[i] = static_cast<int32_t>(i);
-}
-
 // out row i = fp row perm[i]; one thread per 16 bytes
 __global__ void gatherRowsKernel(const uint4* __restrict__ fp, const int32_t* __restrict__ perm, size_t n, int chunks,
                                  uint4* __restrict__ out) {

@@ -157,83 +157,8 @@ int bitsFor(size_t n) {  // bits that hold 0 .. n - 1
   return b;
 }
 
-unsigned blocksFor(unsigned long long items, int perBlock) {
-  return static_cast<unsigned>(std::max<unsigned long long>(1, std::min<unsigned long long>((items + perBlock - 1) / perBlock,
-                                                                                            static_cast<unsigned long long>(smCount()) * 16)));
-}
-
-void thresholdSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t nLib, bool self, int words, const Measure& m, double t,
-                     int64_t* indptr, int32_t* indices, double* values, uint64_t cap, uint64_t* hNnz, cudaStream_t s) {
-  Scratch<int32_t> popQ(nQ, s), popLibOwn(self ? 0 : nLib, s), counts(nQ, s);
-  launchRowPopcount(q, nQ, words, popQ.get(), s);
-  if (!self) launchRowPopcount(lib, nLib, words, popLibOwn.get(), s);
-  const int32_t* popLib = self ? popQ.get() : popLibOwn.get();
-  Scratch<unsigned long long> stat(4, s);
-
-  // The pass's list: sized for a result that fits `cap` (a self search lists each off-diagonal pair once), plus room
-  // for the cosine tile's near misses; a longer list is rerun into a buffer of its exact size.
-  const double       allPairs = self ? static_cast<double>(nQ) * (static_cast<double>(nQ) - 1.0) / 2.0
-                                     : static_cast<double>(nQ) * static_cast<double>(nLib);
-  const uint64_t     want     = std::min<uint64_t>(self ? cap / 2 : cap, 1ull << 27);
-  unsigned long long listCap  = std::max<unsigned long long>(1, static_cast<unsigned long long>(
-                                                                  std::min(allPairs, static_cast<double>(std::max<uint64_t>(1ull << 20, want + want / 8)))));
-  unsigned long long h[4]     = {0, 0, 0, 0};
-  Scratch<int2>      list;
-  Scratch<double>    vals;
-  for (int attempt = 0;; ++attempt) {
-    list = Scratch<int2>(listCap, s);
-    vals = Scratch<double>(listCap, s);
-    B200_CUDA(cudaMemsetAsync(stat.get(), 0, 4 * sizeof(unsigned long long), s));
-    {
-      PhaseTimer timer("threshold_pass", s);
-      SimLaunch  p;
-      p.x         = q;
-      p.y         = lib;
-      p.nX        = nQ;
-      p.nY        = nLib;
-      p.words     = words;
-      p.measure   = m;
-      p.cutoff    = t;
-      p.atLeast   = true;
-      p.rowCounts = counts.get();
-      p.symmetric = self;
-      p.edges     = list.get();
-      p.edgeCursor = stat.get();
-      p.edgeCap   = listCap;
-      B200_CUDA(cudaMemsetAsync(counts.get(), 0, nQ * sizeof(int32_t), s));
-      // Tanimoto and Dice count with their exact tables; cosine and Tversky list by a float bound
-      launchSimilarity(m.kind == kCosine || m.kind == kTversky ? kList : kCount, p, s);
-    }
-    {
-      PhaseTimer timer("threshold_recount", s);
-      const unsigned blocks = blocksFor(listCap * kRecountLanes, 256);
-      const auto     recount = isWeighted(m.kind) ? recountKernel<true> : recountKernel<false>;
-      recount<<<blocks, 256, 0, s>>>(q, lib, words, popQ.get(), popLib, m, t, list.get(), listCap, vals.get(), stat.get());
-      B200_LAUNCHED();
-      if (self) {
-        nonEmptyKernel<<<static_cast<unsigned>((nQ + 255) / 256), 256, 0, s>>>(popQ.get(), nQ, stat.get());
-        B200_LAUNCHED();
-      }
-    }
-    // the one host read of an attempt
-    B200_CUDA(cudaMemcpyAsync(h, stat.get(), 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
-    B200_CUDA(cudaStreamSynchronize(s));
-    if (h[0] <= listCap) break;
-    B200_REQUIRE(attempt == 0, "threshold search: the pass listed %llu pairs, then more than that on a rerun", h[0]);
-    listCap = h[0];
-  }
-  const unsigned long long listed = h[0];
-  const unsigned long long nnz    = (self ? 2 * h[1] + h[2] : h[1]);
-  *hNnz                           = nnz;
-  if (nnz > cap) return;  // the caller asks again with room for nnz
-
-  PhaseTimer timer("threshold_assembly", s);
-  assembleThresholdCsr(list.get(), vals.get(), listed, self, popQ.get(), nQ, self ? nQ : nLib, m.kind, nnz, stat.get(), indptr,
-                       indices, values, s);
-}
-
-}  // namespace
-
+// (b) to (d): list[0 .. listed) the listed pairs (i, j) (i = -1: dropped) with their values vals[], nnz the entries they
+// give, written to the caller's CSR; stat[3], zero on entry, is the fill cursor
 void assembleThresholdCsr(const int2* list, const double* vals, unsigned long long listed, bool symmetric, const int32_t* popX,
                           size_t nX, size_t nCols, MeasureKind kind, unsigned long long nnz, unsigned long long* stat,
                           int64_t* indptr, int32_t* indices, double* values, cudaStream_t s) {
@@ -257,6 +182,88 @@ void assembleThresholdCsr(const int2* list, const double* vals, unsigned long lo
   B200_LAUNCHED();
 }
 
+}  // namespace
+
+void thresholdCsr(unsigned long long listCap, const ListPairs& listPairs, const ResultSize& nnzOf, bool symmetric,
+                  const int32_t* popX, size_t nX, size_t nCols, MeasureKind kind, int64_t* indptr, int32_t* indices,
+                  double* values, uint64_t cap, uint64_t* hNnz, cudaStream_t s) {
+  Scratch<unsigned long long> stat(4, s);
+  unsigned long long          h[3] = {0, 0, 0};
+  Scratch<int2>               list;
+  Scratch<double>             vals;
+  for (int attempt = 0;; ++attempt) {
+    list = Scratch<int2>(listCap, s);
+    vals = Scratch<double>(listCap, s);
+    B200_CUDA(cudaMemsetAsync(stat.get(), 0, 4 * sizeof(unsigned long long), s));
+    listPairs(list.get(), vals.get(), listCap, stat.get());
+    // the one host read of an attempt
+    B200_CUDA(cudaMemcpyAsync(h, stat.get(), sizeof(h), cudaMemcpyDeviceToHost, s));
+    B200_CUDA(cudaStreamSynchronize(s));
+    if (h[0] <= listCap) break;
+    B200_REQUIRE(attempt == 0, "threshold search: the pass listed %llu pairs, then more than that on a rerun", h[0]);
+    listCap = h[0];
+  }
+  const unsigned long long nnz = nnzOf(h);
+  *hNnz                        = nnz;
+  if (nnz > cap) return;  // the caller asks again with room for nnz
+
+  PhaseTimer timer("threshold_assembly", s);
+  assembleThresholdCsr(list.get(), vals.get(), h[0], symmetric, popX, nX, nCols, kind, nnz, stat.get(), indptr, indices, values, s);
+}
+
+namespace {
+
+void thresholdSearch(const uint32_t* q, size_t nQ, const uint32_t* lib, size_t nLib, bool self, int words, const Measure& m, double t,
+                     int64_t* indptr, int32_t* indices, double* values, uint64_t cap, uint64_t* hNnz, cudaStream_t s) {
+  Scratch<int32_t> popQ(nQ, s), popLibOwn(self ? 0 : nLib, s), counts(nQ, s);
+  launchRowPopcount(q, nQ, words, popQ.get(), s);
+  if (!self) launchRowPopcount(lib, nLib, words, popLibOwn.get(), s);
+  const int32_t* popLib = self ? popQ.get() : popLibOwn.get();
+
+  // The pass's list: sized for a result that fits `cap` (a self search lists each off-diagonal pair once), plus room
+  // for the cosine tile's near misses.
+  const double   allPairs = self ? static_cast<double>(nQ) * (static_cast<double>(nQ) - 1.0) / 2.0
+                                 : static_cast<double>(nQ) * static_cast<double>(nLib);
+  const uint64_t want     = std::min<uint64_t>(self ? cap / 2 : cap, 1ull << 27);
+  const unsigned long long firstCap = std::max<unsigned long long>(1, static_cast<unsigned long long>(
+                                        std::min(allPairs, static_cast<double>(std::max<uint64_t>(1ull << 20, want + want / 8)))));
+  auto listPairs = [&](int2* list, double* vals, unsigned long long listCap, unsigned long long* stat) {
+    {
+      PhaseTimer timer("threshold_pass", s);
+      SimLaunch  p;
+      p.x         = q;
+      p.y         = lib;
+      p.nX        = nQ;
+      p.nY        = nLib;
+      p.words     = words;
+      p.measure   = m;
+      p.cutoff    = t;
+      p.atLeast   = true;
+      p.rowCounts = counts.get();
+      p.symmetric = self;
+      p.edges     = list;
+      p.edgeCursor = stat;
+      p.edgeCap   = listCap;
+      B200_CUDA(cudaMemsetAsync(counts.get(), 0, nQ * sizeof(int32_t), s));
+      // Tanimoto and Dice count with their exact tables; cosine and Tversky list by a float bound
+      launchSimilarity(m.kind == kCosine || m.kind == kTversky ? kList : kCount, p, s);
+    }
+    PhaseTimer     timer("threshold_recount", s);
+    const unsigned blocks  = blocksFor(listCap * kRecountLanes, 256);
+    const auto     recount = isWeighted(m.kind) ? recountKernel<true> : recountKernel<false>;
+    recount<<<blocks, 256, 0, s>>>(q, lib, words, popQ.get(), popLib, m, t, list, listCap, vals, stat);
+    B200_LAUNCHED();
+    if (self) {
+      nonEmptyKernel<<<static_cast<unsigned>((nQ + 255) / 256), 256, 0, s>>>(popQ.get(), nQ, stat);
+      B200_LAUNCHED();
+    }
+  };
+  // the pairs the re-count keeps, mirrored in a self search together with the non-empty queries' diagonal
+  auto nnzOf = [self](const unsigned long long* h) { return self ? 2 * h[1] + h[2] : h[1]; };
+  thresholdCsr(firstCap, listPairs, nnzOf, self, popQ.get(), nQ, self ? nQ : nLib, m.kind, indptr, indices, values, cap, hNnz, s);
+}
+
+}  // namespace
 }  // namespace b200
 
 using namespace b200;

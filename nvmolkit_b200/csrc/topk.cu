@@ -79,38 +79,15 @@ __global__ void __launch_bounds__(kSelThreads) topkScanKernel(const TopkArgs a, 
   const uint32_t per = (colEnd - colBeg + gridDim.x - 1) / gridDim.x;
   const uint32_t c0 = min(colEnd, colBeg + blockIdx.x * per), c1 = min(colEnd, c0 + per);
   const int      pa = a.popQ[q], chunks = a.words / 4;
-  const int      room = kSelItems - k - kSelThreads;  // pending entries from which a round could run out of slots
-  auto cut = [&]() {  // sort list + pending, keep k, raise the bar to the k-th if there is one
-    const int n2 = nextPow2(k + nPend);
-    for (int i = k + nPend + tid; i < n2; i += kSelThreads) val[i] = -1.0, idx[i] = kNoIdx;
-    sortBestFirst(val, idx, n2);
-    if (tid == 0) {
-      nPend = 0;
-      if (idx[k - 1] != kNoIdx && better(val[k - 1], idx[k - 1], barV, barI)) barV = val[k - 1], barI = idx[k - 1];
+  scanBest(val, idx, k, nPend, barV, barI, c0, c1, [&](uint32_t col) {
+    const uint4* row = reinterpret_cast<const uint4*>(a.lib + static_cast<size_t>(col) * a.words);
+    int          c   = 0;
+    for (int w = 0; w < chunks; ++w) {
+      const uint4 y = __ldg(row + w), x = reinterpret_cast<const uint4*>(sq)[w];
+      c += __popc(x.x & y.x) + __popc(x.y & y.y) + __popc(x.z & y.z) + __popc(x.w & y.w);
     }
-    __syncthreads();
-  };
-  for (uint32_t base = c0; base < c1; base += kSelThreads) {
-    const uint32_t col = base + tid;
-    if (col < c1) {
-      const uint4* row = reinterpret_cast<const uint4*>(a.lib + static_cast<size_t>(col) * a.words);
-      int          c   = 0;
-      for (int w = 0; w < chunks; ++w) {
-        const uint4 y = __ldg(row + w), x = reinterpret_cast<const uint4*>(sq)[w];
-        c += __popc(x.x & y.x) + __popc(x.y & y.y) + __popc(x.z & y.z) + __popc(x.w & y.w);
-      }
-      const double v = measureFromCounts<WEIGHTED>(a.measure, c, pa, a.popLib[col]);
-      if (better(v, static_cast<int32_t>(col), barV, barI)) {
-        const int at = k + atomicAdd(&nPend, 1);
-        val[at] = v, idx[at] = static_cast<int32_t>(col);
-      }
-    }
-    __syncthreads();
-    const int pending = nPend;
-    __syncthreads();  // (every thread has read it before the next round adds to it)
-    if (pending > room) cut();
-  }
-  cut();
+    return measureFromCounts<WEIGHTED>(a.measure, c, pa, a.popLib[col]);
+  });
   for (int i = tid; i < k; i += kSelThreads)
     a.cand[static_cast<size_t>(q) * a.cap + blockIdx.x * k + i] = idx[i] == kNoIdx ? kNoCand : static_cast<uint32_t>(idx[i]);
 }

@@ -1,5 +1,6 @@
 // What the exact top-k searches share (topk.cu on packed bits, count_similarity.cu on count vectors): the order of the
-// contract, the CTA-wide bitonic sort of the select and scan kernels, and the sizes of their lists and candidate slots.
+// contract, the CTA-wide bitonic sort of the select and scan kernels, the scan kernels' CTA-local list, and the sizes of
+// their lists and candidate slots.
 #pragma once
 #include <cstdint>
 
@@ -46,6 +47,42 @@ __device__ __forceinline__ int nextPow2(int n) {
   int p = 2;
   while (p < n) p <<= 1;
   return p;
+}
+
+// The CTA-local list of a scan kernel: columns [c0, c1) of one query, a thread per column, value(col) the column's fp64
+// value. A column that beats the bar (barV, barI) is parked in val / idx [k ..); when that fills up, the parked entries
+// are sorted with the list [0, k) and cut to k, which raises the bar. A final cut leaves the CTA's k best, best first,
+// in val / idx [0, k). nPend (0), barV and barI are in shared memory, set before the call. Called by the whole CTA.
+template <class Value>
+__device__ __forceinline__ void scanBest(double* val, int32_t* idx, int k, int& nPend, double& barV, int32_t& barI, uint32_t c0,
+                                         uint32_t c1, Value value) {
+  const int tid  = threadIdx.x;
+  const int room = kSelItems - k - kSelThreads;  // pending entries from which a round could run out of slots
+  auto cut = [&]() {  // sort list + pending, keep k, raise the bar to the k-th if there is one
+    const int n2 = nextPow2(k + nPend);
+    for (int i = k + nPend + tid; i < n2; i += kSelThreads) val[i] = -1.0, idx[i] = kNoIdx;
+    sortBestFirst(val, idx, n2);
+    if (tid == 0) {
+      nPend = 0;
+      if (idx[k - 1] != kNoIdx && better(val[k - 1], idx[k - 1], barV, barI)) barV = val[k - 1], barI = idx[k - 1];
+    }
+    __syncthreads();
+  };
+  for (uint32_t base = c0; base < c1; base += kSelThreads) {
+    const uint32_t col = base + tid;
+    if (col < c1) {
+      const double v = value(col);
+      if (better(v, static_cast<int32_t>(col), barV, barI)) {
+        const int at = k + atomicAdd(&nPend, 1);
+        val[at] = v, idx[at] = static_cast<int32_t>(col);
+      }
+    }
+    __syncthreads();
+    const int pending = nPend;
+    __syncthreads();  // (every thread has read it before the next round adds to it)
+    if (pending > room) cut();
+  }
+  cut();
 }
 
 }  // namespace

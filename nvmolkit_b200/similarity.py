@@ -8,13 +8,16 @@ import numpy as np
 import torch
 
 from nvmolkit_b200 import _lib
-from nvmolkit_b200._interop import as_tensor, fingerprint_matrix, require_cuda, stream_ctx, stream_ptr
+from nvmolkit_b200._interop import as_tensor, check_stream, fingerprint_matrix, require_cuda, stream_ctx, stream_ptr
 from nvmolkit_b200.types import AsyncGpuResult
 
 
-def _entry(operation: str, measure):
+def _entry(operation: str, measure, counts: bool = False):
     """The C entry point of an operation ("cross", "topk", "threshold" or "cross_host") for a measure (a key of
-    _lib.METRIC, or the (alpha, beta) of Tversky), and the measure's arguments to it."""
+    _lib.METRIC, or the (alpha, beta) of Tversky), and the measure's arguments to it. counts: the entry point on count
+    vectors ("cross", "topk" or "threshold"), which takes every measure as its (alpha, beta)."""
+    if counts:
+        return f"b200mol_count_{operation}", measure
     if not isinstance(measure, str):
         return f"b200mol_tversky_{operation}", measure
     if operation == "cross":  # (one entry point per metric)
@@ -22,26 +25,42 @@ def _entry(operation: str, measure):
     return f"b200mol_similarity_{operation}", (_lib.METRIC[measure],)
 
 
-def _check_width(a, b) -> None:
+def _check_width(a, b, counts: bool = False) -> None:
     if b is not None and a.shape[1] != b.shape[1]:
+        if counts:
+            raise ValueError(f"count vector widths differ: {a.shape[1]} vs {b.shape[1]} bins")
         raise ValueError(f"fingerprint widths differ: {a.shape[1]} vs {b.shape[1]} words")
 
 
-def _fingerprints(one, two):
-    """CUDA, both fingerprint matrices and their widths; b is None for a search of group one against itself."""
+def _fingerprints(one, two, counts: bool = False):
+    """CUDA, both matrices (packed bits, or count vectors when counts) and their widths; b is None for a search of
+    group one against itself."""
     require_cuda()
-    a = fingerprint_matrix(one, "fingerprint_group_one")
-    b = None if two is None else fingerprint_matrix(two, "fingerprint_group_two")
-    _check_width(a, b)
+    check = _count_matrix if counts else fingerprint_matrix
+    a = check(one, "fingerprint_group_one")
+    b = None if two is None else check(two, "fingerprint_group_two")
+    _check_width(a, b, counts)
     return a, b
 
 
-def _operands(one, two, stream):
-    """The stream pointer and both fingerprint matrices (b = a when group two is None), the stream checked first, like
-    the reference (TypeError)."""
+def _operands(one, two, stream, counts: bool):
+    """The stream pointer and both matrices (b None for a self search), the stream checked first, like the reference
+    (TypeError)."""
     sptr = stream_ptr(stream)
-    a, b = _fingerprints(one, two)
-    return sptr, a, a if b is None else b
+    return (sptr, *_fingerprints(one, two, counts))
+
+
+def _prepare(x, counts: bool):
+    """A checked matrix as the binding passes it (None stays None), on the call's stream: count vectors as int32."""
+    return x.to(torch.int32).contiguous() if counts and x is not None else x
+
+
+def _library(a, b, counts: bool):
+    """The library a cross or top-k call passes: group two's, else for a self search group one's own (packed bits) or
+    none (count vectors)."""
+    if b is not None:
+        return b.data_ptr()
+    return None if counts else a.data_ptr()
 
 
 def _keep_alive(*tensors) -> None:
@@ -51,12 +70,15 @@ def _keep_alive(*tensors) -> None:
             x.record_stream(torch.cuda.current_stream())
 
 
-def _cross(measure, one, two, stream) -> AsyncGpuResult:
-    sptr, a, b = _operands(one, two, stream)
-    fn, args = _entry("cross", measure)
+def _cross(measure, one, two, stream, counts: bool = False) -> AsyncGpuResult:
+    sptr, a, b = _operands(one, two, stream, counts)
+    n_b = (a if b is None else b).shape[0]
+    fn, args = _entry("cross", measure, counts)
     with stream_ctx(stream):
-        out = torch.empty((a.shape[0], b.shape[0]), dtype=torch.float64, device=a.device)
-        _lib.call(fn, a.data_ptr(), a.shape[0], b.data_ptr(), b.shape[0], a.shape[1], *args, out.data_ptr(), sptr)
+        a, b = _prepare(a, counts), _prepare(b, counts)
+        out = torch.empty((a.shape[0], n_b), dtype=torch.float64, device=a.device)
+        _lib.call(fn, a.data_ptr(), a.shape[0], _library(a, b, counts), n_b, a.shape[1], *args, out.data_ptr(),
+                  sptr)
         _keep_alive(a, b)
     return AsyncGpuResult(out)
 
@@ -81,15 +103,17 @@ def _check_k(k, library_size: int) -> int:
     return k
 
 
-def _topk(measure, one, two, k, stream):
-    sptr, a, b = _operands(one, two, stream)
-    k = _check_k(k, b.shape[0])
-    fn, args = _entry("topk", measure)
+def _topk(measure, one, two, k, stream, counts: bool = False):
+    sptr, a, b = _operands(one, two, stream, counts)
+    n_lib = (a if b is None else b).shape[0]
+    k = _check_k(k, n_lib)
+    fn, args = _entry("topk", measure, counts)
     with stream_ctx(stream):
+        a, b = _prepare(a, counts), _prepare(b, counts)
         values = torch.empty((a.shape[0], k), dtype=torch.float64, device=a.device)
         indices = torch.empty((a.shape[0], k), dtype=torch.int32, device=a.device)
-        _lib.call(fn, a.data_ptr(), a.shape[0], b.data_ptr(), b.shape[0], a.shape[1], *args, k, values.data_ptr(),
-                  indices.data_ptr(), sptr)
+        _lib.call(fn, a.data_ptr(), a.shape[0], _library(a, b, counts), n_lib, a.shape[1], *args, k,
+                  values.data_ptr(), indices.data_ptr(), sptr)
         _keep_alive(a, b)
     return AsyncGpuResult(values), AsyncGpuResult(indices)
 
@@ -118,12 +142,14 @@ def _check_threshold(threshold) -> float:
     return t
 
 
-def _threshold(measure, one, two, threshold, stream):
-    sptr = stream_ptr(stream)  # validates `stream` first, like the matrix calls (TypeError)
+def _threshold(measure, one, two, threshold, stream, counts: bool = False):
+    check_stream(stream)  # first, like the matrix calls (TypeError)
     t = _check_threshold(threshold)
-    a, b = _fingerprints(one, two)
+    sptr = stream_ptr(stream)
+    a, b = _fingerprints(one, two, counts)
     n_q, n_lib = a.shape[0], (a.shape[0] if b is None else b.shape[0])
     with stream_ctx(stream):
+        a, b = _prepare(a, counts), _prepare(b, counts)
         if n_q == 0 or n_lib == 0:  # no pair (and an empty tensor's address may be 0, the C-ABI's "no library")
             return (AsyncGpuResult(torch.zeros(n_q + 1, dtype=torch.int64, device=a.device)),
                     AsyncGpuResult(torch.empty(0, dtype=torch.int32, device=a.device)),
@@ -131,7 +157,7 @@ def _threshold(measure, one, two, threshold, stream):
         indptr = torch.empty(n_q + 1, dtype=torch.int64, device=a.device)
         # a first guess at the result size; a larger result is reported and the call is made once more with room for it
         cap = min(max(1 << 20, 64 * n_q), n_q * n_lib)
-        fn, args = _entry("threshold", measure)
+        fn, args = _entry("threshold", measure, counts)
         for _ in range(2):
             indices = torch.empty(cap, dtype=torch.int32, device=a.device)
             values = torch.empty(cap, dtype=torch.float64, device=a.device)
@@ -305,90 +331,18 @@ def _count_matrix(obj, name: str) -> torch.Tensor:
     return t
 
 
-def _count_operands(one, two):
-    """Both count matrices, checked (b None: group one against itself)."""
-    require_cuda()
-    a = _count_matrix(one, "fingerprint_group_one")
-    b = None if two is None else _count_matrix(two, "fingerprint_group_two")
-    if b is not None and a.shape[1] != b.shape[1]:
-        raise ValueError(f"count vector widths differ: {a.shape[1]} vs {b.shape[1]} bins")
-    return a, b
-
-
-def _int32(*xs):
-    """the count matrices as the binding passes them (on the call's stream, after every check)"""
-    return tuple(None if x is None else x.to(torch.int32).contiguous() for x in xs)
-
-
-def _count_cross(weights, one, two, stream) -> AsyncGpuResult:
-    sptr = stream_ptr(stream)
-    a, b = _count_operands(one, two)
-    n_b = a.shape[0] if b is None else b.shape[0]
-    with stream_ctx(stream):
-        a, b = _int32(a, b)
-        out = torch.empty((a.shape[0], n_b), dtype=torch.float64, device=a.device)
-        _lib.call("b200mol_count_cross", a.data_ptr(), a.shape[0], None if b is None else b.data_ptr(), n_b, a.shape[1],
-                  *weights, out.data_ptr(), sptr)
-        _keep_alive(a, b)
-    return AsyncGpuResult(out)
-
-
-def _count_topk(weights, one, two, k, stream):
-    sptr = stream_ptr(stream)
-    a, b = _count_operands(one, two)
-    n_b = a.shape[0] if b is None else b.shape[0]
-    k = _check_k(k, n_b)
-    with stream_ctx(stream):
-        a, b = _int32(a, b)
-        values = torch.empty((a.shape[0], k), dtype=torch.float64, device=a.device)
-        indices = torch.empty((a.shape[0], k), dtype=torch.int32, device=a.device)
-        _lib.call("b200mol_count_topk", a.data_ptr(), a.shape[0], None if b is None else b.data_ptr(), n_b,
-                  a.shape[1], *weights, k, values.data_ptr(), indices.data_ptr(), sptr)
-        _keep_alive(a, b)
-    return AsyncGpuResult(values), AsyncGpuResult(indices)
-
-
-def _count_threshold(weights, one, two, threshold, stream):
-    t = _check_threshold(threshold)
-    sptr = stream_ptr(stream)
-    a, b = _count_operands(one, two)
-    n_q, n_lib = a.shape[0], (a.shape[0] if b is None else b.shape[0])
-    with stream_ctx(stream):
-        a, b = _int32(a, b)
-        if n_q == 0 or n_lib == 0:  # no pair
-            return (AsyncGpuResult(torch.zeros(n_q + 1, dtype=torch.int64, device=a.device)),
-                    AsyncGpuResult(torch.empty(0, dtype=torch.int32, device=a.device)),
-                    AsyncGpuResult(torch.empty(0, dtype=torch.float64, device=a.device)))
-        indptr = torch.empty(n_q + 1, dtype=torch.int64, device=a.device)
-        # a first guess at the result size; a larger result is reported and the call is made once more with room for it
-        cap = min(max(1 << 20, 64 * n_q), n_q * n_lib)
-        for _ in range(2):
-            indices = torch.empty(cap, dtype=torch.int32, device=a.device)
-            values = torch.empty(cap, dtype=torch.float64, device=a.device)
-            nnz = C.c_uint64(0)
-            _lib.call("b200mol_count_threshold", a.data_ptr(), n_q, None if b is None else b.data_ptr(), n_lib,
-                      a.shape[1], *weights, t, indptr.data_ptr(), indices.data_ptr(), values.data_ptr(), cap,
-                      C.byref(nnz), sptr)
-            if nnz.value <= cap:
-                break
-            cap = int(nnz.value)
-        _keep_alive(a, b)
-    n = int(nnz.value)
-    return AsyncGpuResult(indptr), AsyncGpuResult(indices[:n]), AsyncGpuResult(values[:n])
-
-
 def crossTanimotoCountSimilarity(fingerprint_group_one, fingerprint_group_two=None, stream=None) -> AsyncGpuResult:
     """(n, m) fp64 Tanimoto similarities of count vectors, c / (a + b - c) with a, b the row sums and c the sum of the
     bin-wise minima (0 when c == 0), RDKit's ``TanimotoSimilarity`` on count fingerprints bit for bit; all-to-all within
     group one when group two is None. Inputs: 2D uint8, int16 or int32 CUDA tensors (or ``AsyncGpuResult``) of counts in
     ``0 .. 65535``, 1 to 4096 bins, e.g. ``GetCountFingerprints``. Synchronises ``stream`` (the range check)."""
-    return _count_cross(TANIMOTO, fingerprint_group_one, fingerprint_group_two, stream)
+    return _cross(TANIMOTO, fingerprint_group_one, fingerprint_group_two, stream, counts=True)
 
 
 def crossDiceCountSimilarity(fingerprint_group_one, fingerprint_group_two=None, stream=None) -> AsyncGpuResult:
     """Dice twin of ``crossTanimotoCountSimilarity``: 2c / (a + b), RDKit's ``DiceSimilarity`` on count fingerprints
     bit for bit. Synchronises ``stream``."""
-    return _count_cross(DICE, fingerprint_group_one, fingerprint_group_two, stream)
+    return _cross(DICE, fingerprint_group_one, fingerprint_group_two, stream, counts=True)
 
 
 def crossTverskyCountSimilarity(fingerprint_group_one, fingerprint_group_two=None, *, alpha, beta,
@@ -397,7 +351,7 @@ def crossTverskyCountSimilarity(fingerprint_group_one, fingerprint_group_two=Non
     only the row (group one) has. ``0 <= alpha, beta <= 1000``. See the module note on RDKit parity. Synchronises
     ``stream``."""
     weights = _check_weights(alpha, beta)  # (before anything touches the device)
-    return _count_cross(weights, fingerprint_group_one, fingerprint_group_two, stream)
+    return _cross(weights, fingerprint_group_one, fingerprint_group_two, stream, counts=True)
 
 
 def topKTanimotoCountSimilarity(fingerprint_group_one, fingerprint_group_two=None, k=10, stream=None):
@@ -405,18 +359,18 @@ def topKTanimotoCountSimilarity(fingerprint_group_one, fingerprint_group_two=Non
     when None): ``(values, indices)``, fp64 and int32 ``[Q, k]``, the first k columns of each row of
     ``crossTanimotoCountSimilarity`` ordered by (value descending, column ascending), values bit-identical to the matrix.
     The matrix is never stored. ``1 <= k <= min(len(library), TOPK_MAX)``. Synchronises ``stream`` (the range check)."""
-    return _count_topk(TANIMOTO, fingerprint_group_one, fingerprint_group_two, k, stream)
+    return _topk(TANIMOTO, fingerprint_group_one, fingerprint_group_two, k, stream, counts=True)
 
 
 def topKDiceCountSimilarity(fingerprint_group_one, fingerprint_group_two=None, k=10, stream=None):
     """Dice twin of ``topKTanimotoCountSimilarity``: rows of ``crossDiceCountSimilarity``."""
-    return _count_topk(DICE, fingerprint_group_one, fingerprint_group_two, k, stream)
+    return _topk(DICE, fingerprint_group_one, fingerprint_group_two, k, stream, counts=True)
 
 
 def topKTverskyCountSimilarity(fingerprint_group_one, fingerprint_group_two=None, k=10, *, alpha, beta, stream=None):
     """Tversky twin of ``topKTanimotoCountSimilarity``: rows of ``crossTverskyCountSimilarity``."""
     weights = _check_weights(alpha, beta)
-    return _count_topk(weights, fingerprint_group_one, fingerprint_group_two, k, stream)
+    return _topk(weights, fingerprint_group_one, fingerprint_group_two, k, stream, counts=True)
 
 
 def thresholdTanimotoCountSimilarity(fingerprint_group_one, fingerprint_group_two=None, *, threshold, stream=None):
@@ -424,16 +378,16 @@ def thresholdTanimotoCountSimilarity(fingerprint_group_one, fingerprint_group_tw
     ``[Q + 1]``, int32 and fp64 ``[nnz]``: row q lists exactly the columns whose ``crossTanimotoCountSimilarity`` entry
     is ``>= threshold``, ascending, with those values (group two None: group one against itself, self-matches
     included). ``0 < threshold <= 1``. The matrix is never stored. Synchronises ``stream``."""
-    return _count_threshold(TANIMOTO, fingerprint_group_one, fingerprint_group_two, threshold, stream)
+    return _threshold(TANIMOTO, fingerprint_group_one, fingerprint_group_two, threshold, stream, counts=True)
 
 
 def thresholdDiceCountSimilarity(fingerprint_group_one, fingerprint_group_two=None, *, threshold, stream=None):
     """Dice twin of ``thresholdTanimotoCountSimilarity``: entries of ``crossDiceCountSimilarity``."""
-    return _count_threshold(DICE, fingerprint_group_one, fingerprint_group_two, threshold, stream)
+    return _threshold(DICE, fingerprint_group_one, fingerprint_group_two, threshold, stream, counts=True)
 
 
 def thresholdTverskyCountSimilarity(fingerprint_group_one, fingerprint_group_two=None, *, alpha, beta, threshold,
                                     stream=None):
     """Tversky twin of ``thresholdTanimotoCountSimilarity``: entries of ``crossTverskyCountSimilarity``."""
     weights = _check_weights(alpha, beta)
-    return _count_threshold(weights, fingerprint_group_one, fingerprint_group_two, threshold, stream)
+    return _threshold(weights, fingerprint_group_one, fingerprint_group_two, threshold, stream, counts=True)

@@ -115,6 +115,14 @@ def test_weights_are_keyword_only_and_stream_threshold_checks():
             S.thresholdDiceCountSimilarity(x, threshold=t)
 
 
+def test_count_threshold_checks_the_stream_before_the_threshold():
+    """As the bit threshold calls do (test_threshold.py): both arguments bad is a TypeError."""
+    with pytest.raises(TypeError):
+        S.thresholdTanimotoCountSimilarity(object(), threshold=float("nan"), stream="not a stream")
+    with pytest.raises(TypeError):
+        S.thresholdTverskyCountSimilarity(object(), alpha=0.5, beta=0.5, threshold=2.0, stream=0)
+
+
 def test_the_library_exports_the_entry_points_and_checks_their_arguments(built_lib):
     L = built_lib
     nnz = C.c_uint64(0)
